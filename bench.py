@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""bench.py -- Instant-NGP lego training throughput on N B200s (BASELINE.json metric: NGP lego iters/s & rays/s).
+"""bench.py -- Instant-NGP lego training throughput on N H100s (BASELINE.json metric: NGP lego iters/s & rays/s).
 
   python bench.py --gpus N --steps K --warmup W            our arm   (torchrun for N>1: one rank per GPU, NCCL)
   python bench.py --impl reference --gpus N --steps K ...  reference arm: the path's CPU implementation (oracle port)
+  python bench.py ... --dump-outputs DIR                   also write what the last timed step computed to DIR/<name>.npy
 
 A step = one full training iteration of projects/ngp/configs/ngp_base.py + fp16 (BASELINE config #2):
 [density-grid update every 16] -> ray gen -> march -> fused hash+MLP forward -> composite + Huber + composite
@@ -43,21 +44,11 @@ def peaks():
         p = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         return p["hbm_gbs"], p["bf16_tflops"], "measured"
     except Exception:
-        return 6650.0, 1590.0, "fallback"
-
-
-def measured_traffic(stage):
-    """DRAM bytes per launch (read + write) of the stage's kernel from the committed ncu --set full capture, or None."""
-    try:
-        k = json.load(open(os.path.join(ROOT, "profiles", "r02_traffic.json")))["kernels"]
-        e = k[{"network_bwd": "network_bwd256_kernel", "network_fwd": "network_fwd_kernel<0>"}[stage]]
-        return e["dram_bytes_read"] + e["dram_bytes_write"]
-    except Exception:
-        return None
+        return 3350.0, 989.0, "H100 SXM data sheet (HBM3, dense BF16)"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled every 20 ms from before the warm-up; samples inside the timed region are kept (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled every 20 ms from before the warm-up; samples inside the timed region are kept."""
     Q = "timestamp,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown," \
         "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
@@ -266,15 +257,18 @@ def run_ours(args):
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     t_host0 = clocks.mark()
     e0.record()
+    loss = None
     for _ in range(args.steps):
         rays += runner.sampler.n_rays_per_batch
-        runner.train_step()
+        loss = runner.train_step()
     runner._table_ready()                 # N>1: the last step's all-gather belongs to the timed region
     e1.record()
     sync()
     t_host1 = clocks.mark()
     if profiling:
         torch.cuda.profiler.stop()
+    if args.dump_outputs and rank == 0:               # after the clock window: the copies to the host are not part of the timed steps
+        dump_outputs(runner, loss, args.dump_outputs)
     ms = torch.tensor([e0.elapsed_time(e1)], device="cuda")
     launches = lib.launch_count - launches0
     if world > 1:
@@ -328,10 +322,8 @@ def run_ours(args):
     algo = dict(ALGO[dom])
     t_dom = stage[dom] * 1e-3
     gbs = n_samples * algo["bytes"] / t_dom / 1e9
-    roofline = {"kernel": dom, "bound": "hbm", "achieved": gbs, "peak": hbm, "unit": "GB/s", "frac": gbs / hbm, "traffic": measured_traffic(dom),
-                "traffic_note": "dram__bytes_read.sum + dram__bytes_write.sum per launch, profiles/r02_traffic.json (gradient atomics resolve in L2, "
-                                "so DRAM traffic is well below the algorithmic bytes)",
-                "peak_source": f"{src} (MEASURED_PEAKS.json hbm_gbs)", "launch_ms": stage[dom], "samples_per_launch": n_samples,
+    roofline = {"kernel": dom, "bound": "hbm", "achieved": gbs, "peak": hbm, "unit": "GB/s", "frac": gbs / hbm,
+                "peak_source": src, "launch_ms": stage[dom], "samples_per_launch": n_samples,
                 "algorithmic_bytes_per_sample": algo["bytes"],
                 "tensor": {"achieved_tflops": n_samples * algo["flops"] / t_dom / 1e12, "peak_tflops": tfl,
                            "frac": n_samples * algo["flops"] / t_dom / 1e12 / tfl},
@@ -347,7 +339,7 @@ def run_ours(args):
                                f"{' (2^18)' if args.target_batch == 1 << 18 else ''}, adaptive ray batch "
                                f"({runner.sampler.n_rays_per_batch} rays/iter/GPU at measurement), pretrain {args.pretrain} steps",
                    "parallelism": f"dp{world}", "target_batch_size": args.target_batch,
-                   "l2": "per-step working set (24 MB table + 171 MB optimizer state + 7 MB samples) exceeds the 126 MB L2; no explicit flush",
+                   "l2": "per-step working set (24 MB table + 171 MB optimizer state + 7 MB samples) exceeds the 50 MB L2; no explicit flush",
                    "step_pipeline": ({"enabled": True, "front_starts_at": runner._pipe["at"], "fronts_prefetched": int(runner._pipe["prefetched"]),
                                       "note": "ray generation + march of step i+1 on a second stream under step i's network kernels / optimizer sweep; "
                                               "every timed step contains one front and one back"}
@@ -363,6 +355,21 @@ def run_ours(args):
         print(json.dumps(out))
     if world > 1:
         dist.destroy_process_group()
+
+
+def dump_outputs(runner, loss, out_dir):
+    """Writes what the timed path hands its caller after the last timed step: that step's loss (Runner.train_step's return value)
+    and the trained parameters, as float32 DIR/<name>.npy.  A parameter of more than 2^20 entries (the hash grid) is sampled at a
+    fixed, seeded set of indices, so the files stay small and two builds can be compared entry for entry."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"loss": loss}
+    arrays.update({f"param.{k}": v for k, v in runner.model.state_dict().items()})
+    for name, t in arrays.items():
+        a = t.detach().float().cpu().numpy().ravel()
+        if a.size > 1 << 20:
+            a = a[np.sort(np.random.default_rng(0).choice(a.size, 1 << 20, replace=False))]
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def stage_times(runner, iters):
@@ -426,8 +433,11 @@ def main():
     ap.add_argument("--target-batch", type=int, default=1 << 18,
                     help="target_batch_size, samples per iteration per GPU (ngp_base.py:75); BASELINE config #5 sweeps 2^16 .. 2^22 (tools/sweep.py)")
     ap.add_argument("--scaling", default="weak", choices=["weak", "strong"],
-                    help="weak: --target-batch samples per iteration PER GPU (the contract's default); strong: --target-batch is the GLOBAL "
+                    help="weak: --target-batch samples per iteration PER GPU (the default); strong: --target-batch is the GLOBAL "
                          "sample budget of an iteration, split evenly over the GPUs")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write the last step's loss and the trained parameters (the hash grid sampled) to DIR/<name>.npy; "
+                         "inputs are seeded and the training step is deterministic, so the same arguments give the same files")
     args = ap.parse_args()
     if args.scaling == "strong":
         args.target_batch_global = args.target_batch

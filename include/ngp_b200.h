@@ -1,5 +1,5 @@
 /*
- * ngp_b200.h -- C ABI of libngp_b200.so: the B200-native (sm_100a) Instant-NGP inner loop behind
+ * ngp_b200.h -- C ABI of libngp_b200.so: the H100-native (sm_90a) Instant-NGP inner loop behind
  * JNeRF's operator boundary.
  *
  * Every entry point is what a `jt.code(...)` body of the reference would call in place of its inline
@@ -13,7 +13,7 @@
  *   - every function returns 0 on success, non-zero on error; ngp_last_error() gives the message
  *     (the reference throws std::runtime_error from host code or leaves launches unchecked);
  *   - dtype: 0 = float32, 1 = float16 (the reference's `grad_t` / `in0_type`).
- * Paths in comments are relative to /root/reference/python/jnerf/:
+ * Paths in comments are relative to python/jnerf/ of the JNeRF reference:
  *   HE = models/position_encoders/hash_encoder, SH = models/position_encoders/sh_encoder,
  *   DGS = models/samplers/density_grid_sampler, OPS = ops/code_ops.
  */
@@ -62,7 +62,7 @@ int ngp_hash_bwd(void* stream, uint32_t n, const float* x, const void* dy, int d
 /* ---- R4  spherical harmonics, degree 4 (SH/op_header/SphericalEncode.h:44-150; SH/sh_encoder.py:26-53) ---- */
 int ngp_sh_fwd(void* stream, uint32_t n, const float* dirs, int dtype, void* out);
 
-/* ---- R7  fully-fused MLP (tcgen05) -------------------------------------------------------------------
+/* ---- R7  fully-fused MLP (wgmma) ---------------------------------------------------------------------
  * Replaces mlp_fused_forward_func / mlp_fused_backward_func + the cuBLAS wgrad chain
  * (OPS/op_header/fully_fused_mlp_header.h:26-60; OPS/fully_fused_mlp.py:58-75,101-143).
  * WIDTH 64, input 32, output padded to 16, ReLU hidden, no output activation, no bias, fp16.
@@ -93,8 +93,11 @@ int ngp_mlp_param_count(uint32_t n_hidden_matmuls);
  * out (n_max,4) fp16 = {rgb, sigma_raw}; enc_save (n_max,32) fp16 (kept for backward) may be NULL. */
 int ngp_network_fwd(void* stream, uint32_t n_max, const uint32_t* n_dev, const float* coords, const void* grid,
                     const void* levels_dev, const void* w_density, const void* w_rgb, void* out, void* enc_save);
-/* Backward of the above: dout (n_max,4) fp16 -> grid_grad (fp16, ACCUMULATED with atomics: caller zeroes),
- * dw_density / dw_rgb (fp32, ACCUMULATED: caller zeroes).  Recomputes the MLP forward from enc_save. */
+/* Backward of the above: dout (n_max,4) fp16 -> grid_grad (fp16, ACCUMULATED: caller zeroes),
+ * dw_density / dw_rgb (fp32, ACCUMULATED: caller zeroes).  Recomputes the MLP forward from enc_save.
+ * Deterministic (the result does not depend on how the GPU schedules the work), except for a call captured in a CUDA graph on a
+ * stream that has not run an uncaptured call with this level table before (that one reduces with order-dependent rounding), and for
+ * the entries of a level table that grew in place past the table the stream saw first. */
 int ngp_network_bwd(void* stream, uint32_t n_max, const uint32_t* n_dev, const float* coords, const void* enc_save,
                     const void* levels_dev, const void* w_density, const void* w_rgb, const void* dout,
                     void* grid_grad, float* dw_density, float* dw_rgb);

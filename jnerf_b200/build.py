@@ -1,4 +1,4 @@
-"""Builds libngp_b200.so (all CUDA kernels + the C ABI of include/ngp_b200.h) in-tree with nvcc for sm_100a.
+"""Builds libngp_b200.so (all CUDA kernels + the C ABI of include/ngp_b200.h) in-tree with nvcc for sm_90a (H100).
 No torch headers are involved: the library's boundary is plain C (pointers and sizes)."""
 import os
 import subprocess
@@ -7,7 +7,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libngp_b200.so")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 EXTRA = os.environ.get("NGP_NVCC_FLAGS", "").split()          # extra nvcc flags for experiments
 COMMON = EXTRA + ["-O3", "-std=c++17", "-lineinfo", "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC", "-I", os.path.join(HERE, "..", "include")]
 # per-file extra flags: the sampler / grid code must not contract multiply-adds on its own (bit-exact sample indices)

@@ -15,10 +15,10 @@ void ngp_set_error(const std::string& msg) { g_err = msg; }
 int ngp_num_sms() {
     static int sms[64] = {0};                                     // per device: a process may drive several GPUs
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
     if (sms[dev] == 0) {
         int n = 0;
-        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) return 148;
+        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) return 132;
         sms[dev] = n;
     }
     return sms[dev];

@@ -1,7 +1,7 @@
 // Link-level compatibility with the one native boundary the reference already has (SURVEY.md 8b): the two C++ functions of the
 // prebuilt tiny-cuda-nn object `OPS/op_header/fully_fused_mlp_function.o`, declared in OPS/op_header/fully_fused_mlp_header.h:26-60
 // and called from the jt.code bodies of OPS/fully_fused_mlp.py:58-75 (forward) and :101-115 (backward).  That object carries
-// sm_75/80/86 SASS only and cannot load on a B200; exporting the same two MANGLED symbols from libngp_b200.so lets
+// sm_75/80/86 SASS only and cannot load on an H100; exporting the same two MANGLED symbols from libngp_b200.so lets
 // fully_fused_mlp.py link unchanged (`-Xlinker <path to libngp_b200.so>` in place of the .o, INTEGRATION.md section 3).
 //
 // Contract taken from the call sites (the object has no source in the reference tree):

@@ -1,11 +1,11 @@
 // NGPNetworks.execute / .density and their backward as ONE kernel each (models/networks/ngp_network.py:77-89):
 //   hash-grid gather (R2) -> density MLP 32->64->16 -> SH(dir) (R4) -> colour MLP 32->64->64->16 (R7) -> (N,4)
-// Encoded features, SH features and all hidden activations stay in shared memory / TMEM; HBM sees only the
+// Encoded features, SH features and all hidden activations stay in shared memory / registers; HBM sees only the
 // 28 B coordinate, the 8 B output and (training) a 64 B encoded-feature row kept for backward.
 //
 // Backward reloads the 64 B encoded row, recomputes the MLP forward on the tensor cores (cheaper than storing
-// 448 B of hidden activations per sample), runs the dgrad chain, accumulates all five weight gradients in TMEM
-// across the CTA's tiles, and scatters dL/d(enc) into the hash-grid gradient with f16x2 reductions (R3) without
+// 448 B of hidden activations per sample), runs the dgrad chain, accumulates all five weight gradients in registers
+// across the CTA's tiles, and scatters dL/d(enc) into the hash-grid gradient (R3) without
 // ever materialising dL/d(enc) in HBM.
 //
 // Roofline (DESIGN.md): forward is bound by the gather (524 B algorithmic per sample, L2-resident table);
@@ -13,6 +13,8 @@
 #include "mlp_tc.cuh"
 #include <cstdlib>
 #include <cstdio>
+#include <mutex>
+#include <vector>
 
 int* ngp_err_flag();
 
@@ -22,6 +24,7 @@ using namespace mlp;
 // flat weight offsets (halfs) inside the two parameter vectors (OPS/fully_fused_mlp.py:26-40)
 constexpr int WD_W0 = 0, WD_WOUT = 64 * 32, WD_N = 64 * 32 + 16 * 64;
 constexpr int WR_W0 = 0, WR_W1 = 64 * 32, WR_WOUT = 64 * 32 + 64 * 64, WR_N = 64 * 32 + 64 * 64 + 16 * 64;
+constexpr int W_PART = WD_N + WR_N;   // one CTA's weight-gradient sums: [dwd | dwr]
 
 // ---- shared-memory maps -------------------------------------------------------------------------------
 // activation slab groups
@@ -36,8 +39,7 @@ struct SmemFwd {
     static constexpr uint32_t w1r = w0r + 64 * 32 * 2;
     static constexpr uint32_t woutr = w1r + 64 * 64 * 2;
     static constexpr uint32_t levels = woutr + 16 * 64 * 2;
-    static constexpr uint32_t bar = levels + N_LEVELS * 32;
-    static constexpr uint32_t total = bar + 64;
+    static constexpr uint32_t total = levels + N_LEVELS * 32;
 };
 template <class S>
 __device__ __forceinline__ void stage_all_weights(uint8_t* smem, const __half* wd, const __half* wr, uint32_t t) {
@@ -89,49 +91,46 @@ __device__ __forceinline__ void gather_tile(const float* __restrict__ s_pos /* s
     }
 }
 
-// Forward chain up to (and including) the colour net's last hidden layer.  Expects enc in ACT[G_ENC..+4).
-// Returns the fp16 density output h[0] of row t (sigma_raw) and leaves hd / rin / h1 / h2 in the slab.
-template <class S, uint32_t G_H2, bool CHAIN128 = false>
-__device__ __forceinline__ uint32_t forward_chain(uint8_t* smem, uint32_t g_enc /* G_ENC or G_ENC1 */,
-                                                  const float* s_coords, uint32_t tbase, Pipe& pipe, uint32_t t, uint32_t warp,
-                                                  bool density_only, uint32_t chain_bar = 1) {
+// Forward chain of one warpgroup up to (and including) the colour net's last hidden layer.  Expects enc in ACT[G_ENC..+4) and,
+// unless density_only, the SH features of the tile in ACT[G_RIN+2..+4).  Stores the fp16 density output h[0] of the thread's four
+// fragment rows (64m + frag_row + 8h) in sig[2m + h] and leaves hd / rin / h1 / h2 in the slab.  bar_id: named barrier of the 128
+// chain threads (0 = __syncthreads).
+template <class S, uint32_t G_H2>
+__device__ __forceinline__ void forward_chain(uint8_t* smem, uint32_t g_enc /* G_ENC or G_ENC1 */, uint32_t tw, bool density_only,
+                                              uint32_t bar_id, uint16_t (&sig)[4]) {
     uint8_t* act = smem + S::act;
     const uint32_t smem_s = smem_u32(smem), act_s = smem_s + S::act;
-    const uint32_t D_H = 0, D_S = 64;
     // density L0: enc(32) -> hd(64)
-    if (warp == 0) { if (elect_one()) { issue_fwd<32, 64>(tbase + D_H, act_s, g_enc, smem_s + S::w0d); pipe.commit(); } __syncwarp(); }
-    pipe.wait();
-    epi_hidden_relu(tbase, D_H, warp, act, G_HD, t, nullptr);
-    if constexpr (CHAIN128) sync_chain(chain_bar); else sync_before_issue<false>();
-    // density L1: hd(64) -> h(16)
-    if (warp == 0) { if (elect_one()) { issue_fwd<64, 16>(tbase + D_S, act_s, G_HD, smem_s + S::woutd); pipe.commit(); } __syncwarp(); }
-    pipe.wait();
-    uint32_t sigma_half;
-    {
-        float v[16];
-        tmem_ld16(tmem_addr(tbase, warp, D_S), v);
-        uint4 lo, hi;
-        pack16(v, lo, hi);
-        sigma_half = lo.x & 0xFFFFu;
-        if (density_only) return sigma_half;
-        slab_store16(act, G_RIN, t, lo, hi);
-        float sh[16];
-        sh4(s_coords[t * 7 + 4], s_coords[t * 7 + 5], s_coords[t * 7 + 6], sh);
-        pack16(sh, lo, hi);
-        slab_store16(act, G_RIN + 2, t, lo, hi);
-    }
-    if constexpr (CHAIN128) sync_chain(chain_bar); else sync_before_issue<false>();
+    layer<64>([&](float (&d)[32], uint32_t m) { mma_fwd<32, 64>(d, act_s, g_enc, smem_s + S::w0d, m); },
+              [&](const float (&d)[32], uint32_t m) { frag_to_slab<64, true>(d, act, G_HD, m, tw); });
+    operands_ready(bar_id, 128);
+    // density L1: hd(64) -> h(16) = the first 16 colour-net inputs
+    layer<16>([&](float (&d)[8], uint32_t m) { mma_fwd<64, 16>(d, act_s, G_HD, smem_s + S::woutd, m); },
+              [&](const float (&d)[8], uint32_t m) {
+                  sig[2 * m] = (uint16_t)(pack_half2(d[0], d[1]) & 0xFFFFu);
+                  sig[2 * m + 1] = (uint16_t)(pack_half2(d[2], d[3]) & 0xFFFFu);
+                  if (!density_only) frag_to_slab<16, false>(d, act, G_RIN, m, tw);
+              });
+    if (density_only) return;
+    operands_ready(bar_id, 128);
     // colour L0: [h | sh](32) -> h1(64)
-    if (warp == 0) { if (elect_one()) { issue_fwd<32, 64>(tbase + D_H, act_s, G_RIN, smem_s + S::w0r); pipe.commit(); } __syncwarp(); }
-    pipe.wait();
-    epi_hidden_relu(tbase, D_H, warp, act, G_H1, t, nullptr);
-    if constexpr (CHAIN128) sync_chain(chain_bar); else sync_before_issue<false>();
+    layer<64>([&](float (&d)[32], uint32_t m) { mma_fwd<32, 64>(d, act_s, G_RIN, smem_s + S::w0r, m); },
+              [&](const float (&d)[32], uint32_t m) { frag_to_slab<64, true>(d, act, G_H1, m, tw); });
+    operands_ready(bar_id, 128);
     // colour L1: h1(64) -> h2(64)
-    if (warp == 0) { if (elect_one()) { issue_fwd<64, 64>(tbase + D_H, act_s, G_H1, smem_s + S::w1r); pipe.commit(); } __syncwarp(); }
-    pipe.wait();
-    epi_hidden_relu(tbase, D_H, warp, act, G_H2, t, nullptr);
-    if constexpr (CHAIN128) sync_chain(chain_bar); else sync_before_issue<false>();
-    return sigma_half;
+    layer<64>([&](float (&d)[32], uint32_t m) { mma_fwd<64, 64>(d, act_s, G_H1, smem_s + S::w1r, m); },
+              [&](const float (&d)[32], uint32_t m) { frag_to_slab<64, true>(d, act, G_H2, m, tw); });
+    operands_ready(bar_id, 128);
+}
+// SH(dir) of row t -> ACT[G_RIN+2..+4), the last 16 colour-net inputs
+__device__ __forceinline__ void sh_to_slab(uint8_t* act, const float* s_coords, uint32_t t) {
+    float sh[16];
+    sh4(s_coords[t * 7 + 4], s_coords[t * 7 + 5], s_coords[t * 7 + 6], sh);
+    uint32_t p[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) p[i] = pack_half2(sh[2 * i], sh[2 * i + 1]);
+    *reinterpret_cast<uint4*>(act + (G_RIN + 2) * GB + t * 16) = make_uint4(p[0], p[1], p[2], p[3]);
+    *reinterpret_cast<uint4*>(act + (G_RIN + 3) * GB + t * 16) = make_uint4(p[4], p[5], p[6], p[7]);
 }
 
 // Warp-specialised forward: warps 4-7 ("gather") stage the coordinates of tile i+1 and encode them into one of two enc slabs while
@@ -144,11 +143,10 @@ constexpr int FWD_GW = 8;
 constexpr int FWD_THREADS = 128 + 32 * FWD_GW;
 
 template <bool DENSITY_ONLY>
-__global__ void __launch_bounds__(FWD_THREADS, 2)   // two CTAs per SM (128 TMEM columns each): <= 85 registers per thread
+__global__ void __launch_bounds__(FWD_THREADS, 2)   // two CTAs per SM: <= 85 registers per thread
 network_fwd_kernel(uint32_t n_max, const uint32_t* __restrict__ n_dev, const float* __restrict__ coords, const __half* __restrict__ grid,
                    const NgpLevel* __restrict__ levels, const __half* __restrict__ wd, const __half* __restrict__ wr,
-                   __half* __restrict__ out, __half* __restrict__ enc_save, int* __restrict__ err,
-                   const __grid_constant__ NgpTensorMap enc_map, uint32_t enc_tma) {
+                   __half* __restrict__ out, __half* __restrict__ enc_save, const __grid_constant__ NgpTensorMap enc_map, uint32_t enc_tma) {
     // enc_tma: the encoded-feature rows kept for the backward pass leave the SM as four TMA tensor stores per tile, straight from the
     // slab the gather warps fill (one 8-column x 128-row box per feature group), instead of 16 four-byte global stores per row from the
     // gather warps -- which are the LSU-bound side of this kernel.  enc_save is then only the base address the tensor map was built for.
@@ -156,9 +154,7 @@ network_fwd_kernel(uint32_t n_max, const uint32_t* __restrict__ n_dev, const flo
     using S = SmemFwd;
     constexpr int CS = DENSITY_ONLY ? 3 : 7;
     const uint32_t t = threadIdx.x, warp = t >> 5;
-    const bool is_chain = warp < 4;
-    uint64_t* bar = reinterpret_cast<uint64_t*>(smem + S::bar);
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bar + 1);
+    const bool is_chain = warp < 4;                                     // warps 0-3: the warpgroup that runs the MLP chain
     NgpLevel* s_lv = reinterpret_cast<NgpLevel*>(smem + S::levels);
 
     stage_weights(smem + S::w0d, wd + WD_W0, 64, 32, t, FWD_THREADS);
@@ -169,54 +165,62 @@ network_fwd_kernel(uint32_t n_max, const uint32_t* __restrict__ n_dev, const flo
         stage_weights(smem + S::woutr, wr + WR_WOUT, 16, 64, t, FWD_THREADS);
     }
     if (t < N_LEVELS) s_lv[t] = levels[t];
-    if (t == 0) { mbar_init(bar, 1); fence_mbar_init(); }
-    if (warp == 0) tmem_alloc(tmem_ptr, 128);
-    sync_before_issue();
-    const uint32_t tbase = *tmem_ptr;
+    operands_ready(0, FWD_THREADS);
     const uint32_t n_live = n_dev ? min(*n_dev, n_max) : n_max;
     const uint32_t ntiles = (n_live + ROWS - 1) / ROWS;
 
     if (is_chain) {
-        Pipe pipe{bar, 0, err};
+        uint8_t* act = smem + S::act;
+        const uint32_t smem_s = smem_u32(smem), r0 = frag_row(t);
         uint32_t it = 0;
         for (uint32_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-            const uint32_t buf = it & 1, row = tile * ROWS + t;
+            const uint32_t buf = it & 1;
             const float* s_coords = reinterpret_cast<const float*>(smem + S::coords + buf * 3584);
             named_bar_sync(2 + buf, FWD_THREADS);                       // FULL[buf]: enc slab + coordinates of this tile are in smem
-            tc_fence_after();
             if (!DENSITY_ONLY && enc_tma && warp == 0) {                 // the gather threads fenced their slab writes for the async proxy
                 if (elect_one()) {
 #pragma unroll
                     for (uint32_t g4 = 0; g4 < 4; ++g4)
-                        tma_store_2d(&enc_map, 8 * g4, tile * ROWS, smem_u32(smem) + S::act + ((buf ? G_ENC1 : G_ENC) + g4) * GB);
+                        tma_store_2d(&enc_map, 8 * g4, tile * ROWS, smem_s + S::act + ((buf ? G_ENC1 : G_ENC) + g4) * GB);
                     tma_store_commit();
                 }
                 __syncwarp();
             }
-            // forward_chain releases nothing itself: the enc slab is dead after layer 0, the coordinates after the SH epilogue;
+            if (!DENSITY_ONLY) sh_to_slab(act, s_coords, t);            // read by colour L0, after the chain's first barrier
+            // forward_chain releases nothing itself: the enc slab is dead after layer 0, the coordinates after the SH features;
             // both are handed back together right after the chain (the gather runs a full tile ahead, so this is not on its path)
-            const uint32_t sig = forward_chain<S, G_H2F, true>(smem, buf ? G_ENC1 : G_ENC, s_coords, tbase, pipe, t, warp, DENSITY_ONLY);
+            uint16_t sig[4];
+            forward_chain<S, G_H2F>(smem, buf ? G_ENC1 : G_ENC, t, DENSITY_ONLY, 1, sig);
             if (!DENSITY_ONLY && enc_tma && warp == 0) {                 // the tensor stores have read the slab before it is handed back
                 if (elect_one()) tma_store_wait_read();
                 __syncwarp();
             }
             if (tile + 2 * gridDim.x < ntiles) named_bar_arrive(4 + buf, FWD_THREADS);   // EMPTY[buf]
             if constexpr (DENSITY_ONLY) {
-                if (row < n_live) reinterpret_cast<uint16_t*>(out)[row] = (uint16_t)sig;
-                sync_before_issue<true>();                      // TMEM reads of this tile precede the next tile's MMAs
-            } else {
-                if (warp == 0) { if (elect_one()) { issue_fwd<64, 16>(tbase + 64, smem_u32(smem) + S::act, G_H2F, smem_u32(smem) + S::woutr); pipe.commit(); } __syncwarp(); }
-                pipe.wait();
-                float v[16];
-                tmem_ld16(tmem_addr(tbase, warp, 64), v);
-                if (row < n_live) {
-                    uint2 o;
-                    o.x = pack_half2(v[0], v[1]);
-                    o.y = (pack_half2(v[2], 0.f) & 0xFFFFu) | (sig << 16);
-                    reinterpret_cast<uint2*>(out)[row] = o;
+                if ((t & 3u) == 0) {
+#pragma unroll
+                    for (uint32_t i = 0; i < 4; ++i) {
+                        const uint32_t row = tile * ROWS + 64 * (i >> 1) + r0 + 8 * (i & 1);
+                        if (row < n_live) reinterpret_cast<uint16_t*>(out)[row] = sig[i];
+                    }
                 }
-                sync_before_issue<true>();
+            } else {
+                layer<16>([&](float (&d)[8], uint32_t m) { mma_fwd<64, 16>(d, smem_s + S::act, G_H2F, smem_s + S::woutr, m); },
+                          [&](const float (&d)[8], uint32_t m) {
+#pragma unroll
+                              for (uint32_t h = 0; h < 2; ++h) {
+                                  const float c2 = __shfl_down_sync(0xffffffffu, d[2 * h], 1);   // column 2 sits in the next lane
+                                  const uint32_t row = tile * ROWS + 64 * m + r0 + 8 * h;
+                                  if ((t & 3u) == 0 && row < n_live) {
+                                      uint2 o;
+                                      o.x = pack_half2(d[2 * h], d[2 * h + 1]);
+                                      o.y = (pack_half2(c2, 0.f) & 0xFFFFu) | ((uint32_t)sig[2 * m + h] << 16);
+                                      reinterpret_cast<uint2*>(out)[row] = o;
+                                  }
+                              }
+                          });
             }
+            named_bar_sync(1, 128);                                      // this tile's wgmmas are done before the next tile's stores
         }
     } else {
         const uint32_t tg = t - 128, level = tg & 15, sub = tg >> 4;
@@ -232,7 +236,7 @@ network_fwd_kernel(uint32_t n_max, const uint32_t* __restrict__ n_dev, const flo
             named_bar_sync(6, 32 * FWD_GW);
             gather_tile<CS, 64 / FWD_GW>(s_coords, lv, g, smem + S::act, buf ? G_ENC1 : G_ENC, level, sub, (DENSITY_ONLY || enc_tma) ? nullptr : enc_save, row0,
                                          n_live);
-            fence_proxy_async_smem();                           // the enc slab is read by the tensor core (async proxy)
+            fence_proxy_async_smem();                           // the enc slab is read by the tensor core and the TMA (async proxy)
             named_bar_arrive(2 + buf, FWD_THREADS);                     // FULL[buf]
         }
     }
@@ -240,29 +244,28 @@ network_fwd_kernel(uint32_t n_max, const uint32_t* __restrict__ n_dev, const flo
         if (elect_one()) tma_store_wait_all();
         __syncwarp();
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_free(tbase, 128);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
 // Backward over 256 rows per stage (network_bwd256_kernel).
 //
-// The MLP chain is a strictly serial sequence of 10 stages per tile -- MMA -> commit -> TMEM load -> convert -> shared store ->
-// barrier, ~1.5 k cycles each of which the tensor pipe works 130 -- so the fixed latency of a stage is amortised over TWO 128-row
-// tiles that move through the chain in lock step: a dedicated issuer warp queues the MMAs of tile A and tile B back to back on one
-// commit, the eight epilogue warps (0-3: rows of tile A, 4-7: rows of tile B; two warps per scheduler hide each other's latencies)
-// drain both accumulators at once, and the weight gradients of both tiles accumulate into the same TMEM columns.  Two independent
-// chains per CTA with in-place gradient slabs did NOT pay (every stage's weight-gradient MMAs sat on the critical path: 112 us against
-// 106 us for one chain of 128 rows, profiles/r02_call8; this kernel: 101 us, profiles/r02_call9).  Here gradients rotate through
-// buffers that died one stage earlier instead:
+// The MLP chain is a strictly serial sequence of 10 stages per tile -- wgmma -> wait -> convert -> shared store -> barrier -- so two
+// 128-row tiles move through the chain in lock step, one per warpgroup (warps 0-3: tile A, warps 4-7: tile B), and the weight
+// gradients of both tiles accumulate into the same registers: each weight gradient is owned by one warpgroup, which contracts over
+// the rows of both tiles (tile A's warpgroup: Woutr, W1r; tile B's: W0r, Woutd, W0d -- 40 accumulator registers each).  A barrier of
+// the 256 chain threads ends every stage, so a weight-gradient wgmma of stage s may read the other tile's slabs written in stage s-1.
+// Gradients rotate through buffers that died one stage earlier:
 //     g_h2 -> GX (the one extra slab), g_h1 -> the h2 slab, dYd -> the dYr slab, g_hd -> the h1 slab,
-// whose last reader (a weight-gradient MMA) was queued before the dgrad MMA the writing epilogue waits for.
-// Warps: 0-7 epilogue, 8 MMA issuer, 9-14 hash-grid scatter of the previous pair of tiles.
+// whose last reader (a weight-gradient wgmma) completed before the stage barrier the writing warpgroup passed.
+// Warps: 0-7 MLP chain, 8-13 hash-grid scatter of the previous pair of tiles.
+//
+// Both gradient sums are independent of scheduling, so that a training run is reproducible: each CTA stores its weight-gradient sums
+// in its own slot (layout [dwd | dwr]) and wgrad_reduce_kernel adds the slots in CTA order; the scatter adds into a 64-bit fixed-point
+// copy of the hash-grid gradient (integer sums do not depend on their order) that grid_grad_flush_kernel rounds once into the fp16
+// gradient and clears again.  Without that scratch (see ngp_network_bwd) the kernel reduces straight into the outputs instead, with
+// fp32 / f16x2 reductions whose rounding depends on their order.
 constexpr uint32_t B3_G_GX = 32, B3_G_DY = 40, B3_G_DENC = 42, B3_GROUPS = 46;   // slab groups of one tile after the 32 activation groups
-// 8 epilogue + 1 issuer + 6 scatter = 15 warps: registers are allocated for warps in groups of four, so 16 warps x 128 registers
-// is what fits (17 warps -- four scatter warps per tile -- would be charged as 20)
-constexpr uint32_t B3_EPI_THREADS = 256, B3_SCATTER_WARPS = 6, B3_THREADS = 256 + 32 + 32 * B3_SCATTER_WARPS;
+constexpr uint32_t B3_EPI_THREADS = 256, B3_SCATTER_WARPS = 6, B3_THREADS = B3_EPI_THREADS + 32 * B3_SCATTER_WARPS;
 constexpr uint32_t B3_RUN = (2 * 128 * 16 + 32 * B3_SCATTER_WARPS - 1) / (32 * B3_SCATTER_WARPS);   // consecutive rows per scatter thread (22)
 struct SmemBwd3 {
     static constexpr uint32_t coords = 0;                           // [tile][buf] 128 x 7 f32 (3584 B each)
@@ -274,24 +277,186 @@ struct SmemBwd3 {
     static constexpr uint32_t w1r = w0r + 64 * 32 * 2;
     static constexpr uint32_t woutr = w1r + 64 * 64 * 2;
     static constexpr uint32_t levels = woutr + 16 * 64 * 2;
-    static constexpr uint32_t bar = levels + N_LEVELS * 32;         // 2 mbarriers, then the TMEM base word
-    static constexpr uint32_t total = bar + 64;
+    static constexpr uint32_t dsig = levels + N_LEVELS * 32;        // [tile][128] fp16 dL/dsigma
+    static constexpr uint32_t bar = dsig + 2 * ROWS * 2;            // [tile] mbarrier of the encoded-feature TMA loads
+    static constexpr uint32_t total = bar + 16;
 };
 static_assert(SmemBwd3::total <= 227 * 1024, "backward CTA does not fit");
-constexpr uint32_t B3_READY = 1, B3_FULL = 2, B3_EMPTY = 3;         // named barriers
+constexpr uint32_t B3_STAGE = 1, B3_FULL = 2, B3_EMPTY = 3;         // named barriers (4 + T: the 128 threads of tile T)
+
+// Fixed-point hash-grid gradient: feature f of entry e is the signed 64-bit integer fx[2e + f] in units of 2^-32.  The unit is below
+// the smallest fp16 spacing (2^-24), so every contribution keeps more precision than an fp16 reduction gives it, and a sum cannot wrap
+// while it is within the fp16 range: a contribution is clamped to +-65504 first, and 2^31 units of 1 are 2^31 / 65504 > 32 000 of them.
+constexpr float FX_SCALE = 4294967296.0f, FX_INV = 1.0f / 4294967296.0f;
+__device__ __forceinline__ void red_add_fx(unsigned long long* p, float v) {
+    const long long q = __float2ll_rn(fminf(fmaxf(v, -65504.f), 65504.f) * FX_SCALE);
+    if (q) asm volatile("red.global.add.u64 [%0], %1;" ::"l"(__cvta_generic_to_global(p)), "l"((unsigned long long)q) : "memory");
+}
+// entry idx of a level: into the fixed-point copy if the scratch holds it, straight into the fp16 gradient otherwise
+__device__ __forceinline__ void red_add_entry(unsigned long long* fx, uint32_t fx_live, __half2* gg, uint32_t idx, float2 v) {
+    if (idx < fx_live) { red_add_fx(fx + 2 * (size_t)idx, v.x); red_add_fx(fx + 2 * (size_t)idx + 1, v.y); }
+    else red_add_h2(gg + idx, v.x, v.y);
+}
+
+// The MLP chain of tile T (one warpgroup) over all pairs of the CTA, then the flush of the weight gradients it owns.
+template <uint32_t T>
+__device__ __forceinline__ void bwd_chain(uint8_t* smem, uint32_t tid, uint32_t n_live, uint32_t npairs, const float* __restrict__ coords,
+                                          const __half* __restrict__ enc_save, const __half* __restrict__ dout, float* __restrict__ w_part,
+                                          float* __restrict__ dwd, float* __restrict__ dwr, int* __restrict__ err, uint32_t dbg, const NgpTensorMap* enc_map, uint32_t enc_tma) {
+    using S = SmemBwd3;
+    const uint32_t t = tid & 127, tq = (tid >> 5) & 3, r0 = frag_row(t);
+    uint8_t* act = smem + S::tile0 + T * S::tile_stride;                // this tile's slabs
+    const uint32_t smem_s = smem_u32(smem), a0 = smem_s + S::tile0, a1 = a0 + S::tile_stride, a_s = T ? a1 : a0;
+    __half* s_dsig = reinterpret_cast<__half*>(smem + S::dsig) + T * ROWS;
+    uint64_t* bar_t = reinterpret_cast<uint64_t*>(smem + S::bar) + T;
+    const bool wg = !(dbg & 4);
+    // zero-initialised: a CTA without a pair of tiles still stores its (empty) sums
+    float acc_woutr[8] = {}, acc_w1r[32] = {};              // tile A's warpgroup: [64 in][16 out], [64 out][64 in]
+    float acc_w0r[16] = {}, acc_woutd[8] = {}, acc_w0d[16] = {};   // tile B's warpgroup: [64 out][32 in], [64 in][16 out], [64 out][32 in]
+    auto stage = [&]() { operands_ready(B3_STAGE, B3_EPI_THREADS); };
+    float pf_c[7];
+    uint4 pf_e[4];
+    uint2 pf_d;
+    auto prefetch = [&](uint32_t pair) {
+        const uint32_t tile_ = 2 * pair + T, rr0 = tile_ * ROWS, r = rr0 + t;
+        const bool ok = r < n_live;
+#pragma unroll
+        for (int j = 0; j < 7; ++j) {
+            const uint32_t i = t + 128 * j;
+            pf_c[j] = (rr0 + i / 7 < n_live) ? __ldg(coords + (size_t)rr0 * 7 + i) : 0.f;
+        }
+        if (!enc_tma) {
+            const uint4* es = reinterpret_cast<const uint4*>(enc_save + (size_t)r * 32);
+#pragma unroll
+            for (int g = 0; g < 4; ++g) pf_e[g] = ok ? __ldg(es + g) : make_uint4(0, 0, 0, 0);
+        }
+        pf_d = ok ? __ldg(reinterpret_cast<const uint2*>(dout) + r) : make_uint2(0, 0);
+    };
+    if (blockIdx.x < npairs) prefetch(blockIdx.x);
+    uint32_t it = 0, acc = 0;   // acc = 0 on the CTA's first pair: the weight-gradient accumulators are overwritten
+    for (uint32_t pair = blockIdx.x; pair < npairs; pair += gridDim.x, ++it, acc = 1) {
+        const uint32_t buf = it & 1;
+        float* s_coords = reinterpret_cast<float*>(smem + S::coords + (2 * T + buf) * 3584);
+        if (it >= 1) named_bar_sync(B3_STAGE, B3_EPI_THREADS);         // both warpgroups' wgmmas of the previous pair have read their slabs
+#pragma unroll
+        for (int j = 0; j < 7; ++j) s_coords[t + 128 * j] = pf_c[j];
+        if (enc_tma) {
+            // encoded-feature rows of this tile: four tensor loads (8-column x 128-row boxes = the four slab groups) by one thread
+            if (tq == 0) {
+                if (elect_one()) {
+                    mbar_expect_tx(bar_t, ROWS * 64);
+#pragma unroll
+                    for (uint32_t g4 = 0; g4 < 4; ++g4)
+                        tma_load_2d(smem_u32(act) + (G_ENC + g4) * GB, enc_map, 8 * g4, (2 * pair + T) * ROWS, bar_t);
+                }
+                __syncwarp();
+            }
+        } else {
+#pragma unroll
+            for (int g = 0; g < 4; ++g) *reinterpret_cast<uint4*>(act + (G_ENC + g) * GB + t * 16) = pf_e[g];
+        }
+        s_dsig[t] = __ushort_as_half((unsigned short)(pf_d.y >> 16));
+        *reinterpret_cast<uint4*>(act + B3_G_DY * GB + t * 16) = make_uint4(pf_d.x, pf_d.y & 0xFFFFu, 0, 0);   // dYr: 3 colour gradients, K padded to 16
+        *reinterpret_cast<uint4*>(act + (B3_G_DY + 1) * GB + t * 16) = make_uint4(0, 0, 0, 0);
+        if (pair + gridDim.x < npairs) prefetch(pair + gridDim.x);     // in flight during the whole chain
+        if (enc_tma) {
+            if (!mbar_wait(bar_t, it & 1)) atomicExch(err, 4);
+            if ((2 * pair + T) * ROWS + t >= n_live) {                  // rows past the live samples hold whatever an earlier step left: zero them
+#pragma unroll
+                for (int g = 0; g < 4; ++g) *reinterpret_cast<uint4*>(act + (G_ENC + g) * GB + t * 16) = make_uint4(0, 0, 0, 0);
+            }
+        }
+        named_bar_sync(4 + T, 128);                                     // the SH features read other threads' coordinate words
+        sh_to_slab(act, s_coords, t);
+        stage();
+        // F1 density L0: enc -> hd
+        layer<64>([&](float (&d)[32], uint32_t m) { mma_fwd<32, 64>(d, a_s, G_ENC, smem_s + S::w0d, m); },
+                  [&](const float (&d)[32], uint32_t m) { frag_to_slab<64, true>(d, act, G_HD, m, t); });
+        stage();
+        // F2 density L1: hd -> h (16) = the first 16 colour-net inputs
+        layer<16>([&](float (&d)[8], uint32_t m) { mma_fwd<64, 16>(d, a_s, G_HD, smem_s + S::woutd, m); },
+                  [&](const float (&d)[8], uint32_t m) { frag_to_slab<16, false>(d, act, G_RIN, m, t); });
+        stage();
+        // F3 colour L0 -> h1 ; F4 colour L1 -> h2
+        layer<64>([&](float (&d)[32], uint32_t m) { mma_fwd<32, 64>(d, a_s, G_RIN, smem_s + S::w0r, m); },
+                  [&](const float (&d)[32], uint32_t m) { frag_to_slab<64, true>(d, act, G_H1, m, t); });
+        stage();
+        layer<64>([&](float (&d)[32], uint32_t m) { mma_fwd<64, 64>(d, a_s, G_H1, smem_s + S::w1r, m); },
+                  [&](const float (&d)[32], uint32_t m) { frag_to_slab<64, true>(d, act, G_H2B, m, t); });
+        stage();
+        // B1: g_h2 = (dYr Woutr) . relu'(h2) -> GX ; Woutr [in][out] += h2^T dYr
+        if (T == 0 && wg) { wgmma_fence(); mma_wgrad<16>(acc_woutr, a0, G_H2B, a0, B3_G_DY, acc); mma_wgrad<16>(acc_woutr, a1, G_H2B, a1, B3_G_DY, 1); }
+        layer<64>([&](float (&d)[32], uint32_t m) { mma_dgrad<16, 64>(d, a_s, B3_G_DY, smem_s + S::woutr, m); },
+                  [&](const float (&d)[32], uint32_t m) { frag_dgrad_mask<64>(d, act, G_H2B, act, B3_G_GX, m, t); });
+        stage();
+        // B2: g_h1 = (g_h2 W1r) . relu'(h1) -> over h2 ; W1r [out][in] += g_h2^T h1
+        if (T == 0 && wg) { wgmma_fence(); mma_wgrad<64>(acc_w1r, a0, B3_G_GX, a0, G_H1, acc); mma_wgrad<64>(acc_w1r, a1, B3_G_GX, a1, G_H1, 1); }
+        layer<64>([&](float (&d)[32], uint32_t m) { mma_dgrad<64, 64>(d, a_s, B3_G_GX, smem_s + S::w1r, m); },
+                  [&](const float (&d)[32], uint32_t m) { frag_dgrad_mask<64>(d, act, G_H1, act, G_H2B, m, t); });
+        stage();
+        // B3: dYd = (g_h1 W0r)[:, 0..16) + dL/dsigma (ngp_network.py:83) -> over dYr (the other 16 columns of d_rin are dL/dSH, unused) ;
+        //     W0r [out][in] += g_h1^T rin
+        if (T == 1 && wg) { wgmma_fence(); mma_wgrad<32>(acc_w0r, a0, G_H2B, a0, G_RIN, acc); mma_wgrad<32>(acc_w0r, a1, G_H2B, a1, G_RIN, 1); }
+        layer<16>([&](float (&d)[8], uint32_t m) { mma_dgrad<64, 16>(d, a_s, G_H2B, smem_s + S::w0r, m); },
+                  [&](const float (&d)[8], uint32_t m) {
+                      float v[8];
+#pragma unroll
+                      for (int i = 0; i < 8; ++i) v[i] = d[i];
+                      if ((t & 3u) == 0) {                                // column 0 = dL/dsigma of rows r and r + 8
+                          v[0] += __half2float(s_dsig[64 * m + r0]);
+                          v[2] += __half2float(s_dsig[64 * m + r0 + 8]);
+                      }
+                      frag_to_slab<16, false>(v, act, B3_G_DY, m, t);
+                  });
+        stage();
+        // B4: g_hd = (dYd Woutd) . relu'(hd) -> over h1 ; Woutd [in][out] += hd^T dYd
+        if (T == 1 && wg) { wgmma_fence(); mma_wgrad<16>(acc_woutd, a0, G_HD, a0, B3_G_DY, acc); mma_wgrad<16>(acc_woutd, a1, G_HD, a1, B3_G_DY, 1); }
+        layer<64>([&](float (&d)[32], uint32_t m) { mma_dgrad<16, 64>(d, a_s, B3_G_DY, smem_s + S::woutd, m); },
+                  [&](const float (&d)[32], uint32_t m) { frag_dgrad_mask<64>(d, act, G_HD, act, G_H1, m, t); });
+        stage();
+        // B5: d_enc = g_hd W0d -> DENC (the scatter warps read the previous pair's until EMPTY) ; W0d [out][in] += g_hd^T enc
+        if (T == 1 && wg) { wgmma_fence(); mma_wgrad<32>(acc_w0d, a0, G_H1, a0, G_ENC, acc); mma_wgrad<32>(acc_w0d, a1, G_H1, a1, G_ENC, 1); }
+        if (it >= 1) named_bar_sync(B3_EMPTY, B3_EPI_THREADS + 32 * B3_SCATTER_WARPS);
+        layer<32>([&](float (&d)[16], uint32_t m) { mma_dgrad<64, 32>(d, a_s, G_H1, smem_s + S::w0d, m); },
+                  [&](const float (&d)[16], uint32_t m) { frag_to_slab<32, false>(d, act, B3_G_DENC, m, t); });
+        named_bar_arrive(B3_FULL, B3_EPI_THREADS + 32 * B3_SCATTER_WARPS);   // dL/d(enc) and coords of this pair are ready
+    }
+    // the weight-gradient sums this warpgroup owns (colour Wout rows >= 3 stay zero, fully_fused_mlp.py:136): into the CTA's slot,
+    // or without one added straight to the outputs
+    if (!w_part) {
+        if (!it) return;
+        if (T == 0) {
+            frag_red_add<16>(acc_woutr, dwr + WR_WOUT, 1, 64, 64, 3, t);
+            frag_red_add<64>(acc_w1r, dwr + WR_W1, 64, 1, 64, 64, t);
+        } else {
+            frag_red_add<32>(acc_w0r, dwr + WR_W0, 32, 1, 64, 32, t);
+            frag_red_add<16>(acc_woutd, dwd + WD_WOUT, 1, 64, 64, 16, t);
+            frag_red_add<32>(acc_w0d, dwd + WD_W0, 32, 1, 64, 32, t);
+        }
+        return;
+    }
+    dwd = w_part + (size_t)blockIdx.x * W_PART;
+    dwr = dwd + WD_N;
+    if (T == 0) {
+        frag_store<16>(acc_woutr, dwr + WR_WOUT, 1, 64, 3, t);
+        frag_store<64>(acc_w1r, dwr + WR_W1, 64, 1, 64, t);
+    } else {
+        frag_store<32>(acc_w0r, dwr + WR_W0, 32, 1, 32, t);
+        frag_store<16>(acc_woutd, dwd + WD_WOUT, 1, 64, 16, t);
+        frag_store<32>(acc_w0d, dwd + WD_W0, 32, 1, 32, t);
+    }
+}
 
 __global__ void __launch_bounds__(B3_THREADS, 1)
 network_bwd256_kernel(uint32_t n_max, const uint32_t* __restrict__ n_dev, const float* __restrict__ coords, const __half* __restrict__ enc_save,
                       const NgpLevel* __restrict__ levels, const __half* __restrict__ wd, const __half* __restrict__ wr,
                       const __half* __restrict__ dout, __half* __restrict__ grid_grad, float* __restrict__ dwd, float* __restrict__ dwr,
+                      unsigned long long* __restrict__ grid_fx, uint32_t fx_entries, float* __restrict__ w_part,
                       int* __restrict__ err, uint32_t dbg, const __grid_constant__ NgpTensorMap enc_map, uint32_t enc_tma) {
     extern __shared__ __align__(1024) uint8_t smem[];
     using S = SmemBwd3;
     const uint32_t tid = threadIdx.x, warp = tid >> 5;
-    uint64_t* bar_d = reinterpret_cast<uint64_t*>(smem + S::bar);  // the forward / dgrad MMAs of the current stage are done
-    uint64_t* bar_w = bar_d + 1;                                   // all weight-gradient MMAs of the pair of tiles are done
-    uint64_t* bar_t = bar_d + 2;                                   // [2]: the TMA loads of a tile's encoded-feature rows have landed
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bar_d + 4);
+    uint64_t* bar_t = reinterpret_cast<uint64_t*>(smem + S::bar);
     NgpLevel* s_lv = reinterpret_cast<NgpLevel*>(smem + S::levels);
 
     stage_weights(smem + S::w0d, wd + WD_W0, 64, 32, tid, B3_THREADS);
@@ -300,218 +465,25 @@ network_bwd256_kernel(uint32_t n_max, const uint32_t* __restrict__ n_dev, const 
     stage_weights(smem + S::w1r, wr + WR_W1, 64, 64, tid, B3_THREADS);
     stage_weights(smem + S::woutr, wr + WR_WOUT, 16, 64, tid, B3_THREADS);
     if (tid < N_LEVELS) s_lv[tid] = levels[tid];
-    // zero both tiles once: dYr columns 4..15 are never rewritten, and M = 128 weight-gradient operands run past their slab
+    // zero both tiles once: dYr columns 4..15 are never rewritten, and 64-feature weight-gradient operands run past their slab
     for (uint32_t i = tid; i < 2 * S::tile_stride / 16; i += B3_THREADS) *reinterpret_cast<uint4*>(smem + S::tile0 + i * 16) = make_uint4(0, 0, 0, 0);
-    if (tid == 0) { mbar_init(bar_d, 1); mbar_init(bar_w, 1); mbar_init(bar_t, 1); mbar_init(bar_t + 1, 1); fence_mbar_init(); }
-    if (warp == 0) tmem_alloc(tmem_ptr, 512);
-    sync_before_issue();
-    const uint32_t tbase = *tmem_ptr;
+    if (tid == 0) { mbar_init(bar_t, 1); mbar_init(bar_t + 1, 1); fence_mbar_init(); }
+    operands_ready(0, B3_THREADS);
     const uint32_t n_live = n_dev ? min(*n_dev, n_max) : n_max;
     const uint32_t ntiles = (n_live + ROWS - 1) / ROWS, npairs = (ntiles + 1) / 2;
-    // TMEM columns: working accumulators of tile A / tile B, then the five weight-gradient accumulators (both tiles add into them)
-    constexpr uint32_t D_H = 0, D_S = 64, TB = 96 /* tile B's working columns */, A_W0D = 192, A_WOUTD = 256, A_W0R = 272, A_W1R = 336, A_WOUTR = 400;
-    static_assert(A_WOUTR + 16 <= 512, "TMEM columns");
 
-    if (warp < 8) {
-        // ------------------------------------------------------------------ epilogue threads: thread t = row t of tile T
-        const uint32_t T = warp >> 2, t = tid & 127, tq = warp & 3;
-        uint8_t* act = smem + S::tile0 + T * S::tile_stride;       // this tile's slabs
-        const uint32_t tb = tbase + T * TB;
-        uint32_t phase = 0;
-        auto wait_mma = [&]() {
-            if (!mbar_wait(bar_d, phase)) atomicExch(err, 1);
-            phase ^= 1;
-            tc_fence_after();
-        };
-        auto ready = [&]() {                                       // operands written, accumulators read: the issuer may queue the next stage
-            tc_fence_before();
-            fence_proxy_async_smem();
-            named_bar_arrive(B3_READY, B3_EPI_THREADS + 32);
-        };
-        float pf_c[7];
-        uint4 pf_e[4];
-        uint2 pf_d;
-        auto prefetch = [&](uint32_t pair) {
-            const uint32_t tile_ = 2 * pair + T, r0 = tile_ * ROWS, r = r0 + t;
-            const bool ok = r < n_live;
-#pragma unroll
-            for (int j = 0; j < 7; ++j) {
-                const uint32_t i = t + 128 * j;
-                pf_c[j] = (r0 + i / 7 < n_live) ? __ldg(coords + (size_t)r0 * 7 + i) : 0.f;
-            }
-            if (!enc_tma) {
-                const uint4* es = reinterpret_cast<const uint4*>(enc_save + (size_t)r * 32);
-#pragma unroll
-                for (int g = 0; g < 4; ++g) pf_e[g] = ok ? __ldg(es + g) : make_uint4(0, 0, 0, 0);
-            }
-            pf_d = ok ? __ldg(reinterpret_cast<const uint2*>(dout) + r) : make_uint2(0, 0);
-        };
-        if (blockIdx.x < npairs) prefetch(blockIdx.x);
-        uint32_t it = 0;
-        for (uint32_t pair = blockIdx.x; pair < npairs; pair += gridDim.x, ++it) {
-            const uint32_t buf = it & 1;
-            float* s_coords = reinterpret_cast<float*>(smem + S::coords + (2 * T + buf) * 3584);
-            if (it >= 1) { if (!mbar_wait(bar_w, (it - 1) & 1)) atomicExch(err, 2); }   // the previous pair's wgrad MMAs have read their slabs
-#pragma unroll
-            for (int j = 0; j < 7; ++j) s_coords[t + 128 * j] = pf_c[j];
-            if (enc_tma) {
-                // encoded-feature rows of this tile: four tensor loads (8-column x 128-row boxes = the four slab groups) by one thread
-                if (tq == 0) {
-                    if (elect_one()) {
-                        mbar_expect_tx(bar_t + T, ROWS * 64);
-#pragma unroll
-                        for (uint32_t g4 = 0; g4 < 4; ++g4)
-                            tma_load_2d(smem_u32(act) + (G_ENC + g4) * GB, &enc_map, 8 * g4, (2 * pair + T) * ROWS, bar_t + T);
-                    }
-                    __syncwarp();
-                }
-            } else {
-#pragma unroll
-                for (int g = 0; g < 4; ++g) *reinterpret_cast<uint4*>(act + (G_ENC + g) * GB + t * 16) = pf_e[g];
-            }
-            const uint32_t dsig = pf_d.y >> 16;
-            *reinterpret_cast<uint4*>(act + B3_G_DY * GB + t * 16) = make_uint4(pf_d.x, pf_d.y & 0xFFFFu, 0, 0);   // dYr: 3 colour gradients, K padded to 16
-            *reinterpret_cast<uint4*>(act + (B3_G_DY + 1) * GB + t * 16) = make_uint4(0, 0, 0, 0);
-            if (pair + gridDim.x < npairs) prefetch(pair + gridDim.x);     // in flight during the whole chain
-            if (enc_tma) {
-                if (!mbar_wait(bar_t + T, it & 1)) atomicExch(err, 4);
-                if ((2 * pair + T) * ROWS + t >= n_live) {                  // rows past the live samples hold whatever an earlier step left: zero them
-#pragma unroll
-                    for (int g = 0; g < 4; ++g) *reinterpret_cast<uint4*>(act + (G_ENC + g) * GB + t * 16) = make_uint4(0, 0, 0, 0);
-                }
-            }
-            named_bar_sync(4 + T, 128);                                     // the SH epilogue reads other threads' coordinate words
-            ready();
-            // F1 density L0: enc -> hd
-            wait_mma();
-            epi_hidden_relu(tb, D_H, tq, act, G_HD, t, nullptr);
-            ready();
-            // F2 density L1: hd -> h (16), + SH(dir) -> colour-net input
-            wait_mma();
-            {
-                float v[16];
-                tmem_ld16(tmem_addr(tb, tq, D_S), v);
-                uint4 lo, hi;
-                pack16(v, lo, hi);
-                slab_store16(act, G_RIN, t, lo, hi);
-                float sh[16];
-                sh4(s_coords[t * 7 + 4], s_coords[t * 7 + 5], s_coords[t * 7 + 6], sh);
-                pack16(sh, lo, hi);
-                slab_store16(act, G_RIN + 2, t, lo, hi);
-            }
-            ready();
-            // F3 colour L0 -> h1 ; F4 colour L1 -> h2
-            wait_mma();
-            epi_hidden_relu(tb, D_H, tq, act, G_H1, t, nullptr);
-            ready();
-            wait_mma();
-            epi_hidden_relu(tb, D_H, tq, act, G_H2B, t, nullptr);
-            ready();
-            // B1: g_h2 = (dYr Woutr) . relu'(h2) -> GX
-            wait_mma();
-            epi_dgrad_mask(tb, D_H, tq, act, G_H2B, act, B3_G_GX, t, nullptr);
-            ready();
-            // B2: g_h1 = (g_h2 W1r) . relu'(h1) -> over h2 (dead: its last reader, the Woutr weight gradient, was queued before this stage's dgrad)
-            wait_mma();
-            epi_dgrad_mask(tb, D_H, tq, act, G_H1, act, G_H2B, t, nullptr);
-            ready();
-            // B3: d_rin = g_h1 W0r (the last 16 of its 32 columns are dL/dSH, unused) ; dYd = d_rin[0..16) + dL/dsigma -> over dYr
-            wait_mma();
-            {
-                float v[16];
-                tmem_ld16(tmem_addr(tb, tq, D_S), v);
-                v[0] += __half2float(__ushort_as_half((unsigned short)dsig));   // ngp_network.py:83
-                uint4 lo, hi;
-                pack16(v, lo, hi);
-                slab_store16(act, B3_G_DY, t, lo, hi);
-            }
-            ready();
-            // B4: g_hd = (dYd Woutd) . relu'(hd) -> over h1
-            wait_mma();
-            epi_dgrad_mask(tb, D_H, tq, act, G_HD, act, G_H1, t, nullptr);
-            ready();
-            // B5: d_enc = g_hd W0d -> DENC (the scatter warps still read the previous pair's until EMPTY)
-            wait_mma();
-            if (it >= 1) named_bar_sync(B3_EMPTY, B3_EPI_THREADS + 32 * B3_SCATTER_WARPS);
-            {
-                float v[16];
-                uint4 lo, hi;
-                tmem_ld16(tmem_addr(tb, tq, D_S), v);
-                pack16(v, lo, hi);
-                slab_store16(act, B3_G_DENC, t, lo, hi);
-                tmem_ld16(tmem_addr(tb, tq, D_S + 16), v);
-                pack16(v, lo, hi);
-                slab_store16(act, B3_G_DENC + 2, t, lo, hi);
-            }
-            tc_fence_before();
-            named_bar_arrive(B3_FULL, B3_EPI_THREADS + 32 * B3_SCATTER_WARPS);   // dL/d(enc) and coords of this pair are ready
-        }
-        // flush the weight gradients (lane = input feature, column = output feature): rows of tile A's threads
-        if (it && T == 0) {
-            if (!mbar_wait(bar_w, (it - 1) & 1)) atomicExch(err, 2);
-            tc_fence_after();
-            float v[16];
-            const uint32_t f_col[5] = {A_W0D, A_WOUTD, A_W0R, A_W1R, A_WOUTR};
-            const uint32_t f_nout[5] = {64, 16, 64, 64, 16}, f_valid[5] = {64, 16, 64, 64, 3};   // colour Wout rows >= 3 stay zero (fully_fused_mlp.py:136)
-            const uint32_t f_in[5] = {32, 64, 32, 64, 64};
-            float* const f_dst[5] = {dwd + WD_W0, dwd + WD_WOUT, dwr + WR_W0, dwr + WR_W1, dwr + WR_WOUT};
-#pragma unroll 1
-            for (int m = 0; m < 5; ++m) {
-#pragma unroll 1
-                for (uint32_t c = 0; c < f_nout[m] / 16; ++c) {
-                    tmem_ld16(tmem_addr(tbase, tq, f_col[m] + 16 * c), v);
-                    if (t < f_in[m]) {
-#pragma unroll
-                        for (int o = 0; o < 16; ++o)
-                            if (16 * c + o < f_valid[m]) red_add_f32(f_dst[m] + (size_t)(16 * c + o) * f_in[m] + t, v[o]);
-                    }
-                }
-            }
-        }
-    } else if (warp == 8) {
-        // ------------------------------------------------------------------ MMA issuer
-        const uint32_t smem_s = smem_u32(smem), a0 = smem_s + S::tile0, a1 = a0 + S::tile_stride;
-        const uint32_t t0 = tbase, t1 = tbase + TB;
-        uint32_t acc = 0;
-        // one stage: wait until all 256 epilogue threads have written their operands, queue the stage's MMAs for both tiles, commit
-#define B3_STAGE(...)                                                                                  \
-        named_bar_sync(B3_READY, B3_EPI_THREADS + 32);                                                 \
-        tc_fence_after();                                                                              \
-        if (elect_one()) { __VA_ARGS__ }                                                               \
-        __syncwarp();
-        for (uint32_t pair = blockIdx.x; pair < npairs; pair += gridDim.x, acc = 1) {
-            const bool wg = !(dbg & 4);
-            B3_STAGE(issue_fwd<32, 64>(t0 + D_H, a0, G_ENC, smem_s + S::w0d); issue_fwd<32, 64>(t1 + D_H, a1, G_ENC, smem_s + S::w0d); mma_commit(bar_d);)
-            B3_STAGE(issue_fwd<64, 16>(t0 + D_S, a0, G_HD, smem_s + S::woutd); issue_fwd<64, 16>(t1 + D_S, a1, G_HD, smem_s + S::woutd); mma_commit(bar_d);)
-            B3_STAGE(issue_fwd<32, 64>(t0 + D_H, a0, G_RIN, smem_s + S::w0r); issue_fwd<32, 64>(t1 + D_H, a1, G_RIN, smem_s + S::w0r); mma_commit(bar_d);)
-            B3_STAGE(issue_fwd<64, 64>(t0 + D_H, a0, G_H1, smem_s + S::w1r); issue_fwd<64, 64>(t1 + D_H, a1, G_H1, smem_s + S::w1r); mma_commit(bar_d);)
-            // B1: dgrad through Woutr ; wgrad Woutr = h2^T dYr
-            B3_STAGE(issue_dgrad<16, 64>(t0 + D_H, a0, B3_G_DY, smem_s + S::woutr); issue_dgrad<16, 64>(t1 + D_H, a1, B3_G_DY, smem_s + S::woutr); mma_commit(bar_d);
-                     if (wg) { issue_wgrad<16>(tbase + A_WOUTR, a0, G_H2B, a0, B3_G_DY, acc); issue_wgrad<16>(tbase + A_WOUTR, a1, G_H2B, a1, B3_G_DY, 1); })
-            // B2: dgrad through W1r ; wgrad W1r = h1^T g_h2
-            B3_STAGE(issue_dgrad<64, 64>(t0 + D_H, a0, B3_G_GX, smem_s + S::w1r); issue_dgrad<64, 64>(t1 + D_H, a1, B3_G_GX, smem_s + S::w1r); mma_commit(bar_d);
-                     if (wg) { issue_wgrad<64>(tbase + A_W1R, a0, G_H1, a0, B3_G_GX, acc); issue_wgrad<64>(tbase + A_W1R, a1, G_H1, a1, B3_G_GX, 1); })
-            // B3: dgrad through W0r (g_h1 lives in the h2 slab) ; wgrad W0r = rin^T g_h1
-            B3_STAGE(issue_dgrad<64, 32>(t0 + D_S, a0, G_H2B, smem_s + S::w0r); issue_dgrad<64, 32>(t1 + D_S, a1, G_H2B, smem_s + S::w0r); mma_commit(bar_d);
-                     if (wg) { issue_wgrad<64>(tbase + A_W0R, a0, G_RIN, a0, G_H2B, acc); issue_wgrad<64>(tbase + A_W0R, a1, G_RIN, a1, G_H2B, 1); })
-            // B4: dgrad through Woutd (dYd lives in the dYr slab) ; wgrad Woutd = hd^T dYd
-            B3_STAGE(issue_dgrad<16, 64>(t0 + D_H, a0, B3_G_DY, smem_s + S::woutd); issue_dgrad<16, 64>(t1 + D_H, a1, B3_G_DY, smem_s + S::woutd); mma_commit(bar_d);
-                     if (wg) { issue_wgrad<16>(tbase + A_WOUTD, a0, G_HD, a0, B3_G_DY, acc); issue_wgrad<16>(tbase + A_WOUTD, a1, G_HD, a1, B3_G_DY, 1); })
-            // B5: dgrad through W0d (g_hd lives in the h1 slab) ; wgrad W0d = enc^T g_hd ; then everything of this pair is queued
-            B3_STAGE(issue_dgrad<64, 32>(t0 + D_S, a0, G_H1, smem_s + S::w0d); issue_dgrad<64, 32>(t1 + D_S, a1, G_H1, smem_s + S::w0d); mma_commit(bar_d);
-                     if (wg) { issue_wgrad<64>(tbase + A_W0D, a0, G_ENC, a0, G_H1, acc); issue_wgrad<64>(tbase + A_W0D, a1, G_ENC, a1, G_H1, 1); }
-                     mma_commit(bar_w);)
-        }
-#undef B3_STAGE
+    if (warp < 4) {
+        bwd_chain<0>(smem, tid, n_live, npairs, coords, enc_save, dout, w_part, dwd, dwr, err, dbg, &enc_map, enc_tma);
+    } else if (warp < 8) {
+        bwd_chain<1>(smem, tid, n_live, npairs, coords, enc_save, dout, w_part, dwd, dwr, err, dbg, &enc_map, enc_tma);
     } else {
         // ------------------------------------------------------------------ scatter (HashEncode.h:339-347): 192 threads over the pair's 256 rows
         // Thread (level, sub) walks its B3_RUN consecutive samples, accumulates the 8 corner contributions in fp32 registers while the grid
-        // cell stays the same and issues the f16x2 reductions only when the cell changes.  The scatter warps are latency-bound (one
-        // dependent instruction stream per scheduler), not request-bound: measured, 4 warps for both tiles took 100 us against a
-        // 70 us chain, and pairing x-neighbour corners into REDG.F16x4 -- which wins 17 % in the full-occupancy standalone
-        // ngp_hash_bwd -- LOST 33 % here (more instructions on the critical warps).
-        const uint32_t ts = tid - (B3_EPI_THREADS + 32), level = ts & 15, sub = ts >> 4;   // 12 row ranges of B3_RUN rows over the 256 rows of the pair
+        // cell stays the same and issues the reductions only when the cell changes.
+        const uint32_t ts = tid - B3_EPI_THREADS, level = ts & 15, sub = ts >> 4;   // 12 row ranges of B3_RUN rows over the 256 rows of the pair
         const NgpLevel lv = s_lv[level];
+        unsigned long long* fx = grid_fx + 2 * (size_t)lv.offset;
+        const uint32_t fx_live = fx_entries > lv.offset ? fx_entries - lv.offset : 0u;     // entries of this level the scratch holds
         __half2* gg = reinterpret_cast<__half2*>(grid_grad) + lv.offset;
         uint32_t it = 0;
         for (uint32_t pair = blockIdx.x; pair < npairs; pair += gridDim.x, ++it) {
@@ -535,7 +507,7 @@ network_bwd256_kernel(uint32_t n_max, const uint32_t* __restrict__ n_dev, const 
                 if (hc.gx != cgx || hc.gy != cgy || hc.gz != cgz) {
                     if (dirty && !(dbg & 1)) {
 #pragma unroll
-                        for (int c = 0; c < 8; ++c) red_add_h2(gg + idx[c], accv[c].x, accv[c].y);
+                        for (int c = 0; c < 8; ++c) red_add_entry(fx, fx_live, gg, idx[c], accv[c]);
                     }
                     cgx = hc.gx; cgy = hc.gy; cgz = hc.gz;
                     hash_cell_indices(lv, cgx, cgy, cgz, idx);
@@ -550,14 +522,100 @@ network_bwd256_kernel(uint32_t n_max, const uint32_t* __restrict__ n_dev, const 
             }
             if (dirty && !(dbg & 1)) {
 #pragma unroll
-                for (int c = 0; c < 8; ++c) red_add_h2(gg + idx[c], accv[c].x, accv[c].y);
+                for (int c = 0; c < 8; ++c) red_add_entry(fx, fx_live, gg, idx[c], accv[c]);
             }
             if (pair + gridDim.x < npairs) named_bar_arrive(B3_EMPTY, B3_EPI_THREADS + 32 * B3_SCATTER_WARPS);
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_free(tbase, 512);
+}
+
+// dwd / dwr += the CTAs' weight-gradient sums, added in CTA order
+__global__ void wgrad_reduce_kernel(const float* __restrict__ part, uint32_t nparts, float* __restrict__ dwd, float* __restrict__ dwr) {
+    const uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= (uint32_t)W_PART) return;
+    // four running sums over slots k = 0, 1, 2, 3 (mod 4) keep 16 loads in flight; the order of the additions is fixed
+    float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
+    uint32_t k = 0;
+#pragma unroll 4
+    for (; k + 4 <= nparts; k += 4) {
+        a0 += part[(size_t)k * W_PART + e];
+        a1 += part[(size_t)(k + 1) * W_PART + e];
+        a2 += part[(size_t)(k + 2) * W_PART + e];
+        a3 += part[(size_t)(k + 3) * W_PART + e];
+    }
+    for (; k < nparts; ++k) a0 += part[(size_t)k * W_PART + e];
+    const float sum = (a0 + a1) + (a2 + a3);
+    if (e < (uint32_t)WD_N) dwd[e] += sum; else dwr[e - WD_N] += sum;
+}
+
+// grid_grad += the fixed-point sums (one fp16 rounding per feature), and the touched fixed-point entries back to zero.  The level table
+// gives the number of entries; entries beyond the scratch were reduced into grid_grad directly.
+__global__ void grid_grad_flush_kernel(const NgpLevel* __restrict__ levels, uint32_t fx_entries, longlong2* __restrict__ fx,
+                                       __half2* __restrict__ grid_grad) {
+    const uint32_t n = min(levels[N_LEVELS - 1].offset + levels[N_LEVELS - 1].size, fx_entries);
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const longlong2 q = fx[i];
+        if (q.x | q.y) {
+            float2 g = __half22float2(grid_grad[i]);
+            g.x += __ll2float_rn(q.x) * FX_INV;
+            g.y += __ll2float_rn(q.y) * FX_INV;
+            grid_grad[i] = __floats2half2_rn(g.x, g.y);
+            fx[i] = make_longlong2(0, 0);
+        }
+    }
+}
+
+// Scratch of ngp_network_bwd, one per (device, stream) so that calls on different streams never share it: the fixed-point gradient,
+// sized from the level table when a table is first seen on that stream, and the per-CTA weight-gradient slots.
+struct BwdScratch {
+    int dev = -1;
+    cudaStream_t stream = nullptr;
+    const void* levels = nullptr;
+    uint32_t fx_entries = 0;
+    unsigned long long* fx = nullptr;
+    float* part = nullptr;
+};
+std::mutex g_scratch_mu;
+std::vector<BwdScratch*> g_scratch;
+
+// The scratch for this call, or nullptr (the call then reduces straight into its outputs) when it cannot be set up: inside graph
+// capture, where nothing may be allocated or read back.  A table seen for the first time costs one read-back of its last level.
+int bwd_scratch(cudaStream_t s, const void* levels_dev, BwdScratch** out) {
+    *out = nullptr;
+    int dev = 0;
+    NGP_CHECK_CUDA(cudaGetDevice(&dev));
+    BwdScratch* b = nullptr;
+    {
+        std::lock_guard<std::mutex> lock(g_scratch_mu);
+        for (BwdScratch* e : g_scratch)
+            if (e->dev == dev && e->stream == s) b = e;
+        if (!b) {
+            b = new BwdScratch;
+            b->dev = dev;
+            b->stream = s;
+            g_scratch.push_back(b);
+        }
+    }
+    if (b->levels == levels_dev && b->part) { *out = b; return 0; }
+    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+    NGP_CHECK_CUDA(cudaStreamIsCapturing(s, &cap));
+    if (cap != cudaStreamCaptureStatusNone) return 0;
+    NgpLevel last;
+    NGP_CHECK_CUDA(cudaMemcpyAsync(&last, reinterpret_cast<const NgpLevel*>(levels_dev) + N_LEVELS - 1, sizeof(last), cudaMemcpyDeviceToHost, s));
+    NGP_CHECK_CUDA(cudaStreamSynchronize(s));
+    const uint32_t entries = last.offset + last.size;
+    if (entries > b->fx_entries) {
+        if (b->fx) NGP_CHECK_CUDA(cudaFree(b->fx));
+        b->fx = nullptr;
+        b->fx_entries = 0;
+        NGP_CHECK_CUDA(cudaMalloc(&b->fx, sizeof(unsigned long long) * 2 * (size_t)entries));
+        NGP_CHECK_CUDA(cudaMemset(b->fx, 0, sizeof(unsigned long long) * 2 * (size_t)entries));
+        b->fx_entries = entries;
+    }
+    if (!b->part) NGP_CHECK_CUDA(cudaMalloc(&b->part, sizeof(float) * W_PART * (size_t)ngp_num_sms()));
+    b->levels = levels_dev;
+    *out = b;
+    return 0;
 }
 
 }  // namespace
@@ -576,7 +634,7 @@ int ngp_network_fwd(void* stream, uint32_t n_max, const uint32_t* n_dev, const f
     const uint32_t enc_tma = (!no_tma && enc_save && ngp_make_rows32_tensormap(&enc_map, enc_save, n_max)) ? 1u : 0u;
     network_fwd_kernel<false><<<grid_dim, FWD_THREADS, SmemFwd::total, s>>>(n_max, n_dev, coords, (const __half*)grid, (const NgpLevel*)levels_dev,
                                                                    (const __half*)w_density, (const __half*)w_rgb, (__half*)out,
-                                                                   (__half*)enc_save, ngp_err_flag(), enc_map, enc_tma);
+                                                                   (__half*)enc_save, enc_map, enc_tma);
     NGP_LAUNCH_CHECK();
     return 0;
 }
@@ -588,7 +646,7 @@ int ngp_density_fwd(void* stream, uint32_t n, const float* pos, const void* grid
     const uint32_t ntiles = (n + ROWS - 1) / ROWS;
     const uint32_t grid_dim = min(ntiles, (uint32_t)ngp_num_sms() * 2u);
     network_fwd_kernel<true><<<grid_dim, FWD_THREADS, SmemFwd::total, s>>>(n, nullptr, pos, (const __half*)grid, (const NgpLevel*)levels_dev,
-                                                                  (const __half*)w_density, nullptr, (__half*)sigma_out, nullptr, ngp_err_flag(), NgpTensorMap{}, 0u);
+                                                                  (const __half*)w_density, nullptr, (__half*)sigma_out, nullptr, NgpTensorMap{}, 0u);
     NGP_LAUNCH_CHECK();
     return 0;
 }
@@ -605,10 +663,20 @@ int ngp_network_bwd(void* stream, uint32_t n_max, const uint32_t* n_dev, const f
     NgpTensorMap enc_map{};
     static const bool no_tma = getenv("NGP_NO_TMA") != nullptr;           // A/B switch
     const uint32_t enc_tma = (!no_tma && ngp_make_rows32_tensormap(&enc_map, enc_save, n_max)) ? 1u : 0u;
+    BwdScratch* b = nullptr;
+    if (int rc = bwd_scratch(s, levels_dev, &b)) return rc;
     network_bwd256_kernel<<<grid_dim, B3_THREADS, SmemBwd3::total, s>>>(n_max, n_dev, coords, (const __half*)enc_save, (const NgpLevel*)levels_dev,
                                                                        (const __half*)w_density, (const __half*)w_rgb, (const __half*)dout,
-                                                                       (__half*)grid_grad, dw_density, dw_rgb, ngp_err_flag(), dbg, enc_map, enc_tma);
+                                                                       (__half*)grid_grad, dw_density, dw_rgb, b ? b->fx : nullptr,
+                                                                       b ? b->fx_entries : 0u, b ? b->part : nullptr, ngp_err_flag(), dbg, enc_map, enc_tma);
     NGP_LAUNCH_CHECK();
+    if (b) {
+        wgrad_reduce_kernel<<<(W_PART + 255) / 256, 256, 0, s>>>(b->part, grid_dim, dw_density, dw_rgb);
+        NGP_LAUNCH_CHECK();
+        grid_grad_flush_kernel<<<ngp_num_sms() * 8, 256, 0, s>>>((const NgpLevel*)levels_dev, b->fx_entries, reinterpret_cast<longlong2*>(b->fx),
+                                                                 (__half2*)grid_grad);
+        NGP_LAUNCH_CHECK();
+    }
     return 0;
 }
 

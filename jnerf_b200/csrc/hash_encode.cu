@@ -45,10 +45,8 @@ __device__ __forceinline__ void red_add(float2* addr, float a, float b) { red_ad
 // ---- HashEncoder forward / backward (R2 / R3), run-length form -------------------------------------------------------------------
 // Thread (level, sub) walks RUN consecutive points and keeps the 8 corner values (forward) / 8 fp32 corner accumulators (backward) of
 // a grid cell while CONSECUTIVE points stay inside it -- the sampler hands points over ray-ordered, so at the coarse levels dozens
-// do -- which cuts the L2 requests / f16x2 reductions by the mean run length.  Measured on a B200 against the one-point-per-thread
-// kernels of round 1 (profiles/r02_first_call, r02_call2): ray-ordered samples of a training state, forward 61 -> 49 us, backward
-// 277 -> 99 us (the reference's own kernels recompiled for sm_100a: 97 / 417 us); uniformly random points (no runs), forward
-// 109 -> 95 us, backward 216 -> 224 us.  Per point the arithmetic is the reference's (corner order and fma chain of
+// do -- which cuts the L2 requests / f16x2 reductions by the mean run length.  Uniformly random points (no runs) gain nothing from it
+// and lose little.  Per point the arithmetic is the reference's (corner order and fma chain of
 // HashEncode.h:171-201); the backward rounds each run's fp32 sum once instead of once per point.
 constexpr int RUN = 16;
 constexpr int RUN_PTS_PER_BLOCK = (HASH_THREADS / N_LEVELS) * RUN;   // 256

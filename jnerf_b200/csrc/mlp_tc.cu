@@ -1,13 +1,13 @@
 // R7: the fully-fused MLP as a standalone operator pair (FMLP / FullyFusedMlp_weight boundary,
-// OPS/fully_fused_mlp.py:12-145) on tcgen05 tensor cores.
+// OPS/fully_fused_mlp.py:12-145) on Hopper wgmma.
 //
-// Forward:  persistent CTAs of 128 threads, one 128-row tile at a time.  Weights (<= 30 KB) are staged once per
-//   CTA in the canonical K-major UMMA layout; the input tile is written straight into an operand slab; each layer is
-//   K/16 tcgen05.mma (M=128, N=64 or 16) into TMEM; the epilogue (tcgen05.ld -> ReLU -> fp16) writes the next
-//   layer's operand slab and the `output_intermediate` block the reference keeps for backward.
+// Forward:  persistent CTAs of one warpgroup (128 threads), one 128-row tile at a time.  Weights (<= 30 KB) are staged once per
+//   CTA in the canonical K-major GMMA layout; the input tile is written straight into an operand slab; each layer is
+//   K/16 wgmma (M=64 per row block, N=64 or 16) into registers; the epilogue (ReLU -> fp16) writes the next layer's operand slab,
+//   from which the `output_intermediate` block the reference keeps for backward is copied out row by row.
 // Backward: dgrad chain through the same slabs with the weight tiles read MN-major (no transposed copy), and the
-//   weight gradients accumulated across all tiles of the CTA in TMEM (wgrad = A^T dY with both operands read
-//   MN-major from the activation / gradient slabs), flushed once with fp32 atomics.  This replaces the reference's
+//   weight gradients accumulated across all tiles of the CTA in registers (wgrad = dY^T A with both operands read
+//   MN-major from the gradient / activation slabs), flushed once with fp32 reductions.  This replaces the reference's
 //   kernel_mlp_fused_backward + 5 cuBLAS GEMMs with K = batch (fully_fused_mlp.py:123-143).
 // Roofline: tensor (DESIGN.md): 20 480 flop/sample fwd for the two NGP nets, 61 440 fwd+dgrad+wgrad.
 #include "mlp_tc.cuh"
@@ -26,34 +26,27 @@ struct FwdSmem {
     static constexpr uint32_t w0 = 16 * GB;                       // 64x32 -> 4 KB
     static constexpr uint32_t wh = w0 + WIDTH * IN * 2;           // n_hm x 8 KB
     __host__ __device__ static constexpr uint32_t wout(uint32_t nhm) { return wh + nhm * WIDTH * WIDTH * 2; }
-    __host__ __device__ static constexpr uint32_t bar(uint32_t nhm) { return wout(nhm) + OUTP * WIDTH * 2; }
-    __host__ __device__ static constexpr uint32_t total(uint32_t nhm) { return bar(nhm) + 64; }
+    __host__ __device__ static constexpr uint32_t total(uint32_t nhm) { return wout(nhm) + OUTP * WIDTH * 2; }
 };
 
 __global__ void __launch_bounds__(128)
 mlp_fwd_kernel(const __half* __restrict__ W, const __half* __restrict__ X, __half* __restrict__ inter, __half* __restrict__ Y,
-               uint32_t nhm, uint32_t n, int* __restrict__ err) {
+               uint32_t nhm, uint32_t n) {
     extern __shared__ __align__(1024) uint8_t smem[];
-    const uint32_t t = threadIdx.x, warp = t >> 5;
-    uint64_t* bar = reinterpret_cast<uint64_t*>(smem + FwdSmem::bar(nhm));
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bar + 1);
+    const uint32_t t = threadIdx.x;
 
     stage_weights(smem + FwdSmem::w0, W, WIDTH, IN, t, 128);
     for (uint32_t j = 0; j < nhm; ++j)
         stage_weights(smem + FwdSmem::wh + j * WIDTH * WIDTH * 2, W + WIDTH * IN + j * WIDTH * WIDTH, WIDTH, WIDTH, t, 128);
     stage_weights(smem + FwdSmem::wout(nhm), W + WIDTH * IN + nhm * WIDTH * WIDTH, OUTP, WIDTH, t, 128);
-    if (t == 0) { mbar_init(bar, 1); fence_mbar_init(); }
-    if (warp == 0) tmem_alloc(tmem_ptr, 128);
-    sync_before_issue();
-    const uint32_t tbase = *tmem_ptr;
     const uint32_t smem_s = smem_u32(smem);
-    Pipe pipe{bar, 0, err};
-    const uint32_t D_H = 0, D_O = 64;
+    const uint32_t r0 = frag_row(t), cb = (t & 3u) * 4u;
 
     const uint32_t ntiles = (n + ROWS - 1) / ROWS;
     for (uint32_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
         const uint32_t row = tile * ROWS + t;
         const bool valid = row < n;
+        __syncthreads();                                          // the previous tile's last wgmmas have read slab0
         // input row -> slab0 groups 0..3
         {
             const uint4* src = reinterpret_cast<const uint4*>(X + (size_t)row * IN);
@@ -63,98 +56,89 @@ mlp_fwd_kernel(const __half* __restrict__ W, const __half* __restrict__ X, __hal
                 *reinterpret_cast<uint4*>(smem + FwdSmem::slab0 + g * GB + t * 16) = v;
             }
         }
-        sync_before_issue();
+        operands_ready(0, 128);
         uint32_t cur = FwdSmem::slab0, nxt = FwdSmem::slab1;
         // layer 0
-        if (warp == 0) { if (elect_one()) { issue_fwd<IN, WIDTH>(tbase + D_H, smem_s + cur, 0, smem_s + FwdSmem::w0); pipe.commit(); } __syncwarp(); }
-        pipe.wait();
-        epi_hidden_relu(tbase, D_H, warp, smem + nxt, 0, t, (inter && valid) ? inter + ((size_t)0 * n + row) * WIDTH : nullptr);
-        sync_before_issue();
+        layer<WIDTH>([&](float (&d)[WIDTH / 2], uint32_t m) { mma_fwd<IN, WIDTH>(d, smem_s + cur, 0, smem_s + FwdSmem::w0, m); },
+                     [&](const float (&d)[WIDTH / 2], uint32_t m) { frag_to_slab<WIDTH, true>(d, smem + nxt, 0, m, t); });
+        operands_ready(0, 128);
+        if (inter && valid) slab_row_to_global(smem + nxt, 0, t, inter + ((size_t)0 * n + row) * WIDTH);
         { uint32_t s = cur; cur = nxt; nxt = s; }
         for (uint32_t j = 0; j < nhm; ++j) {
-            if (warp == 0) { if (elect_one()) { issue_fwd<WIDTH, WIDTH>(tbase + D_H, smem_s + cur, 0, smem_s + FwdSmem::wh + j * WIDTH * WIDTH * 2); pipe.commit(); } __syncwarp(); }
-            pipe.wait();
-            epi_hidden_relu(tbase, D_H, warp, smem + nxt, 0, t, (inter && valid) ? inter + ((size_t)(j + 1) * n + row) * WIDTH : nullptr);
-            sync_before_issue();
+            const uint32_t w_s = smem_s + FwdSmem::wh + j * WIDTH * WIDTH * 2;
+            layer<WIDTH>([&](float (&d)[WIDTH / 2], uint32_t m) { mma_fwd<WIDTH, WIDTH>(d, smem_s + cur, 0, w_s, m); },
+                         [&](const float (&d)[WIDTH / 2], uint32_t m) { frag_to_slab<WIDTH, true>(d, smem + nxt, 0, m, t); });
+            operands_ready(0, 128);
+            if (inter && valid) slab_row_to_global(smem + nxt, 0, t, inter + ((size_t)(j + 1) * n + row) * WIDTH);
             { uint32_t s = cur; cur = nxt; nxt = s; }
         }
-        if (warp == 0) { if (elect_one()) { issue_fwd<WIDTH, OUTP>(tbase + D_O, smem_s + cur, 0, smem_s + FwdSmem::wout(nhm)); pipe.commit(); } __syncwarp(); }
-        pipe.wait();
-        {
-            float v[16];
-            tmem_ld16(tmem_addr(tbase, warp, D_O), v);
-            uint4 lo, hi;
-            pack16(v, lo, hi);
-            if (valid) {
-                uint4* dst = reinterpret_cast<uint4*>(Y + (size_t)row * OUTP);
-                dst[0] = lo; dst[1] = hi;
-            }
-        }
-        // the next tile's sync_before_issue orders these TMEM reads before the next MMA
+        layer<OUTP>([&](float (&d)[OUTP / 2], uint32_t m) { mma_fwd<WIDTH, OUTP>(d, smem_s + cur, 0, smem_s + FwdSmem::wout(nhm), m); },
+                    [&](const float (&d)[OUTP / 2], uint32_t m) {
+#pragma unroll
+                        for (uint32_t h = 0; h < 2; ++h) {
+                            const uint32_t r = tile * ROWS + 64 * m + r0 + 8 * h;
+                            if (r < n) {
+#pragma unroll
+                                for (uint32_t c = 0; c < 2; ++c)
+                                    *reinterpret_cast<uint32_t*>(reinterpret_cast<uint8_t*>(Y + (size_t)r * OUTP + 8 * c) + cb) =
+                                        pack_half2(d[4 * c + 2 * h], d[4 * c + 2 * h + 1]);
+                            }
+                        }
+                    });
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_free(tbase, 128);
 }
 
 // ------------------------------------------------------------------------------------------------------
 // Backward.  Slab map (groups of 8 features):
 //   ACT: [0,4) X | [4+8k, 12+8k) hidden k                       (nh = nhm+1 hidden layers)
 //   GRD: [0,2) dY | [2+8j, 10+8j) gradient block j (j=0: last hidden layer ... j=nhm: first)   -- `temps` order
-// TMEM columns: [0,64) dgrad scratch | [64,96) dX | wgrad accumulators from 96:
-//   Wout: lanes = in feature (64 valid) x 16 cols ; Wh_j / W0: lanes = in feature x 64 cols.
+// Weight-gradient accumulators (registers, all tiles of the CTA): Wout as [64 in][16 out], Wh_k and W0 as [64 out][in].
 struct BwdLayout {
     uint32_t nhm;
     __host__ __device__ uint32_t act_groups() const { return 4 + 8 * (nhm + 1); }
     __host__ __device__ uint32_t grd_groups() const { return 2 + 8 * (nhm + 1); }
     __host__ __device__ uint32_t act() const { return 0; }
     __host__ __device__ uint32_t grd() const { return act_groups() * GB; }
-    // 16 spare groups so that a 128-lane MN-major read starting at the last gradient block stays in bounds
-    __host__ __device__ uint32_t w0() const { return grd() + (grd_groups() + 16) * GB; }
+    // 8 spare groups so that a 64-feature MN-major read starting at the last gradient block stays in bounds
+    __host__ __device__ uint32_t w0() const { return grd() + (grd_groups() + 8) * GB; }
     __host__ __device__ uint32_t wh() const { return w0() + WIDTH * IN * 2; }
     __host__ __device__ uint32_t wout() const { return wh() + nhm * WIDTH * WIDTH * 2; }
-    __host__ __device__ uint32_t bar() const { return wout() + OUTP * WIDTH * 2; }
-    __host__ __device__ uint32_t total() const { return bar() + 64; }
-    __host__ __device__ uint32_t tmem_cols() const { return (96 + 16 + 64 * (nhm + 1)) <= 256 ? 256 : 512; }
+    __host__ __device__ uint32_t total() const { return wout() + OUTP * WIDTH * 2; }
 };
 
+template <uint32_t NHM>
 __global__ void __launch_bounds__(128)
 mlp_bwd_kernel(const __half* __restrict__ W, const __half* __restrict__ X, const __half* __restrict__ inter,
                const __half* __restrict__ dY, int dy_feature_major, __half* __restrict__ dX, __half* __restrict__ temps,
-               float* __restrict__ dW, uint32_t nhm, uint32_t n_out_valid, uint32_t n, int* __restrict__ err) {
+               float* __restrict__ dW, uint32_t n_out_valid, uint32_t n) {
     // dW == nullptr: dgrad chain only (the link-level mlp_fused_backward_func contract, compat_tcnn.cu); X may then be nullptr.
     // dy_feature_major: dY is (16, n) -- the transposed gradient the reference hands to its backward (fully_fused_mlp.py:117).
     extern __shared__ __align__(1024) uint8_t smem[];
-    const BwdLayout L{nhm};
-    const uint32_t t = threadIdx.x, warp = t >> 5;
-    const uint32_t nh = nhm + 1;
-    uint64_t* bar = reinterpret_cast<uint64_t*>(smem + L.bar());
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bar + 1);
+    constexpr BwdLayout L{NHM};
+    constexpr uint32_t nh = NHM + 1;
+    const uint32_t t = threadIdx.x;
 
     stage_weights(smem + L.w0(), W, WIDTH, IN, t, 128);
-    for (uint32_t j = 0; j < nhm; ++j)
+    for (uint32_t j = 0; j < NHM; ++j)
         stage_weights(smem + L.wh() + j * WIDTH * WIDTH * 2, W + WIDTH * IN + j * WIDTH * WIDTH, WIDTH, WIDTH, t, 128);
-    stage_weights(smem + L.wout(), W + WIDTH * IN + nhm * WIDTH * WIDTH, OUTP, WIDTH, t, 128);
-    // spare groups after GRD are read (and ignored) by 128-lane wgrad operands: keep them finite
-    for (uint32_t i = t; i < 16 * GB / 16; i += 128)
+    stage_weights(smem + L.wout(), W + WIDTH * IN + NHM * WIDTH * WIDTH, OUTP, WIDTH, t, 128);
+    // spare groups after GRD are read (and ignored) by 64-feature weight-gradient operands: keep them finite
+    for (uint32_t i = t; i < 8 * GB / 16; i += 128)
         *reinterpret_cast<uint4*>(smem + L.grd() + L.grd_groups() * GB + i * 16) = make_uint4(0, 0, 0, 0);
-    if (t == 0) { mbar_init(bar, 1); fence_mbar_init(); }
-    if (warp == 0) tmem_alloc(tmem_ptr, L.tmem_cols());
-    sync_before_issue();
-    const uint32_t tbase = *tmem_ptr;
     const uint32_t smem_s = smem_u32(smem);
     const uint32_t act_s = smem_s + L.act(), grd_s = smem_s + L.grd();
     uint8_t* act = smem + L.act();
     uint8_t* grd = smem + L.grd();
-    Pipe pipe{bar, 0, err};
-    const uint32_t D_G = 0, D_X = 64, D_WOUT = 96, D_W = 112;   // D_W + 64*k: k=0 -> W0, k=j -> Wh_{j-1}
+    const uint32_t r0 = frag_row(t), cb = (t & 3u) * 4u;
+    float a_wout[8], a_wh[NHM > 0 ? NHM : 1][32], a_w0[16];   // weight-gradient accumulators
 
     const uint32_t ntiles = (n + ROWS - 1) / ROWS;
-    uint32_t acc = 0;   // 0 on the CTA's first tile: wgrad accumulators are overwritten
+    uint32_t acc = 0;   // 0 on the CTA's first tile: weight-gradient accumulators are overwritten
     for (uint32_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x, acc = 1) {
         const uint32_t row = tile * ROWS + t;
         const bool valid = row < n;
         const uint4 z = make_uint4(0, 0, 0, 0);
+        __syncthreads();                                          // the previous tile's wgmmas have read the slabs
         {
             const uint4* src = reinterpret_cast<const uint4*>(X + (size_t)row * IN);
 #pragma unroll
@@ -179,87 +163,58 @@ mlp_bwd_kernel(const __half* __restrict__ W, const __half* __restrict__ X, const
             *reinterpret_cast<uint4*>(grd + 0 * GB + t * 16) = d0;
             *reinterpret_cast<uint4*>(grd + 1 * GB + t * 16) = d1;
         }
-        sync_before_issue();
-        // gradient at the last hidden layer, and the output layer's wgrad
-        if (warp == 0) {
-            if (elect_one()) {
-                issue_dgrad<OUTP, WIDTH>(tbase + D_G, grd_s, 0, smem_s + L.wout());
-                if (dW) issue_wgrad<OUTP>(tbase + D_WOUT, act_s, 4 + 8 * (nh - 1), grd_s, 0, acc);
-                pipe.commit();
-            }
-            __syncwarp();
-        }
-        pipe.wait();
-        epi_dgrad_mask(tbase, D_G, warp, act, 4 + 8 * (nh - 1), grd, 2, t, (temps && valid) ? temps + ((size_t)0 * n + row) * WIDTH : nullptr);
-        sync_before_issue();
-        // hidden matmuls, last to first: Wh_{k-1} maps hidden k-1 -> hidden k
+        operands_ready(0, 128);
+        // gradient at the last hidden layer, and the output layer's weight gradient [in][out] = h_last^T dY
+        if (dW) { wgmma_fence(); mma_wgrad<OUTP>(a_wout, act_s, 4 + 8 * (nh - 1), grd_s, 0, acc); }
+        layer<WIDTH>([&](float (&d)[WIDTH / 2], uint32_t m) { mma_dgrad<OUTP, WIDTH>(d, grd_s, 0, smem_s + L.wout(), m); },
+                     [&](const float (&d)[WIDTH / 2], uint32_t m) { frag_dgrad_mask<WIDTH>(d, act, 4 + 8 * (nh - 1), grd, 2, m, t); });
+        operands_ready(0, 128);
+        if (temps && valid) slab_row_to_global(grd, 2, t, temps + ((size_t)0 * n + row) * WIDTH);
+        // hidden matmuls, last to first: Wh_{k-1} maps hidden k-1 -> hidden k; its weight gradient [out][in] = g_k^T h_{k-1}
+#pragma unroll
         for (uint32_t k = nh - 1; k >= 1; --k) {
             const uint32_t j = nh - 1 - k;            // gradient block holding g_k
-            if (warp == 0) {
-                if (elect_one()) {
-                    issue_dgrad<WIDTH, WIDTH>(tbase + D_G, grd_s, 2 + 8 * j, smem_s + L.wh() + (k - 1) * WIDTH * WIDTH * 2);
-                    if (dW) issue_wgrad<WIDTH>(tbase + D_W + 64 * k, act_s, 4 + 8 * (k - 1), grd_s, 2 + 8 * j, acc);
-                    pipe.commit();
-                }
-                __syncwarp();
-            }
-            pipe.wait();
-            epi_dgrad_mask(tbase, D_G, warp, act, 4 + 8 * (k - 1), grd, 2 + 8 * (j + 1), t,
-                           (temps && valid) ? temps + ((size_t)(j + 1) * n + row) * WIDTH : nullptr);
-            sync_before_issue();
+            if (dW) { wgmma_fence(); mma_wgrad<WIDTH>(a_wh[k - 1], grd_s, 2 + 8 * j, act_s, 4 + 8 * (k - 1), acc); }
+            const uint32_t w_s = smem_s + L.wh() + (k - 1) * WIDTH * WIDTH * 2;
+            layer<WIDTH>([&](float (&d)[WIDTH / 2], uint32_t m) { mma_dgrad<WIDTH, WIDTH>(d, grd_s, 2 + 8 * j, w_s, m); },
+                         [&](const float (&d)[WIDTH / 2], uint32_t m) { frag_dgrad_mask<WIDTH>(d, act, 4 + 8 * (k - 1), grd, 2 + 8 * (j + 1), m, t); });
+            operands_ready(0, 128);
+            if (temps && valid) slab_row_to_global(grd, 2 + 8 * (j + 1), t, temps + ((size_t)(j + 1) * n + row) * WIDTH);
         }
-        // first layer: dX = g_0 * W0, wgrad W0 = g_0^T X
+        // first layer: dX = g_0 * W0, weight gradient W0 [out][in] = g_0^T X
         if (!dX && !dW) continue;     // dgrad-only call without dL/dinput: nothing left for this tile (uniform over the CTA)
-        if (warp == 0) {
-            if (elect_one()) {
-                if (dX) issue_dgrad<WIDTH, IN>(tbase + D_X, grd_s, 2 + 8 * nhm, smem_s + L.w0());
-                if (dW) issue_wgrad<WIDTH>(tbase + D_W, act_s, 0, grd_s, 2 + 8 * nhm, acc);
-                pipe.commit();
-            }
-            __syncwarp();
+        if (dW) {
+            wgmma_fence();
+            mma_wgrad<IN>(a_w0, grd_s, 2 + 8 * NHM, act_s, 0, acc);
+            wgmma_commit();
         }
-        pipe.wait();
         if (dX) {
-            float v[16];
-            uint4 lo, hi;
-            uint4* dst = reinterpret_cast<uint4*>(dX + (size_t)row * IN);
-            tmem_ld16(tmem_addr(tbase, warp, D_X), v);
-            pack16(v, lo, hi);
-            if (valid) { dst[0] = lo; dst[1] = hi; }
-            tmem_ld16(tmem_addr(tbase, warp, D_X + 16), v);
-            pack16(v, lo, hi);
-            if (valid) { dst[2] = lo; dst[3] = hi; }
+            layer<IN>([&](float (&d)[IN / 2], uint32_t m) { mma_dgrad<WIDTH, IN>(d, grd_s, 2 + 8 * NHM, smem_s + L.w0(), m); },
+                      [&](const float (&d)[IN / 2], uint32_t m) {
+#pragma unroll
+                          for (uint32_t h = 0; h < 2; ++h) {
+                              const uint32_t r = tile * ROWS + 64 * m + r0 + 8 * h;
+                              if (r < n) {
+#pragma unroll
+                                  for (uint32_t c = 0; c < IN / 8; ++c)
+                                      *reinterpret_cast<uint32_t*>(reinterpret_cast<uint8_t*>(dX + (size_t)r * IN + 8 * c) + cb) =
+                                          pack_half2(d[4 * c + 2 * h], d[4 * c + 2 * h + 1]);
+                              }
+                          }
+                      });
         }
+        wgmma_wait<0>();
     }
-    // flush the weight gradients: lane t = input feature, column = output feature
+    // flush the weight gradients
     if (acc && dW) {
         float* dW0 = dW;
         float* dWh = dW + WIDTH * IN;
-        float* dWo = dWh + nhm * WIDTH * WIDTH;
-        float v[16];
-        if (t < WIDTH) {
-            tmem_ld16(tmem_addr(tbase, warp, D_WOUT), v);
+        float* dWo = dWh + NHM * WIDTH * WIDTH;
+        frag_red_add<OUTP>(a_wout, dWo, 1, WIDTH, WIDTH, n_out_valid, t);
 #pragma unroll
-            for (int o = 0; o < 16; ++o)
-                if ((uint32_t)o < n_out_valid) red_add_f32(dWo + o * WIDTH + t, v[o]);
-        } else {
-            tmem_ld16(tmem_addr(tbase, warp, D_WOUT), v);   // keep the warp-collective tcgen05.ld uniform
-        }
-        for (uint32_t k = 0; k <= nhm; ++k) {
-            const uint32_t in_dim = (k == 0) ? IN : WIDTH;
-            float* dst = (k == 0) ? dW0 : dWh + (k - 1) * WIDTH * WIDTH;
-            for (int c = 0; c < 4; ++c) {
-                tmem_ld16(tmem_addr(tbase, warp, D_W + 64 * k + 16 * c), v);
-                if (t < in_dim) {
-#pragma unroll
-                    for (int o = 0; o < 16; ++o) red_add_f32(dst + (size_t)(16 * c + o) * in_dim + t, v[o]);
-                }
-            }
-        }
+        for (uint32_t k = 1; k <= NHM; ++k) frag_red_add<WIDTH>(a_wh[k - 1], dWh + (k - 1) * WIDTH * WIDTH, WIDTH, 1, WIDTH, WIDTH, t);
+        frag_red_add<IN>(a_w0, dW0, IN, 1, WIDTH, IN, t);
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_free(tbase, L.tmem_cols());
 }
 
 int* g_err_flag = nullptr;
@@ -278,7 +233,7 @@ int* ngp_err_flag() { return err_flag(); }
 extern "C" {
 
 
-// Debug aid: 1 if any tcgen05 pipeline wait timed out since the last call (synchronises the device).
+// Debug aid: 1 if any bounded mbarrier wait of a fused kernel timed out since the last call (synchronises the device).
 int ngp_debug_timeout_flag(void) {
     int* f = err_flag();
     if (!f) return -1;
@@ -297,10 +252,8 @@ int ngp_mlp_fwd(void* stream, const void* weights, const void* input, void* inte
     const uint32_t smem = FwdSmem::total(nhm);
     if (ngp_first_use((const void*)mlp_fwd_kernel)) NGP_CHECK_CUDA(cudaFuncSetAttribute(mlp_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FwdSmem::total(MAX_HM)));
     const uint32_t ntiles = (n + ROWS - 1) / ROWS;
-    uint32_t per_sm = 4u;
-    if (const char* e = getenv("NGP_MLP_CTAS_PER_SM")) per_sm = (uint32_t)atoi(e);   // experiment knob
-    const uint32_t grid = min(ntiles, (uint32_t)ngp_num_sms() * per_sm);
-    mlp_fwd_kernel<<<grid, 128, smem, s>>>((const __half*)weights, (const __half*)input, (__half*)inter, (__half*)output, nhm, n, err_flag());
+    const uint32_t grid = min(ntiles, (uint32_t)ngp_num_sms() * 4u);
+    mlp_fwd_kernel<<<grid, 128, smem, s>>>((const __half*)weights, (const __half*)input, (__half*)inter, (__half*)output, nhm, n);
     NGP_LAUNCH_CHECK();
     return 0;
 }
@@ -311,12 +264,14 @@ static int mlp_bwd_launch(void* stream, const void* weights, const void* input, 
     if (dW) NGP_CHECK_CUDA(cudaMemsetAsync(dW, 0, sizeof(float) * ngp_mlp_param_count(nhm), s));
     if (n == 0) return 0;
     const BwdLayout L{nhm};
-    if (ngp_first_use((const void*)mlp_bwd_kernel)) NGP_CHECK_CUDA(cudaFuncSetAttribute(mlp_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BwdLayout{MAX_HM}.total()));
+    void (*kernel)(const __half*, const __half*, const __half*, const __half*, int, __half*, __half*, float*, uint32_t, uint32_t) =
+        nhm == 0 ? mlp_bwd_kernel<0> : nhm == 1 ? mlp_bwd_kernel<1> : nhm == 2 ? mlp_bwd_kernel<2> : mlp_bwd_kernel<3>;
+    if (ngp_first_use((const void*)kernel)) NGP_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.total()));
     const uint32_t ntiles = (n + ROWS - 1) / ROWS;
-    const uint32_t per_sm = L.tmem_cols() <= 256 && L.total() <= 110 * 1024 ? 2u : 1u;
+    const uint32_t per_sm = L.total() <= 110 * 1024 ? 2u : 1u;
     const uint32_t grid = min(ntiles, (uint32_t)ngp_num_sms() * per_sm);
-    mlp_bwd_kernel<<<grid, 128, L.total(), s>>>((const __half*)weights, (const __half*)input, (const __half*)inter, (const __half*)dY,
-                                                dy_feature_major, (__half*)dX, (__half*)temps, dW, nhm, n_out_valid, n, err_flag());
+    kernel<<<grid, 128, L.total(), s>>>((const __half*)weights, (const __half*)input, (const __half*)inter, (const __half*)dY,
+                                        dy_feature_major, (__half*)dX, (__half*)temps, dW, n_out_valid, n);
     NGP_LAUNCH_CHECK();
     return 0;
 }

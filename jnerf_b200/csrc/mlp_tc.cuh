@@ -1,13 +1,12 @@
-// Building blocks of the fully-fused MLP on tcgen05 (used by mlp_tc.cu and fused_net.cu).
-// A tile is 128 rows (samples); thread t of a 128-thread CTA owns row t for every epilogue
-// (TMEM lane t).  Activations and gradients live in shared-memory "slabs" (see tc05.cuh) and never
-// leave the SM between layers.
+// Building blocks of the fully-fused MLP on Hopper wgmma (used by mlp_tc.cu and fused_net.cu).
+// A tile is 128 rows (samples), processed by one warpgroup; loads and global copies use "thread t = row t", epilogues the wgmma
+// accumulator fragment.  Activations and gradients live in shared-memory "slabs" (see wgmma.cuh) and never leave the SM between layers.
 #pragma once
-#include "tc05.cuh"
+#include "wgmma.cuh"
 #include "ngp_common.cuh"
 
 namespace mlp {
-using namespace tc05;
+using namespace wg;
 
 constexpr uint32_t ROWS = 128;
 constexpr uint32_t GB = ROWS * 16;          // bytes of one slab feature-group (8 features x 128 rows)
@@ -21,49 +20,51 @@ static __device__ __noinline__ void stage_weights(uint8_t* dst, const __half* __
     }
 }
 
-// ---- MMA issue -------------------------------------------------------------------------------------------
-// Issued by ONE elected thread (tc05::elect_one) with every shape a template parameter and every shared-memory offset a constant of
-// the kernel: fully unrolled, the descriptors fold into the uniform datapath (UIADD3 / UMOV) and the UTCHMMAs issue back to back.
-// History (tests/cuda/tc_time4.cu, tc_time5.cu): under `if (tid == 0)` every UTCHMMA sat in an ELECT / BRA.U.ANY waterfall loop
-// (190 cycles per MMA); with descriptor records streamed from shared memory (LDS -> R2UR x6 -> UTCHMMA) the issue loop still cost
-// 75-150 cycles per MMA -- more than the 32 cycles a 128 x 64 x 16 MMA executes in -- whatever the operand layout.
+// ---- MMA issue (all 128 threads of one warpgroup) ----------------------------------------------------------
+// A 128-row tile is two wgmma row blocks: m = 0 covers rows [0, 64), m = 1 rows [64, 128).  Every shape is a template parameter and
+// every shared-memory offset a value of the kernel, so the K loop unrolls into back-to-back wgmmas.
 //
-// D[128 x N] (+)= ACT[:, 8*g0 .. 8*g0+K) * W^T          (W staged with rows = N)
+// D[64 x N] = rows [64m, 64m+64) of ACT[:, 8*g0 .. 8*g0+K) * W^T          (W staged with rows = N)
 template <uint32_t K, uint32_t N>
-__device__ __forceinline__ void issue_fwd(uint32_t d, uint32_t act_s, uint32_t g0, uint32_t w_s) {
+__device__ __forceinline__ void mma_fwd(float (&d)[N / 2], uint32_t act_s, uint32_t g0, uint32_t w_s, uint32_t m) {
 #pragma unroll
     for (uint32_t kb = 0; kb < K / 16; ++kb)
-        mma_f16_ss(d, slab_desc_kmajor(act_s, ROWS, g0, kb), slab_desc_kmajor(w_s, N, 0, kb), idesc_f16(128, N, 0, 0), kb > 0 ? 1u : 0u);
+        mma<N, 0, 0>(d, slab_desc_kmajor(act_s + m * 64 * 16, ROWS, g0, kb), slab_desc_kmajor(w_s, N, 0, kb), kb > 0 ? 1u : 0u);
 }
-// D[128 x NIN] = GRD[:, 8*g0 .. 8*g0+KOUT) * W          (W staged with rows = KOUT, K = NIN; read MN-major)
+// D[64 x NIN] = rows [64m, 64m+64) of GRD[:, 8*g0 .. 8*g0+KOUT) * W[:, 0..NIN)          (W staged with rows = KOUT; read MN-major)
 template <uint32_t KOUT, uint32_t NIN>
-__device__ __forceinline__ void issue_dgrad(uint32_t d, uint32_t grd_s, uint32_t g0, uint32_t w_s) {
+__device__ __forceinline__ void mma_dgrad(float (&d)[NIN / 2], uint32_t grd_s, uint32_t g0, uint32_t w_s, uint32_t m) {
 #pragma unroll
     for (uint32_t kb = 0; kb < KOUT / 16; ++kb)
-        mma_f16_ss(d, slab_desc_kmajor(grd_s, ROWS, g0, kb), slab_desc_mnmajor(w_s, KOUT, 0, kb), idesc_f16(128, NIN, 0, 1), kb > 0 ? 1u : 0u);
+        mma<NIN, 0, 1>(d, slab_desc_kmajor(grd_s + m * 64 * 16, ROWS, g0, kb), slab_desc_mnmajor(w_s, KOUT, 0, kb), kb > 0 ? 1u : 0u);
 }
-// D[128 x N] (+)= A^T B : lanes = features [8*ga, 8*ga+128) of slab a, columns = features [8*gb, 8*gb+N) of slab b,
+// D[64 x N] (+)= A^T B : rows = features [8*ga, 8*ga+64) of slab a, columns = features [8*gb, 8*gb+N) of slab b,
 // contraction over the 128 rows of the tile.  `accumulate` = 0 only for the very first tile of the CTA.
 template <uint32_t N>
-__device__ __forceinline__ void issue_wgrad(uint32_t d, uint32_t a_s, uint32_t ga, uint32_t b_s, uint32_t gb, uint32_t accumulate) {
+__device__ __forceinline__ void mma_wgrad(float (&d)[N / 2], uint32_t a_s, uint32_t ga, uint32_t b_s, uint32_t gb, uint32_t accumulate) {
 #pragma unroll
     for (uint32_t kb = 0; kb < ROWS / 16; ++kb)
-        mma_f16_ss(d, slab_desc_mnmajor(a_s, ROWS, ga, kb), slab_desc_mnmajor(b_s, ROWS, gb, kb), idesc_f16(128, N, 1, 1), kb > 0 ? 1u : accumulate);
+        mma<N, 1, 1>(d, slab_desc_mnmajor(a_s, ROWS, ga, kb), slab_desc_mnmajor(b_s, ROWS, gb, kb), kb > 0 ? 1u : accumulate);
+}
+// One layer over a 128-row tile, one row block at a time: issue(d, m) queues the wgmmas of row block m, epi(d, m) consumes them.
+// Any wgmma the warpgroup queued before (weight gradients) completes with the first block.
+template <uint32_t N, class Issue, class Epi>
+__device__ __forceinline__ void layer(Issue issue, Epi epi) {
+#pragma unroll
+    for (uint32_t m = 0; m < 2; ++m) {
+        float d[N / 2];
+#pragma unroll
+        for (uint32_t i = 0; i < N / 2; ++i) d[i] = 0.f;
+        wgmma_fence();
+        issue(d, m);
+        wgmma_commit();
+        wgmma_wait<0>();
+        epi(d, m);
+    }
 }
 
-// ---- epilogue helpers (thread t = row t) ----------------------------------------------------------
-__device__ __forceinline__ void pack16(const float* v, uint4& lo, uint4& hi) {
-    lo = make_uint4(pack_half2(v[0], v[1]), pack_half2(v[2], v[3]), pack_half2(v[4], v[5]), pack_half2(v[6], v[7]));
-    hi = make_uint4(pack_half2(v[8], v[9]), pack_half2(v[10], v[11]), pack_half2(v[12], v[13]), pack_half2(v[14], v[15]));
-}
-// store 16 consecutive features (two groups g, g+1) of row t
-__device__ __forceinline__ void slab_store16(uint8_t* slab, uint32_t g, uint32_t t, const uint4& lo, const uint4& hi) {
-    *reinterpret_cast<uint4*>(slab + (size_t)g * GB + t * 16) = lo;
-    *reinterpret_cast<uint4*>(slab + (size_t)(g + 1) * GB + t * 16) = hi;
-}
-__device__ __forceinline__ uint4 slab_load8(const uint8_t* slab, uint32_t g, uint32_t t) {
-    return *reinterpret_cast<const uint4*>(slab + (size_t)g * GB + t * 16);
-}
+// ---- epilogue helpers (fragment layout, see wgmma.cuh; tw = thread of the warpgroup) ------------------------------
+__device__ __forceinline__ uint32_t frag_row(uint32_t tw) { return 16u * (tw >> 5) + ((tw & 31u) >> 2); }
 // zero the entries of packed half2 `grad` where the matching `act` half is <= 0 (ReLU')
 __device__ __forceinline__ uint32_t relu_mask2(uint32_t grad, uint32_t act) {
     const __half2 a = *reinterpret_cast<const __half2*>(&act);
@@ -71,58 +72,57 @@ __device__ __forceinline__ uint32_t relu_mask2(uint32_t grad, uint32_t act) {
     const uint32_t m = __hgt2_mask(a, z);
     return grad & m;
 }
-__device__ __forceinline__ uint4 relu_mask8(uint4 g, uint4 a) {
-    return make_uint4(relu_mask2(g.x, a.x), relu_mask2(g.y, a.y), relu_mask2(g.z, a.z), relu_mask2(g.w, a.w));
-}
-
-// Hidden-layer epilogue: D[:, 0..64) -> ReLU -> fp16 -> slab groups [g0, g0+8); optionally also to global (row-major 64).
-static __device__ __noinline__ void epi_hidden_relu(uint32_t tbase, uint32_t dcol, uint32_t warp, uint8_t* slab, uint32_t g0, uint32_t t,
-                                                __half* gdst /* row pointer or nullptr */) {
-    uint32_t r[4][16];
+// rows [64m, 64m+64) of D (N columns) -> fp16 (ReLU optional) -> slab groups [g0, g0+N/8)
+template <uint32_t N, bool RELU>
+__device__ __forceinline__ void frag_to_slab(const float (&d)[N / 2], uint8_t* slab, uint32_t g0, uint32_t m, uint32_t tw) {
+    const uint32_t r = 64u * m + frag_row(tw), cb = (tw & 3u) * 4u;
 #pragma unroll
-    for (int c = 0; c < 4; ++c) tmem_ld16_nowait(tmem_addr(tbase, warp & 3, dcol + 16 * c), r[c]);   // 64 columns in flight
-    tmem_ld_wait();
+    for (uint32_t c = 0; c < N / 8; ++c)
 #pragma unroll
-    for (int c = 0; c < 4; ++c) {
-        float v[16];
-#pragma unroll
-        for (int i = 0; i < 16; ++i) v[i] = fmaxf(__uint_as_float(r[c][i]), 0.f);
-        uint4 lo, hi;
-        pack16(v, lo, hi);
-        slab_store16(slab, g0 + 2 * c, t, lo, hi);
-        if (gdst) {
-            reinterpret_cast<uint4*>(gdst)[2 * c] = lo;
-            reinterpret_cast<uint4*>(gdst)[2 * c + 1] = hi;
+        for (uint32_t h = 0; h < 2; ++h) {
+            float a = d[4 * c + 2 * h], b = d[4 * c + 2 * h + 1];
+            if (RELU) { a = fmaxf(a, 0.f); b = fmaxf(b, 0.f); }
+            *reinterpret_cast<uint32_t*>(slab + (g0 + c) * GB + (r + 8 * h) * 16 + cb) = pack_half2(a, b);
         }
-    }
 }
-// dgrad epilogue: D[:, 0..64) -> fp16 -> masked by ReLU'(act) -> grad slab groups [g0,g0+8); optional global copy.
-static __device__ __noinline__ void epi_dgrad_mask(uint32_t tbase, uint32_t dcol, uint32_t warp, const uint8_t* act_slab, uint32_t ga,
-                                               uint8_t* grd_slab, uint32_t g0, uint32_t t, __half* gdst) {
-    uint32_t r[4][16];
+// dgrad epilogue: rows [64m, 64m+64) of D -> fp16 -> masked by ReLU'(act groups [ga, ..)) -> grad slab groups [g0, g0+N/8)
+template <uint32_t N>
+__device__ __forceinline__ void frag_dgrad_mask(const float (&d)[N / 2], const uint8_t* act_slab, uint32_t ga, uint8_t* grd_slab, uint32_t g0,
+                                                uint32_t m, uint32_t tw) {
+    const uint32_t r = 64u * m + frag_row(tw), cb = (tw & 3u) * 4u;
 #pragma unroll
-    for (int c = 0; c < 4; ++c) tmem_ld16_nowait(tmem_addr(tbase, warp & 3, dcol + 16 * c), r[c]);
-    tmem_ld_wait();
+    for (uint32_t c = 0; c < N / 8; ++c)
 #pragma unroll
-    for (int c = 0; c < 4; ++c) {
-        float v[16];
-#pragma unroll
-        for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[c][i]);
-        uint4 lo, hi;
-        pack16(v, lo, hi);
-        lo = relu_mask8(lo, slab_load8(act_slab, ga + 2 * c, t));
-        hi = relu_mask8(hi, slab_load8(act_slab, ga + 2 * c + 1, t));
-        slab_store16(grd_slab, g0 + 2 * c, t, lo, hi);
-        if (gdst) {
-            reinterpret_cast<uint4*>(gdst)[2 * c] = lo;
-            reinterpret_cast<uint4*>(gdst)[2 * c + 1] = hi;
+        for (uint32_t h = 0; h < 2; ++h) {
+            const uint32_t o = (r + 8 * h) * 16 + cb;
+            const uint32_t a = *reinterpret_cast<const uint32_t*>(act_slab + (ga + c) * GB + o);
+            *reinterpret_cast<uint32_t*>(grd_slab + (g0 + c) * GB + o) = relu_mask2(pack_half2(d[4 * c + 2 * h], d[4 * c + 2 * h + 1]), a);
         }
-    }
+}
+// row t of slab groups [g0, g0+8) -> one row-major 64-half row in global memory
+__device__ __forceinline__ void slab_row_to_global(const uint8_t* slab, uint32_t g0, uint32_t t, __half* dst) {
+#pragma unroll
+    for (uint32_t g = 0; g < 8; ++g) reinterpret_cast<uint4*>(dst)[g] = *reinterpret_cast<const uint4*>(slab + (g0 + g) * GB + t * 16);
+}
+// weight-gradient fragment D[64 x N] -> fp32 reductions into dst[r * ld_r + c * ld_c] for r < r_valid, c < c_valid
+template <uint32_t N>
+__device__ __forceinline__ void frag_red_add(const float (&d)[N / 2], float* dst, uint32_t ld_r, uint32_t ld_c, uint32_t r_valid, uint32_t c_valid,
+                                             uint32_t tw) {
+    const uint32_t r0 = frag_row(tw), c0 = 2u * (tw & 3u);
+#pragma unroll
+    for (uint32_t c = 0; c < N / 8; ++c)
+#pragma unroll
+        for (uint32_t h = 0; h < 2; ++h)
+#pragma unroll
+            for (uint32_t j = 0; j < 2; ++j) {
+                const uint32_t r = r0 + 8 * h, col = 8 * c + c0 + j;
+                if (r < r_valid && col < c_valid) red_add_f32(dst + r * ld_r + col * ld_c, d[4 * c + 2 * h + j]);
+            }
 }
 
 // named barriers (bar.sync / bar.arrive) for warp-specialised kernels; id 0 is __syncthreads
 // The barrier id is always emitted as an IMMEDIATE: with a register operand ptxas must reserve all 16 hardware barriers for the
-// CTA ("used 16 barriers"), and barriers are an occupancy limiter (ncu: "Block Limit Barriers") -- two CTAs per SM need <= 8 each.
+// CTA, and barriers are an occupancy limiter -- two CTAs per SM need <= 8 each.
 template <uint32_t ID>
 __device__ __forceinline__ void bar_sync_imm(uint32_t nthreads) { asm volatile("bar.sync %0, %1;" ::"n"(ID), "r"(nthreads) : "memory"); }
 template <uint32_t ID>
@@ -160,38 +160,25 @@ __device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t nthreads)
     }
 }
 
-// Sync point between "all threads wrote smem operands / finished reading TMEM" and "thread 0 issues MMAs".
-// CHAIN128 = true: only the 128 MLP-chain threads (warps 0-3) of a warp-specialised CTA take part (named barrier 1).
-template <bool CHAIN128 = false>
-__device__ __forceinline__ void sync_before_issue() {
-    tc_fence_before();
-    fence_proxy_async_smem();
-    if (CHAIN128) named_bar_sync(1, 128); else __syncthreads();
-    tc_fence_after();
+// weight-gradient fragment D[64 x N] -> plain stores dst[r * ld_r + c * ld_c] for all 64 rows and N columns, 0 for columns >= c_valid
+template <uint32_t N>
+__device__ __forceinline__ void frag_store(const float (&d)[N / 2], float* dst, uint32_t ld_r, uint32_t ld_c, uint32_t c_valid, uint32_t tw) {
+    const uint32_t r0 = frag_row(tw), c0 = 2u * (tw & 3u);
+#pragma unroll
+    for (uint32_t c = 0; c < N / 8; ++c)
+#pragma unroll
+        for (uint32_t h = 0; h < 2; ++h)
+#pragma unroll
+            for (uint32_t j = 0; j < 2; ++j) {
+                const uint32_t r = r0 + 8 * h, col = 8 * c + c0 + j;
+                dst[r * ld_r + col * ld_c] = col < c_valid ? d[4 * c + 2 * h + j] : 0.f;
+            }
 }
 
-// chain-group variant: `bar_id` is the named barrier of the 128 threads that form one MLP chain
-__device__ __forceinline__ void sync_chain(uint32_t bar_id) {
-    tc_fence_before();
+// generic-proxy stores to operand slabs -> visible to the wgmmas of every thread that passes the barrier (0 = __syncthreads)
+__device__ __forceinline__ void operands_ready(uint32_t bar_id, uint32_t nthreads) {
     fence_proxy_async_smem();
-    named_bar_sync(bar_id, 128);
-    tc_fence_after();
+    if (bar_id == 0) __syncthreads(); else named_bar_sync(bar_id, nthreads);
 }
-
-struct Pipe {
-    uint64_t* bar;
-    uint32_t phase;
-    int* err;
-    __device__ __forceinline__ void commit() { mma_commit(bar); }
-    __device__ __forceinline__ void wait() {
-        // The issuing thread's warp-mates must not start polling while it is still issuing: a blocking mbarrier.try_wait on the
-        // divergent path stalls the whole warp, and the single-thread MMA issue took ~570 cycles instead of ~50 per stage
-        // (tools/dbg_timeline_bwd.py).  Reconverge first.
-        __syncwarp();
-        if (!mbar_wait(bar, phase)) { if (err) atomicExch(err, 1); }
-        phase ^= 1;
-        tc_fence_after();
-    }
-};
 
 }  // namespace mlp

@@ -1,4 +1,4 @@
-// Shared host/device helpers for libngp_b200 (sm_100a).
+// Shared host/device helpers for libngp_b200 (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -133,8 +133,8 @@ __device__ __forceinline__ void hash_cell_indices(const NgpLevel& lv, uint32_t g
 // A full-occupancy scatter is bound by the number of L2 reduction REQUESTS (one per lane and instruction), not by bytes.  Corners c and
 // c+1 of a cell are x-neighbours: whenever their entries share an aligned 8-byte word -- dense levels: even index; hashed levels:
 // even x, because (x+1) ^ h = (x ^ h) ^ 1 then -- one REDG.F16x4 serves both.  Half of all cells qualify, i.e. 6 requests per cell
-// instead of 8 on average; the sums formed are exactly the same.  Measured (profiles/r02_kernels/call12): standalone ngp_hash_bwd
-// 99 -> 83 us.  The same idea for the gather (64-bit loads) and inside the fused kernels did not pay and is not used there.
+// instead of 8 on average; the sums formed are exactly the same.  Used by the standalone ngp_hash_bwd; the gather (64-bit loads) and
+// the fused kernels do not use it.
 __device__ __forceinline__ void red_add_corners(__half2* __restrict__ g, const uint32_t idx[8], const float2 acc[8]) {
 #pragma unroll
     for (int c = 0; c < 8; c += 2) {

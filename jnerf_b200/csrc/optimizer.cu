@@ -26,7 +26,7 @@ __device__ __forceinline__ float adam_one(float g, float& m, float& v, float& ma
 // Each thread handles 4 consecutive parameters per slot, so that every 16-byte (fp32) / 8-byte (fp16) access of a warp is one
 // fully coalesced 512 B / 256 B request; UNROLL slots are issued back to back to keep ~100 B per thread in flight.
 // (The first version let a thread own 8 consecutive parameters = 32 B-strided float4 accesses: only 17 of 32 bytes per sector
-//  were used per request and the kernel stalled on the LSU queue at 1.9 TB/s, profiles/r01_step_ncu.md.)
+//  were used per request and the kernel stalled on the LSU queue.)
 template <typename PT, typename GT>
 __global__ void __launch_bounds__(256) adam_ema_kernel(uint64_t n, PT* __restrict__ param, GT* __restrict__ grad, float* __restrict__ m,
                                                        float* __restrict__ v, float* __restrict__ master, AdamArgs a, int zero_grad,

@@ -80,7 +80,7 @@ def load():
     global _lib
     if _lib is None:
         if not os.path.exists(LIB_PATH):
-            raise NgpError(f"{LIB_PATH} is missing: build it with `python jnerf_b200/build.py` (nvcc, sm_100a). "
+            raise NgpError(f"{LIB_PATH} is missing: build it with `python jnerf_b200/build.py` (nvcc, sm_90a). "
                            "There is no CPU fallback.")
         lib = C.CDLL(LIB_PATH)
         for name, (res, args) in SIGNATURES.items():

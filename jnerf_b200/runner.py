@@ -1,5 +1,5 @@
 """Thin training / evaluation driver: the caller of the hot path, mirroring runner/runner.py:14-264 step for step
-(SURVEY.md section 3.1).  `train_step` is the B200 fast path: no autograd graph, no host sync (except the
+(SURVEY.md section 3.1).  `train_step` is the fast path: no autograd graph, no host sync (except the
 reference's own batch-size adaptation every 16 steps), one C-ABI call per stage:
 
     [grid update /16] -> raygen -> march -> (compaction bookkeeping) -> fused network fwd ->
@@ -83,9 +83,8 @@ class Runner:
         if self.world_size == 1:
             # Device-resident step state (include/ngp_b200.h: ngp_step_state_*): the sampler rng, the pixel cursor and Adam's step
             # factors live on the device, so every launch of a training step has the same arguments and the step can be captured in
-            # a CUDA graph per ray-batch size.  Opt-in (NGP_GRAPHS=1): measured +2.5 % at 2^18 samples per iteration once every
-            # ray-batch size of the run has its graph, nothing over 1 000 steps of a still-converging scene (17 sizes, 17 captures),
-            # and -4 % at 2^20 where a capture allocates hundreds of MB (profiles/r02_kernels/call17, r02_final, DESIGN.md section 5).
+            # a CUDA graph per ray-batch size.  Opt-in (NGP_GRAPHS=1): every ray-batch size of a run needs its own capture, and a
+            # capture at large batches allocates hundreds of MB.
             self._dev_state = ops.step_state_new()
             self._dev_expect = None
             self._graphs, self._graph_seen, self._graph_pool, self._cap_stream = {}, {}, None, None

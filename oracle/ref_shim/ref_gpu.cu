@@ -1,4 +1,4 @@
-// oracle/_ref build (SURVEY.md F1): the reference's own CUDA kernels compiled UNMODIFIED for sm_100a, each header in
+// oracle/_ref build (SURVEY.md F1): the reference's own CUDA kernels compiled UNMODIFIED for sm_90a, each header in
 // its own namespace, behind extern "C" launchers that replicate the reference's launch shapes (SURVEY.md 2b).
 // TEST / BENCH INFRASTRUCTURE: the GPU comparator ("the kernel to beat") and the bit-exactness anchor for sample
 // indices (SURVEY.md H4).  Never linked into libngp_b200.so.  Compile with -DREF_CONST_DT=1 (lego) or 0 (fox).

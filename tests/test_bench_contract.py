@@ -109,10 +109,12 @@ def test_our_arm_fox_workload(monkeypatch, capsys):
 def test_sweep_summary_from_a_committed_bench_line():
     sys.path.insert(0, os.path.join(ROOT, "tools"))
     import sweep
-    line = json.load(open(os.path.join(ROOT, "profiles", "r01_bench_full.json")))
+    line = json.load(open(os.path.join(ROOT, "tests", "golden", "bench_line_h100.json")))    # bench.py --gpus 1 --steps 1000, H100, this build
     row = sweep.summarise(18, 1, line)
     assert row["log2_target"] == 18 and row["gpus"] == 1 and abs(row["iters_per_s"] - line["iters_per_s"]) < 1e-9
     n = line["roofline"]["samples_per_launch"]
     assert abs(row["bwd_gbs"] - n * 1124 / (line["roofline"]["stage_ms"]["network_bwd"] * 1e-3) / 1e9) < 1e-6
-    assert abs(row["bwd_gbs"] - line["roofline"]["achieved"]) < 1e-3 * line["roofline"]["achieved"]      # the same number bench.py reports
+    assert abs(row["fwd_gbs"] - n * 624 / (line["roofline"]["stage_ms"]["network_fwd"] * 1e-3) / 1e9) < 1e-6
+    dom = {"network_fwd": "fwd_gbs", "network_bwd": "bwd_gbs"}[line["roofline"]["kernel"]]
+    assert abs(row[dom] - line["roofline"]["achieved"]) < 1e-3 * line["roofline"]["achieved"]      # the same number bench.py reports
     assert sweep.summarise(16, 2, {"error": "x" * 1000, "returncode": 1})["error"] == "x" * 300

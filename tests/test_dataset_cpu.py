@@ -11,6 +11,10 @@ import torch
 
 from jnerf_b200.plugin import dataset as D
 
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
+FOX_JSON = os.path.join(GOLDEN, "fox_transforms_train.json")       # data/fox/transforms_train.json of the reference capture, as shipped
+FOX_FRAMES = os.path.join(GOLDEN, "fox_small", "frames")            # the frames of that capture that exist on disk (reduced 6x)
+
 
 @pytest.fixture()
 def cpu_device(monkeypatch):
@@ -39,21 +43,6 @@ def check_against_json(ds, jd, root, n_expected):
     for k in (0, n_expected // 2, n_expected - 1):
         assert np.array_equal(xf[k], ref_nerf2ngp(frames[k]["transform_matrix"]))
     assert ds.image_data.shape == (n_expected, ds.H * ds.W, 4) and ds.image_data.dtype == torch.uint8
-
-
-def test_reference_fox_capture_loads(cpu_device):
-    root = "/root/reference/data/fox"
-    if not os.path.isdir(root):
-        pytest.skip("reference tree absent")
-    ds = D.NerfDataset(root, 4096, mode="train")
-    jd = json.load(open(os.path.join(root, "transforms_train.json")))
-    check_against_json(ds, jd, root, 50)                     # 67 frames listed, 50 on disk: missing files are skipped (dataset.py:103-107)
-    assert ds.aabb_scale == 4 and ds.resolution == [1080, 1920]
-    assert bool((ds.image_data[:, :, 3] == 255).all())       # JPEG frames: alpha filled with 1 (dataset.py:167-168)
-    pix = ds.next_pixels(4096)
-    assert pix.shape == (4096,) and int(pix.max()) < 50 * 1080 * 1920
-    rgba = ds.rgba_for(pix)
-    assert rgba.shape == (4096, 4) and float(rgba.max()) <= 1.0
 
 
 def test_blender_style_dataset(tmp_path, cpu_device):
@@ -95,15 +84,13 @@ def test_blender_style_dataset(tmp_path, cpu_device):
 def test_fox_stand_in_has_the_captures_numbers():
     """SyntheticNerfDataset(style='fox') takes its resolution / intrinsics / aabb / frame count from data/fox (BASELINE config #3)."""
     F = D.SyntheticNerfDataset.FOX
-    p = "/root/reference/data/fox/transforms_train.json"
-    if os.path.exists(p):
-        jd = json.load(open(p))
-        assert (F["W"], F["H"]) == (int(jd["w"]), int(jd["h"])) and F["fl"] == (jd["fl_x"], jd["fl_y"]) and F["c"] == (jd["cx"], jd["cy"])
-        assert F["aabb_scale"] == jd["aabb_scale"]
-        on_disk = [f for f in jd["frames"] if os.path.exists(os.path.join(os.path.dirname(p), f["file_path"]))]
-        assert F["n_images"] == len(on_disk)
-        dist = np.mean([np.linalg.norm(np.array(f["transform_matrix"])[:3, 3]) for f in jd["frames"]])
-        assert abs(F["radius"] - dist) < 0.05
+    jd = json.load(open(FOX_JSON))
+    assert (F["W"], F["H"]) == (int(jd["w"]), int(jd["h"])) and F["fl"] == (jd["fl_x"], jd["fl_y"]) and F["c"] == (jd["cx"], jd["cy"])
+    assert F["aabb_scale"] == jd["aabb_scale"]
+    on_disk = [f for f in jd["frames"] if os.path.exists(os.path.join(FOX_FRAMES, os.path.basename(f["file_path"])))]
+    assert F["n_images"] == len(on_disk)
+    dist = np.mean([np.linalg.norm(np.array(f["transform_matrix"])[:3, 3]) for f in jd["frames"]])
+    assert abs(F["radius"] - dist) < 0.05
     cams = D.synthetic_cameras(16, radius=F["radius"], azimuth=F["azimuth"], elevation=F["elevation"])
     for m in cams:
         pos = m[:3, 3]
@@ -174,7 +161,7 @@ def test_synthetic_datasets_construct_and_render(cpu_device, monkeypatch, style)
 
 def test_reduced_fox_capture_fixture(tmp_path, cpu_device):
     """tests/golden/fox_small: the reference's data/fox reduced 6x (make_fox_small.py), materialised in the reference's dataset layout
-    and read by NerfDataset -- the real-capture input of the GPU end-to-end test, which has no /root/reference to read."""
+    and read by NerfDataset -- the real-capture input of the GPU end-to-end test."""
     import sys
     sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden"))
     from make_fox_small import materialise
@@ -185,12 +172,10 @@ def test_reduced_fox_capture_fixture(tmp_path, cpu_device):
     check_against_json(ds, jd, root, 50)
     assert ds.resolution == [180, 320] and ds.aabb_scale == 4 and bool((ds.image_data[:, :, 3] == 255).all())
     assert D.NerfDataset(root, 4096, mode="test", preload_shuffle=False).n_images == 2
-    ref = "/root/reference/data/fox/transforms_train.json"
-    if os.path.exists(ref):                                          # same poses as the capture, intrinsics scaled by the reduction
-        rj = json.load(open(ref))
-        assert [f["file_path"] for f in rj["frames"]] == [f["file_path"] for f in jd["frames"]]
-        assert np.array_equal(np.array([f["transform_matrix"] for f in rj["frames"]]), np.array([f["transform_matrix"] for f in jd["frames"]]))
-        for k in ("fl_x", "fl_y", "cx", "cy"):
-            assert abs(jd[k] * 6 - rj[k]) < 1e-9
-        assert jd["aabb_scale"] == rj["aabb_scale"] and (jd["w"], jd["h"]) == (rj["w"] // 6, rj["h"] // 6)
+    rj = json.load(open(FOX_JSON))                                   # same poses as the capture, intrinsics scaled by the reduction
+    assert [f["file_path"] for f in rj["frames"]] == [f["file_path"] for f in jd["frames"]]
+    assert np.array_equal(np.array([f["transform_matrix"] for f in rj["frames"]]), np.array([f["transform_matrix"] for f in jd["frames"]]))
+    for k in ("fl_x", "fl_y", "cx", "cy"):
+        assert abs(jd[k] * 6 - rj[k]) < 1e-9
+    assert jd["aabb_scale"] == rj["aabb_scale"] and (jd["w"], jd["h"]) == (rj["w"] // 6, rj["h"] // 6)
     assert float(ds.image_data[:, :, :3].float().std()) > 20         # photographs, not blanks

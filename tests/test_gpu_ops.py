@@ -1,4 +1,4 @@
-"""Parity tests proper: every C-ABI operator of libngp_b200.so (sm_100a) against the oracle on identical seeded
+"""Parity tests proper: every C-ABI operator of libngp_b200.so (sm_90a) against the oracle on identical seeded
 inputs, and against the committed golden vectors.  Integer / index outputs (march, compaction, bitfields, sample
 indices) must be bit-exact; floating point is checked at the tolerance stated beside each assert
 (north_star: fp16/fp32 radiance within 1e-3 relative)."""
@@ -173,7 +173,7 @@ def test_mlp_fwd_bwd(ops, nhm, n):
     assert np.abs(npy(temps).astype(np.float32) - tempsr.astype(np.float32)).max() <= 3e-3
     assert np.abs(npy(dX).astype(np.float32) - dXr.astype(np.float32)).max() <= 3e-3
     dWg = npy(dW)
-    assert np.abs(dWg - dWr).max() <= 2e-3 * max(1.0, np.abs(dWr).max())      # fp32 TMEM accumulation vs float64
+    assert np.abs(dWg - dWr).max() <= 2e-3 * max(1.0, np.abs(dWr).max())      # fp32 register accumulation vs float64
     off = 64 * 32 + nhm * 64 * 64
     assert (dWg[off + n_valid * 64:] == 0).all()
 

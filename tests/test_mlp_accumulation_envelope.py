@@ -1,12 +1,9 @@
 """The reference defines its MLP twice: the prebuilt tiny-cuda-nn object (fp16 accumulators: every tensor instruction in
-fully_fused_mlp_function.o is HMMA.*.F16 -- checked below when the file is present) and the nn.Linear fallback
+fully_fused_mlp_function.o is HMMA.*.F16) and the nn.Linear fallback
 (models/networks/ngp_network.py:59-67, wide accumulation).  The oracle and the CUDA kernels follow the second.  This test restates
 the first as a numerical MODEL (fp16 rounding of the accumulator after every 16-wide K block) and measures how far apart the two
 definitions are on NGP-shaped inputs: that distance is the floor under any float tolerance for R7, and the tolerance the GPU
 parity tests use (6e-3 absolute on O(1) outputs, tests/test_gpu_ops.py) sits above it."""
-import os
-import subprocess
-
 import numpy as np
 
 import oracle_lib as ol
@@ -41,16 +38,3 @@ def test_distance_between_the_references_two_mlp_definitions():
         assert d.max() <= 6e-3 * max(1.0, scale), (d.max(), scale)
         assert d.max() > 0, "an fp16 accumulator must differ somewhere"
         assert d.mean() <= 1e-3
-
-
-def test_reference_binary_uses_fp16_accumulators():
-    obj = "/root/reference/python/jnerf/ops/code_ops/op_header/fully_fused_mlp_function.o"
-    if not os.path.exists(obj):
-        import pytest
-        pytest.skip("reference tree absent")
-    sass = subprocess.run(["cuobjdump", "-sass", obj], capture_output=True, text=True).stdout
-    import re
-    kinds = set(re.findall(r"HMMA\.[0-9]+\.(F16|F32)", sass))
-    assert kinds == {"F16"}, kinds
-    assert "kernel_mlp_fusedILi64ELi8E6__halfL10Activation0ELb0EE" in sass and "kernel_mlp_fused_backwardILi64ELi8EL10Activation0E" in sass
-    assert set(re.findall(r"arch = (sm_\d+)", sass)) == {"sm_75", "sm_80", "sm_86"}          # nothing a B200 can load

@@ -1,14 +1,60 @@
 """Pins the C restatement (oracle/ngp_oracle.c) against the reference's own kernel sources executed on the host
-(oracle/_ref, built by `make -C oracle ref` from /root/reference through ref_shim/shim.h).  Runs only where the
-_ref build exists (this container); the committed goldens (tests/golden) carry the same pins to the GPU box.
+(oracle/_ref, built by `make -C oracle ref` from the reference tree through ref_shim/shim.h).
 Integer / index outputs must be bit-exact; float outputs are bit-exact too in host-shim arithmetic (fma_mode 0)
-except where libm expf replaces the device intrinsic identically on both sides."""
+except where libm expf replaces the device intrinsic identically on both sides.
+
+The reference's outputs for these inputs are stored in tests/golden/ref_pins.npz, so the comparison runs everywhere.  Where
+oracle/_ref exists they are also recomputed and must equal the stored ones; NGP_WRITE_REF_PINS=1 rewrites the file from such a run.
+Arrays above 64 KB are stored as their SHA-256 (every comparison here is exact)."""
+import hashlib
+import os
+
 import numpy as np
 import pytest
 import oracle_lib as ol
 
-pytestmark = pytest.mark.skipif(ol.ref("ref_hash_cpu") is None or ol.ref("ref_sampler_cpu_constdt") is None,
-                                reason="oracle/_ref not built (reference tree absent)")
+PINS_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "ref_pins.npz")
+PINS = dict(np.load(PINS_PATH)) if os.path.exists(PINS_PATH) else {}
+LIVE = ol.ref("ref_hash_cpu") is not None and ol.ref("ref_sampler_cpu_constdt") is not None
+_NEW = {}
+
+
+def _stored(a):
+    a = np.ascontiguousarray(a)
+    if a.nbytes <= 1 << 16:
+        return a
+    return np.frombuffer(hashlib.sha256(a.tobytes()).digest(), np.uint8).copy()
+
+
+def pinned(key, compute):
+    """The reference's output(s) for `key`: computed by `compute()` with oracle/_ref where it exists (and checked against the stored
+    pin), the stored pin otherwise.  Returns a tuple of arrays; a hashed array comes back as its digest (compare with `same`)."""
+    if LIVE:
+        vals = tuple(np.asarray(v) for v in compute())
+        for i, v in enumerate(vals):
+            _NEW[f"{key}.{i}"] = _stored(v)
+            if f"{key}.{i}" in PINS and os.environ.get("NGP_WRITE_REF_PINS") != "1":
+                assert np.array_equal(_stored(v), PINS[f"{key}.{i}"]), f"stored reference pin {key}.{i} is stale"
+        return vals
+    n = len([k for k in PINS if k.rsplit(".", 1)[0] == key])
+    assert n, f"no stored reference pin {key} and no oracle/_ref build"
+    return tuple(PINS[f"{key}.{i}"] for i in range(n))
+
+
+def same(a, ref):
+    """Exact equality with a reference output that may be stored as a SHA-256."""
+    a = np.ascontiguousarray(a)
+    ref = np.asarray(ref)
+    if a.nbytes > 1 << 16 and ref.dtype == np.uint8 and ref.size == 32 and a.nbytes != 32:
+        return np.array_equal(_stored(a), ref)
+    return a.shape == ref.shape and np.array_equal(a.view(np.uint8), np.ascontiguousarray(ref, a.dtype).view(np.uint8))
+
+
+@pytest.fixture(scope="module", autouse=True)
+def write_pins():
+    yield
+    if LIVE and os.environ.get("NGP_WRITE_REF_PINS") == "1":
+        np.savez_compressed(PINS_PATH, **dict(PINS, **_NEW))
 
 
 @pytest.fixture(autouse=True)
@@ -19,20 +65,24 @@ def host_arith():
 
 
 def test_pcg32_kat():
-    r = ol.ref("ref_sampler_cpu_constdt")
+    def compute():
+        r = ol.ref("ref_sampler_cpu_constdt")
+        si_ref = np.zeros(2, np.uint64)
+        r.ref_pcg32_seed_constdt(ol._u64(1337), ol._ptr(si_ref))
+        adv = si_ref.copy()
+        r.ref_pcg32_advance_constdt(ol._ptr(adv), ol._i64(1 << 32))
+        return si_ref, adv
+    si_ref, adv_ref = pinned("pcg32", compute)
     si = ol.pcg32_seed(1337)
-    si_ref = np.zeros(2, np.uint64)
-    r.ref_pcg32_seed_constdt(ol._u64(1337), ol._ptr(si_ref))
     assert (si == si_ref).all()
     assert int(si[0]) == 0x4cfa1d1cde85af8f and int(si[1]) == 3          # SURVEY.md section 8c KAT
     f1 = ol.oracle().orc_pcg32_next_float(ol._ptr(si))
     f2 = ol.oracle().orc_pcg32_next_float(ol._ptr(si))
     # values as produced by the reference pcg32 itself (SURVEY.md 8c lists the same two numbers in swapped order)
     assert abs(f1 - 0.147699356) < 1e-8 and abs(f2 - 0.471029401) < 1e-8
-    a, b = ol.pcg32_seed(1337), ol.pcg32_seed(1337)
+    a = ol.pcg32_seed(1337)
     ol.pcg32_advance(a, 1 << 32)
-    r.ref_pcg32_advance_constdt(ol._ptr(b), ol._i64(1 << 32))
-    assert (a == b).all()
+    assert (a == adv_ref).all()
 
 
 @pytest.mark.parametrize("aabb,log2T", [(1, 14), (1, 19), (4, 19)])
@@ -53,14 +103,14 @@ def test_hash_fwd_bwd(dtype, log2T):
     x[0] = 0.0
     x[1] = 1.0                                     # the corner cases that hit index == resolution
     grid = np.random.default_rng(1).uniform(-1e-4, 1e-4, cfg.n_params).astype(dtype)
-    out_ref, pos_soa = ol.ref_hash_fwd(cfg, x, grid)
-    out = ol.hash_fwd(cfg, x, grid)
-    assert np.array_equal(out.view(np.uint16 if dtype == np.float16 else np.uint32),
-                          out_ref.view(np.uint16 if dtype == np.float16 else np.uint32))
     dy = (rng.standard_normal((n, 32)) * 1e-2).astype(dtype)
-    g_ref = ol.ref_hash_bwd(cfg, pos_soa, dy)
-    g = ol.hash_bwd(cfg, x, dy)
-    assert np.array_equal(g, g_ref)
+
+    def compute():
+        out_ref, pos_soa = ol.ref_hash_fwd(cfg, x, grid)
+        return out_ref, ol.ref_hash_bwd(cfg, pos_soa, dy)
+    out_ref, g_ref = pinned(f"hash_{np.dtype(dtype).name}_{log2T}", compute)
+    assert same(ol.hash_fwd(cfg, x, grid), out_ref)
+    assert same(ol.hash_bwd(cfg, x, dy), g_ref)
 
 
 def test_hash_kat():
@@ -72,12 +122,15 @@ def test_hash_kat():
 
 @pytest.mark.parametrize("dtype", [np.float32, np.float16])
 def test_sh(dtype):
-    r = ol.ref("ref_sampler_cpu_constdt")
     d = np.random.default_rng(3).random((257, 3), dtype=np.float32)
-    out_ref = np.empty((257, 16), dtype)
-    (r.ref_sh_f32_constdt if dtype == np.float32 else r.ref_sh_f16_constdt)(ol._u32(257), ol._ptr(d), ol._ptr(out_ref))
-    out = ol.sh(d, dtype)
-    assert np.array_equal(out, out_ref)
+
+    def compute():
+        r = ol.ref("ref_sampler_cpu_constdt")
+        out_ref = np.empty((257, 16), dtype)
+        (r.ref_sh_f32_constdt if dtype == np.float32 else r.ref_sh_f16_constdt)(ol._u32(257), ol._ptr(d), ol._ptr(out_ref))
+        return (out_ref,)
+    (out_ref,) = pinned(f"sh_{np.dtype(dtype).name}", compute)
+    assert same(ol.sh(d, dtype), out_ref)
 
 
 @pytest.mark.parametrize("const_dt", [True, False])
@@ -86,25 +139,31 @@ def test_march_compact(const_dt):
     o, d = ol.random_rays(300, seed=5)
     aabb = (0.0, 1.0) if const_dt else (-1.5, 2.5)
     a = ol.march(o, d, bits, aabb=aabb, const_dt=const_dt, max_samples=300 * 1024)
-    b = ol.ref_march(o, d, bits, aabb=aabb, const_dt=const_dt, max_samples=300 * 1024)
+    S = int(a[3][1])
+    cap = S - 777                                                      # force truncation
+
+    def compute():
+        b = ol.ref_march(o, d, bits, aabb=aabb, const_dt=const_dt, max_samples=300 * 1024)
+        out = [b[0][:int(b[3][1])], b[1], b[2], b[3]]
+        if const_dt:
+            out += list(ol.ref_compact(b[0], b[2], cap))
+        return out
+    b = pinned(f"march_{int(const_dt)}", compute)
     assert (a[3] == b[3]).all() and a[3][1] > 1000
     assert np.array_equal(a[2], b[2])                                  # numsteps + base, ray order
-    S = int(a[3][1])
-    assert np.array_equal(a[0][:S].view(np.uint32), b[0][:S].view(np.uint32))   # sample coords bit-exact
+    assert same(a[0][:S], b[0])                                        # sample coords bit-exact
     assert np.array_equal(a[1], b[1])
     if const_dt:
-        cap = S - 777                                                  # force truncation
         ca = ol.compact(a[0], a[2], cap)
-        cb = ol.ref_compact(b[0], b[2], cap)
-        assert np.array_equal(ca[0], cb[0]) and np.array_equal(ca[1], cb[1]) and (ca[2] == cb[2]).all()
+        assert same(ca[0], b[4]) and same(ca[1], b[5]) and (ca[2] == b[6]).all()
 
 
 def test_march_overflow():
     bits, _ = ol.sphere_bitfield(0.3)
     o, d = ol.random_rays(64, seed=6)
     a = ol.march(o, d, bits, max_samples=2000)
-    b = ol.ref_march(o, d, bits, max_samples=2000)
-    assert np.array_equal(a[2], b[2]) and (a[3] == b[3]).all()
+    b = pinned("march_overflow", lambda: ol.ref_march(o, d, bits, max_samples=2000)[2:4])
+    assert np.array_equal(a[2], b[0]) and (a[3] == b[1]).all()
     assert (a[2][:, 0] == 0).any()
 
 
@@ -119,18 +178,16 @@ def test_composite(dtype):
     net = rng.standard_normal((S - 100, 4)).astype(dtype)
     bg = rng.random((200, 3), dtype=np.float32)
     lg = (rng.standard_normal((200, 3))).astype(np.float32)
-    rgb_ref, dnet_ref, rgbi_ref, alpha_ref = ol.ref_composite(net, cc, numsteps, ns_c, bg, lg, mean=0.001)
+    rgb_ref, dnet_ref, rgbi_ref, alpha_ref = pinned(f"composite_{np.dtype(dtype).name}",
+                                                    lambda: ol.ref_composite(net, cc, numsteps, ns_c, bg, lg, mean=0.001))
     rgb = ol.composite_fwd(net, cc, numsteps, ns_c, bg)
-    np.testing.assert_array_equal(rgb, rgb_ref)
-    dnet = ol.composite_bwd(net, cc, ns_c, lg, rgb, 0.001)
-    np.testing.assert_array_equal(dnet, dnet_ref)
+    assert same(rgb, rgb_ref)
+    assert same(ol.composite_bwd(net, cc, ns_c, lg, rgb, 0.001), dnet_ref)
     rgbi, alpha = ol.composite_infer(net, cc, ns_c)
-    np.testing.assert_array_equal(rgbi, rgbi_ref)
-    np.testing.assert_array_equal(alpha, alpha_ref)
+    assert same(rgbi, rgbi_ref) and same(alpha, alpha_ref)
 
 
 def test_grid_update():
-    r = ol.ref("ref_sampler_cpu_constdt")
     n_img = 7
     rng = np.random.default_rng(9)
     # cameras on a sphere looking at the centre, column-major 3x4
@@ -143,31 +200,49 @@ def test_grid_update():
         xf[j] = np.concatenate([xc, yc, zc, pos]).astype(np.float32)
     focal = np.full((n_img, 2), 1100.0, np.float32)
     n_el = ol.G3 * 5
-    g_a = np.zeros(n_el, np.float32); g_b = np.zeros(n_el, np.float32)
+    g_a = np.zeros(n_el, np.float32)
     ol.mark_untrained(g_a, focal, xf, (800, 800))
-    r.ref_mark_untrained_constdt(ol._u32(n_el), ol._ptr(g_b), ol._u32(n_img), ol._ptr(focal), ol._ptr(xf), ol._i32(800), ol._i32(800))
-    assert np.array_equal(g_a, g_b) and (g_a < 0).any() and (g_a == 0).any()
     si = ol.pcg32_seed()
+    n = 20000
+    runs = []
     for thresh, step, casc in [(-0.01, 0, 1), (0.01, 3, 3)]:
-        n = 20000
         g_in = np.where(rng.random(n_el) < 0.3, rng.random(n_el) * 0.05, -1.0).astype(np.float32)
         pa, ia = ol.generate_grid_samples(n, si, step, (-1.5, 2.5), g_in, casc, thresh)
-        pb = np.empty((n, 3), np.float32); ib = np.empty(n, np.uint32)
-        r.ref_generate_grid_samples_constdt(ol._u32(n), ol._u64(int(si[0])), ol._u64(int(si[1])), ol._u32(step), ol._f32(-1.5), ol._f32(2.5),
-                                            ol._ptr(g_in), ol._ptr(pb), ol._ptr(ib), ol._u32(casc), ol._f32(thresh))
-        assert np.array_equal(ia, ib) and np.array_equal(pa, pb)
+        runs.append((thresh, step, casc, int(si[0]), int(si[1]), g_in, pa, ia))
+    mlps, tas = [], []
     for dt in (np.float32, np.float16):
-        mlp = rng.standard_normal(n).astype(dt)
-        ta = np.zeros(n_el, np.float32); tb = np.zeros(n_el, np.float32)
-        ol.splat(ia, mlp, ta)
-        (r.ref_splat_f32_constdt if dt == np.float32 else r.ref_splat_f16_constdt)(ol._u32(n), ol._ptr(ia), ol._ptr(mlp), ol._ptr(tb))
-        assert np.array_equal(ta, tb)
-    ga, gb = g_in.copy(), g_in.copy()
-    ol.ema(ga, ta)
-    r.ref_ema_constdt(ol._u32(n_el), ol._f32(0.95), ol._ptr(gb), ol._ptr(tb))
-    assert np.array_equal(ga, gb)
+        mlps.append(rng.standard_normal(n).astype(dt))
+        tas.append(np.zeros(n_el, np.float32))
+        ol.splat(ia, mlps[-1], tas[-1])
+    ga = g_in.copy()
+    ol.ema(ga, tas[-1])
     mean = ol.grid_mean(ga)
     ba = ol.update_bitfield(ga, mean)
-    bb = np.zeros_like(ba)
-    r.ref_update_bitfield_constdt(ol._ptr(gb), ol._ptr(np.array([mean], np.float32)), ol._ptr(bb))
-    assert np.array_equal(ba, bb) and ba.any()
+
+    def compute():
+        r = ol.ref("ref_sampler_cpu_constdt")
+        g_b = np.zeros(n_el, np.float32)
+        r.ref_mark_untrained_constdt(ol._u32(n_el), ol._ptr(g_b), ol._u32(n_img), ol._ptr(focal), ol._ptr(xf), ol._i32(800), ol._i32(800))
+        out = [g_b]
+        for thresh, step, casc, s0, s1, g_in_, _, _ in runs:
+            pb = np.empty((n, 3), np.float32); ib = np.empty(n, np.uint32)
+            r.ref_generate_grid_samples_constdt(ol._u32(n), ol._u64(s0), ol._u64(s1), ol._u32(step), ol._f32(-1.5), ol._f32(2.5),
+                                                ol._ptr(g_in_), ol._ptr(pb), ol._ptr(ib), ol._u32(casc), ol._f32(thresh))
+            out += [pb, ib]
+        for mlp in mlps:
+            tb = np.zeros(n_el, np.float32)
+            (r.ref_splat_f32_constdt if mlp.dtype == np.float32 else r.ref_splat_f16_constdt)(ol._u32(n), ol._ptr(ia), ol._ptr(mlp), ol._ptr(tb))
+            out.append(tb)
+        gb = g_in.copy()
+        r.ref_ema_constdt(ol._u32(n_el), ol._f32(0.95), ol._ptr(gb), ol._ptr(out[-1]))
+        bb = np.zeros_like(ba)
+        r.ref_update_bitfield_constdt(ol._ptr(gb), ol._ptr(np.array([mean], np.float32)), ol._ptr(bb))
+        return out + [gb, bb]
+    ref = pinned("grid_update", compute)
+    assert same(g_a, ref[0]) and (g_a < 0).any() and (g_a == 0).any()
+    for k, (_, _, _, _, _, _, pa, ia_) in enumerate(runs):
+        assert same(ia_, ref[2 + 2 * k]) and same(pa, ref[1 + 2 * k])
+    for k, ta in enumerate(tas):
+        assert same(ta, ref[5 + k])
+    assert same(ga, ref[7])
+    assert same(ba, ref[8]) and ba.any()

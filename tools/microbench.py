@@ -9,7 +9,7 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from jnerf_b200 import ops  # noqa: E402
 
-PEAKS = {"hbm_gbs": 6582.5, "bf16_tflops": 1683.9}
+PEAKS = {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}                         # H100 SXM data sheet; MEASURED_PEAKS.json overrides
 try:
     PEAKS.update(json.load(open(os.path.join(os.path.dirname(__file__), "..", "MEASURED_PEAKS.json"))))
 except Exception:
@@ -38,7 +38,7 @@ def main():
     N = int(sys.argv[1]) if len(sys.argv) > 1 else 262144
     dev = "cuda"
     torch.manual_seed(0)
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)     # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)     # > 50 MB L2
     lv = ops.HashLevels(1)
     grid = (torch.rand(lv.n_params, device=dev) * 2e-4 - 1e-4).half()
     x = torch.rand(N, 3, device=dev)

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""SURVEY.md 8d(ii): the reference's own kernels, compiled UNMODIFIED for sm_100a with the reference's launch shapes
-(oracle/_ref/libref_gpu_constdt.so, recipe oracle/Makefile), timed and compared against this library on the same B200 and the
+"""SURVEY.md 8d(ii): the reference's own kernels, compiled UNMODIFIED for sm_90a with the reference's launch shapes
+(oracle/_ref/libref_gpu_constdt.so, recipe oracle/Makefile), timed and compared against this library on the same H100 and the
 same inputs -- "the kernel to beat" for R2, R3, R6, R8, R9.
 
     python tools/ref_gpu_compare.py [--steps 300] [--out gpurun_out/ref_gpu_compare.json]
@@ -80,7 +80,7 @@ def main():
         r.train_step()
     torch.cuda.synchronize()
     s, m, ds = r.sampler, r.model, r.dataset["train"]
-    res = {"config": f"lego stand-in after {args.steps} steps; reference kernels = oracle/_ref/libref_gpu_constdt.so (unmodified sources, sm_100a, reference launch shapes)",
+    res = {"config": f"lego stand-in after {args.steps} steps; reference kernels = oracle/_ref/libref_gpu_constdt.so (unmodified sources, sm_90a, reference launch shapes)",
            "unit": "us (median of 15)"}
 
     def section(name, fn):
@@ -199,7 +199,7 @@ def main():
         return {"samples": N,
                 "ours_fused_hash+SH+both_MLPs_forward_us": timeit(lambda: ops.network_fwd(coords, grid, lv, wd, wr, n_dev=cnt_c[0:1], out=net, enc=enc)),
                 "ours_fused_MLP_backward+hash_scatter_us": timeit(lambda: ops.network_bwd(coords, enc, lv, wd, wr, dnet, gg, dwd, dwr, n_dev=cnt_c[0:1])),
-                "note": "the reference's MLP exists only as sm_75/80/86 SASS and cannot run on sm_100; compare against its hash kernels alone above"}
+                "note": "the reference's MLP exists only as sm_75/80/86 SASS and cannot run on sm_90; compare against its hash kernels alone above"}
 
     section("fused network (R2+R4+R7 / R7+R3)", fused_section)
 
