@@ -105,6 +105,31 @@ int ngp_network_bwd(void* stream, uint32_t n_max, const uint32_t* n_dev, const f
 int ngp_density_fwd(void* stream, uint32_t n, const float* pos, const void* grid, const void* levels_dev,
                     const void* w_density, void* sigma_out);
 
+/* ---- M1-M4  mesh extraction (tools/extract_mesh.py of the reference: a trained model -> mesh-origin.ply / mesh-color.ply) --------
+ * Resolution n must be in [2, 1024]; vertices are (V,3) f32, triangles (T,3) int32 (V, T < 2^31); counts are 64-bit.
+ * workspace: *bytes_out of ngp_mesh_workspace_bytes(n, 0, 0, .) for ngp_marching_cubes, of (0, V, T, .) for the other two.
+ * Every result is bit-reproducible (fixed numbering, fixed summation order; DESIGN.md section 4 "Mesh extraction"). */
+int ngp_mesh_workspace_bytes(uint32_t n, uint64_t n_verts, uint64_t n_tris, uint64_t* bytes_out);
+/* M1: the n^3 density lattice of extract_mesh.py:42-70 -- row (i*n + j)*n + k at model position (i, j, k)/(n-1) (the unit cube, not the
+ * aabb), field_out[row] = float(int(max(sigma_raw, 0))) (:68).  Positions are made in the kernel (no coordinate buffer); sigma_raw is
+ * bit-identical to ngp_density_fwd at the same positions. */
+int ngp_density_lattice(void* stream, uint32_t n, const void* grid, const void* levels_dev, const void* w_density, float* field_out);
+/* M2: mcubes.marching_cubes(sigma, iso) + the vertex frame of :78-84 (lattice position / n, first two columns swapped).  A vertex per
+ * lattice edge whose endpoints straddle iso (inside: value > iso), numbered in lattice-edge order; triangles in cell order, their
+ * right-hand normals pointing towards lower values in the written frame.  counts_host[0..1] = vertices, triangles, read back once.
+ * verts = tris = NULL: count only (call again with buffers of at least those sizes). */
+int ngp_marching_cubes(void* stream, uint32_t n, const float* field, float iso, void* workspace, float* verts, uint64_t max_verts,
+                       int32_t* tris, uint64_t max_tris, uint64_t* counts_host);
+/* M3: Open3D cluster_connected_triangles + argmax + remove_triangles_by_index + remove_unreferenced_vertices (:92-97): the largest set of
+ * triangles joined through shared edges (a tie keeps the set holding the lowest triangle), triangles and vertices compacted in order.
+ * verts_out (n_verts,3) / tris_out (n_tris,3) capacities; counts_host[0..1] = kept vertices, kept triangles (synchronises). */
+int ngp_mesh_largest_component(void* stream, uint64_t n_verts, uint64_t n_tris, const float* verts, const int32_t* tris, void* workspace,
+                               float* verts_out, int32_t* tris_out, uint64_t* counts_host);
+/* M4: Open3D compute_vertex_normals (:106): per vertex the sum of its triangles' (v1-v0)x(v2-v0) in triangle order, normalised (a zero
+ * sum stays zero).  normals (n_verts,3). */
+int ngp_mesh_vertex_normals(void* stream, uint64_t n_verts, uint64_t n_tris, const float* verts, const int32_t* tris, void* workspace,
+                            float* normals);
+
 /* ---- R6  ray march (DGS/ray_sampler.py:20-72 -> DGS/op_header/ray_sampler.h:4-114) -------------------
  * counters[0] = rays accepted, counters[1] = total samples (both zeroed here, ray_sampler.py:29).
  * numsteps (R,2) = {count, base}; base is the exclusive prefix sum in RAY ORDER (deterministic; the reference

@@ -142,11 +142,22 @@ __device__ __forceinline__ void sh_to_slab(uint8_t* act, const float* s_coords, 
 constexpr int FWD_GW = 8;
 constexpr int FWD_THREADS = 128 + 32 * FWD_GW;
 
-template <bool DENSITY_ONLY>
+// Lattice mode (LATTICE, density only; extract_mesh.py:42-70): row r = (i*N + j)*N + k is the model position (i, j, k) / (N-1), made by
+// the gather warps from the row index instead of staged from `coords`, and the epilogue writes float(int(max(sigma_raw, 0)))
+// (extract_mesh.py:68) as fp32 into `out`.  The positions are IEEE quotients, so a coordinate buffer holding the same values gives the
+// same sigma_raw bit for bit.
+__device__ __forceinline__ float lattice_coord(uint32_t r, uint32_t axis, uint32_t n) {
+    const uint32_t idx = axis == 0 ? r / (n * n) : axis == 1 ? (r / n) % n : r % n;
+    return __fdiv_rn((float)idx, (float)(n - 1));
+}
+
+template <bool DENSITY_ONLY, bool LATTICE = false>
 __global__ void __launch_bounds__(FWD_THREADS, 2)   // two CTAs per SM: <= 85 registers per thread
 network_fwd_kernel(uint32_t n_max, const uint32_t* __restrict__ n_dev, const float* __restrict__ coords, const __half* __restrict__ grid,
                    const NgpLevel* __restrict__ levels, const __half* __restrict__ wd, const __half* __restrict__ wr,
-                   __half* __restrict__ out, __half* __restrict__ enc_save, const __grid_constant__ NgpTensorMap enc_map, uint32_t enc_tma) {
+                   __half* __restrict__ out, __half* __restrict__ enc_save, const __grid_constant__ NgpTensorMap enc_map, uint32_t enc_tma,
+                   uint32_t lattice_n) {
+    static_assert(DENSITY_ONLY || !LATTICE, "the lattice query is density only");
     // enc_tma: the encoded-feature rows kept for the backward pass leave the SM as four TMA tensor stores per tile, straight from the
     // slab the gather warps fill (one 8-column x 128-row box per feature group), instead of 16 four-byte global stores per row from the
     // gather warps -- which are the LSU-bound side of this kernel.  enc_save is then only the base address the tensor map was built for.
@@ -201,7 +212,9 @@ network_fwd_kernel(uint32_t n_max, const uint32_t* __restrict__ n_dev, const flo
 #pragma unroll
                     for (uint32_t i = 0; i < 4; ++i) {
                         const uint32_t row = tile * ROWS + 64 * (i >> 1) + r0 + 8 * (i & 1);
-                        if (row < n_live) reinterpret_cast<uint16_t*>(out)[row] = sig[i];
+                        if (row >= n_live) continue;
+                        if constexpr (LATTICE) reinterpret_cast<float*>(out)[row] = truncf(fmaxf(__half2float(__ushort_as_half(sig[i])), 0.f));
+                        else reinterpret_cast<uint16_t*>(out)[row] = sig[i];
                     }
                 }
             } else {
@@ -231,8 +244,10 @@ network_fwd_kernel(uint32_t n_max, const uint32_t* __restrict__ n_dev, const flo
             const uint32_t buf = it & 1, row0 = tile * ROWS;
             float* s_coords = reinterpret_cast<float*>(smem + S::coords + buf * 3584);
             if (it >= 2) named_bar_sync(4 + buf, FWD_THREADS);          // EMPTY[buf]: the chain of tile it-2 is done with this buffer
-            for (uint32_t i = tg; i < ROWS * CS; i += 32 * FWD_GW)       // stage the coordinate tile (coalesced)
-                s_coords[i] = (row0 + i / CS < n_live) ? __ldg(coords + (size_t)row0 * CS + i) : 0.f;
+            for (uint32_t i = tg; i < ROWS * CS; i += 32 * FWD_GW) {     // stage the coordinate tile (coalesced)
+                if constexpr (LATTICE) s_coords[i] = (row0 + i / CS < n_live) ? lattice_coord(row0 + i / CS, i % CS, lattice_n) : 0.f;
+                else s_coords[i] = (row0 + i / CS < n_live) ? __ldg(coords + (size_t)row0 * CS + i) : 0.f;
+            }
             named_bar_sync(6, 32 * FWD_GW);
             gather_tile<CS, 64 / FWD_GW>(s_coords, lv, g, smem + S::act, buf ? G_ENC1 : G_ENC, level, sub, (DENSITY_ONLY || enc_tma) ? nullptr : enc_save, row0,
                                          n_live);
@@ -634,7 +649,7 @@ int ngp_network_fwd(void* stream, uint32_t n_max, const uint32_t* n_dev, const f
     const uint32_t enc_tma = (!no_tma && enc_save && ngp_make_rows32_tensormap(&enc_map, enc_save, n_max)) ? 1u : 0u;
     network_fwd_kernel<false><<<grid_dim, FWD_THREADS, SmemFwd::total, s>>>(n_max, n_dev, coords, (const __half*)grid, (const NgpLevel*)levels_dev,
                                                                    (const __half*)w_density, (const __half*)w_rgb, (__half*)out,
-                                                                   (__half*)enc_save, enc_map, enc_tma);
+                                                                   (__half*)enc_save, enc_map, enc_tma, 0u);
     NGP_LAUNCH_CHECK();
     return 0;
 }
@@ -646,7 +661,21 @@ int ngp_density_fwd(void* stream, uint32_t n, const float* pos, const void* grid
     const uint32_t ntiles = (n + ROWS - 1) / ROWS;
     const uint32_t grid_dim = min(ntiles, (uint32_t)ngp_num_sms() * 2u);
     network_fwd_kernel<true><<<grid_dim, FWD_THREADS, SmemFwd::total, s>>>(n, nullptr, pos, (const __half*)grid, (const NgpLevel*)levels_dev,
-                                                                  (const __half*)w_density, nullptr, (__half*)sigma_out, nullptr, NgpTensorMap{}, 0u);
+                                                                  (const __half*)w_density, nullptr, (__half*)sigma_out, nullptr, NgpTensorMap{}, 0u, 0u);
+    NGP_LAUNCH_CHECK();
+    return 0;
+}
+
+int ngp_density_lattice(void* stream, uint32_t n, const void* grid, const void* levels_dev, const void* w_density, float* field_out) {
+    NGP_REQUIRE(n >= 2 && n <= 1024, "ngp_density_lattice: resolution n must be in [2, 1024], got " + std::to_string(n));
+    cudaStream_t s = (cudaStream_t)stream;
+    if (ngp_first_use((const void*)network_fwd_kernel<true, true>))
+        NGP_CHECK_CUDA(cudaFuncSetAttribute(network_fwd_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SmemFwd::total));
+    const uint32_t n3 = n * n * n, ntiles = (n3 + ROWS - 1) / ROWS;
+    const uint32_t grid_dim = min(ntiles, (uint32_t)ngp_num_sms() * 2u);
+    network_fwd_kernel<true, true><<<grid_dim, FWD_THREADS, SmemFwd::total, s>>>(n3, nullptr, nullptr, (const __half*)grid, (const NgpLevel*)levels_dev,
+                                                                                (const __half*)w_density, nullptr, reinterpret_cast<__half*>(field_out),
+                                                                                nullptr, NgpTensorMap{}, 0u, n);
     NGP_LAUNCH_CHECK();
     return 0;
 }

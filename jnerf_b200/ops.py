@@ -121,6 +121,63 @@ def density_fwd(pos, grid, levels, wd):
     return out
 
 
+# ---- mesh extraction (include/ngp_b200.h M1-M4; tools/extract_mesh.py of the reference) ----
+def _mesh_workspace(device, n=0, n_verts=0, n_tris=0):
+    b = np.zeros(1, np.uint64)
+    lib.call("ngp_mesh_workspace_bytes", int(n), int(n_verts), int(n_tris), b.ctypes.data)
+    return torch.empty(max(int(b[0]), 1), dtype=torch.uint8, device=device)
+
+
+def density_lattice(n, grid, levels, wd):
+    """The (n, n, n) fp32 field float(int(max(sigma_raw, 0))) at model positions (i, j, k) / (n-1)."""
+    if not 2 <= int(n) <= 1024:
+        raise lib.NgpError(f"density_lattice: resolution {n} is outside [2, 1024]")
+    field = torch.empty((n, n, n), dtype=torch.float32, device=grid.device)
+    lib.call("ngp_density_lattice", _stream(), int(n), _p(grid), _p(levels.table), _p(wd), _p(field))
+    return field
+
+
+def marching_cubes(field, iso=0.5, workspace=None):
+    """(n, n, n) fp32 field -> vertices (V, 3) f32 in the PLY frame, triangles (T, 3) int32.  One read-back of the counts per call."""
+    import ctypes
+    n = field.shape[0]
+    assert field.dim() == 3 and field.shape == (n, n, n) and field.dtype == torch.float32
+    if workspace is None:
+        workspace = _mesh_workspace(field.device, n=n)
+    counts = np.zeros(2, np.uint64)
+    cp = counts.ctypes.data_as(ctypes.c_void_p)
+    lib.call("ngp_marching_cubes", _stream(), n, _p(field), float(iso), _p(workspace), None, 0, None, 0, cp)
+    V, T = int(counts[0]), int(counts[1])
+    verts = torch.empty((V, 3), dtype=torch.float32, device=field.device)
+    tris = torch.empty((T, 3), dtype=torch.int32, device=field.device)
+    if T or V:
+        lib.call("ngp_marching_cubes", _stream(), n, _p(field), float(iso), _p(workspace), _p(verts), V, _p(tris), T, cp)
+    return verts, tris
+
+
+def mesh_largest_component(verts, tris, workspace=None):
+    """The largest edge-connected set of triangles (ties: the one holding the lowest triangle), compacted in order."""
+    import ctypes
+    V, T = verts.shape[0], tris.shape[0]
+    if workspace is None:
+        workspace = _mesh_workspace(verts.device, n_verts=V, n_tris=T)
+    vo = torch.empty_like(verts)
+    to = torch.empty_like(tris)
+    counts = np.zeros(2, np.uint64)
+    lib.call("ngp_mesh_largest_component", _stream(), V, T, _p(verts), _p(tris), _p(workspace), _p(vo), _p(to), counts.ctypes.data_as(ctypes.c_void_p))
+    return vo[:int(counts[0])], to[:int(counts[1])]
+
+
+def mesh_vertex_normals(verts, tris, workspace=None):
+    """Area-weighted unit vertex normals (V, 3) f32, summed in triangle order."""
+    V, T = verts.shape[0], tris.shape[0]
+    if workspace is None:
+        workspace = _mesh_workspace(verts.device, n_verts=V, n_tris=T)
+    normals = torch.empty_like(verts)
+    lib.call("ngp_mesh_vertex_normals", _stream(), V, T, _p(verts), _p(tris) if T else None, _p(workspace), _p(normals))
+    return normals
+
+
 def march(rays_o, rays_d, bitfield, aabb, max_samples, cone_angle, near, cascades, const_dt, rng, coords=None, workspace=None):
     R = rays_o.shape[0]
     dev = rays_o.device
