@@ -134,7 +134,9 @@ __device__ __forceinline__ void hash_cell_indices(const NgpLevel& lv, uint32_t g
 // c+1 of a cell are x-neighbours: whenever their entries share an aligned 8-byte word -- dense levels: even index; hashed levels:
 // even x, because (x+1) ^ h = (x ^ h) ^ 1 then -- one REDG.F16x4 serves both.  Half of all cells qualify, i.e. 6 requests per cell
 // instead of 8 on average; the sums formed are exactly the same.  Used by the standalone ngp_hash_bwd; the gather (64-bit loads) and
-// the fused kernels do not use it.
+// the fused kernels do not use it.  The fused backward's 64-bit fixed-point scatter has no vector integer reduction to pair corners
+// with (ptxas rejects red.global.add.v2.u64); it gives the features and x-neighbours of a cell to adjacent lanes of one instruction
+// instead, so that one instruction addresses at most two 32-byte sectors per lane group (fused_net.cu, DESIGN.md section 4).
 __device__ __forceinline__ void red_add_corners(__half2* __restrict__ g, const uint32_t idx[8], const float2 acc[8]) {
 #pragma unroll
     for (int c = 0; c < 8; c += 2) {
