@@ -165,6 +165,35 @@ int ngp_composite_loss_bwd(void* stream, uint32_t n_rays, uint32_t n_elements, c
                            const float* target, float huber_delta, const float* density_grid_mean, uint32_t cascades,
                            float* rgb_out, float* loss_out, void* dnet_out, float reg_scale);
 
+/* ---- V1-V4  whole-frame renderer with early ray termination (runner/runner.py:197-264: render_img / render_img_with_pose) ------------
+ * Stands in for the tiled inference path of the reference -- ray_sampler.h per n_rays_per_batch tile, the network, then
+ * compute_rgbs_inference (calc_rgb.h:151-212) over every sample -- with a wavefront loop over rounds that drops a ray once it is opaque
+ * (DESIGN.md section 4, "Rendering").  Per ray: rgb without background, alpha = 1 - T, and the number of composited samples.
+ * One call sequence: ngp_render_init, then per round ngp_render_march_round -> ngp_network_fwd over the round's rows ->
+ * ngp_render_composite_round, until the alive count is 0.  With min_transmittance = 0 every ray composites exactly the samples
+ * ngp_march gives it; the outputs do not depend on k_steps or the capacity.  Capacity 0, a NULL workspace and jitter_tile 0 are errors.
+ * V1: layout_out[0..3] = workspace bytes, then the byte offsets inside it of the round's rows ((capacity,7) f32 NerfCoordinate),
+ * of the network outputs for them ((capacity,4) fp16) and of the device uint32 round row count (the n_dev of ngp_network_fwd). */
+int ngp_render_workspace_bytes(uint32_t n_rays, uint32_t capacity, uint64_t* layout_out);
+/* V2: slab test, near distance and jitter (ray_sampler.h:29-48).  Ray g jitters with the state advanced by
+ * (g / jitter_tile) * 2^32 + (g % jitter_tile) * 8: what ngp_march draws when the rays are marched jitter_tile at a time with one
+ * rng.advance() between tiles (the caller advances its state by ceil(n_rays / jitter_tile) * 2^32 afterwards).  Rays that miss the box
+ * finish with rgb 0, alpha 0, 0 samples.  Zeroes the outputs, builds the alive list; *n_alive_host = its length (synchronises). */
+int ngp_render_init(void* stream, uint32_t n_rays, uint32_t capacity, void* workspace, float aabb_lo, float aabb_hi, const float* rays_o,
+                    const float* rays_d, float cone_angle, float near_distance, uint32_t cascades, int const_dt, uint64_t rng_state,
+                    uint64_t rng_inc, uint32_t jitter_tile, float* rgb_out, float* alpha_out, uint32_t* n_samples_out, uint32_t* n_alive_host);
+/* V3: each of the first min(n_alive, capacity / k_steps) alive rays continues the march of ray_sampler.h:50-72 from its saved state for
+ * up to k_steps samples (a ray ends after 2^20 steps of its t sequence, occupied or skipped, as in ngp_march); their NerfCoordinate rows go to the workspace, dense in ray order, and their total to the device row count. */
+int ngp_render_march_round(void* stream, uint32_t n_rays, uint32_t capacity, void* workspace, uint32_t n_alive, uint32_t k_steps, float aabb_lo,
+                           float aabb_hi, const float* rays_o, const float* rays_d, const uint8_t* bitfield, float cone_angle, uint32_t cascades,
+                           int const_dt);
+/* V4: each marched ray composites its rows in order (calc_rgb.h:151-212 per sample); it stops after the first sample that brings T below
+ * min_transmittance, or when its march has ended (fewer than k_steps samples this round).  Same n_alive / k_steps as V3.  The other rays
+ * form the next alive list (order kept); *n_alive_host = its length (synchronises). */
+int ngp_render_composite_round(void* stream, uint32_t n_rays, uint32_t capacity, void* workspace, uint32_t n_alive, uint32_t k_steps,
+                               float min_transmittance, uint32_t cascades, float* rgb_out, float* alpha_out, uint32_t* n_samples_out,
+                               uint32_t* n_alive_host);
+
 /* ---- R10 occupancy-grid maintenance (DGS/density_grid_sampler.py:204-264 + five headers) ------------- */
 int ngp_grid_mark_untrained(void* stream, uint32_t n_elements, float* grid, uint32_t n_images, const float* focal_lengths,
                             const float* xforms, int res_x, int res_y);

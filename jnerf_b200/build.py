@@ -10,7 +10,7 @@ LIB = os.path.join(HERE, "libngp_b200.so")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 EXTRA = os.environ.get("NGP_NVCC_FLAGS", "").split()          # extra nvcc flags for experiments
 COMMON = EXTRA + ["-O3", "-std=c++17", "-lineinfo", "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC", "-I", os.path.join(HERE, "..", "include")]
-# per-file extra flags: the sampler / grid / mesh code must not contract multiply-adds on its own (bit-exact sample indices)
+# per-file extra flags: the sampler / grid / mesh / render code must not contract multiply-adds on its own (bit-exact sample indices)
 SOURCES = {
     "capi.cu": [],
     "hash_encode.cu": [],
@@ -19,6 +19,7 @@ SOURCES = {
     "sampler.cu": ["-fmad=false"],
     "grid_update.cu": ["-fmad=false"],
     "mesh.cu": ["-fmad=false"],
+    "render.cu": ["-fmad=false"],
     "optimizer.cu": [],
     "compat_tcnn.cu": [],
 }

@@ -178,6 +178,68 @@ def mesh_vertex_normals(verts, tris, workspace=None):
     return normals
 
 
+# ---- whole-frame renderer with early ray termination (include/ngp_b200.h V1-V4) ----
+RENDER_CAPACITY = 1 << 22          # default rows per round: 4 Mi rows = 112 MB of coordinates + 32 MB of network outputs
+RENDER_MAX_K = 64
+
+
+def render_k_steps(capacity, n_alive):
+    """Samples per ray of the next round: as many as let every alive ray march in one round, clamp(capacity / n_alive, 1, RENDER_MAX_K).
+    Early rounds hold many rays and few samples each (most rays stop or leave the box within a few samples); the last few rays take long
+    strides instead of one round per handful of samples.  The output does not depend on this choice."""
+    return max(1, min(RENDER_MAX_K, int(capacity) // max(int(n_alive), 1)))
+
+
+def render_workspace_layout(n_rays, capacity):
+    """(bytes, rows offset, network-output offset, row-count offset) of the renderer's workspace."""
+    lay = np.zeros(4, np.uint64)
+    lib.call("ngp_render_workspace_bytes", int(n_rays), int(capacity), lay.ctypes.data)
+    return tuple(int(x) for x in lay)
+
+
+def render_workspace(n_rays, workspace=None, capacity=RENDER_CAPACITY):
+    """`workspace` if it is large enough for n_rays rays at this capacity, else a new one."""
+    nbytes = render_workspace_layout(n_rays, capacity)[0]
+    if workspace is not None and workspace.numel() >= nbytes:
+        return workspace
+    return torch.empty(max(nbytes, 1), dtype=torch.uint8, device="cuda")
+
+
+def render_rays(rays_o, rays_d, bitfield, aabb, cone_angle, near, cascades, const_dt, rng, grid, levels, wd, wr, jitter_tile,
+                min_transmittance=0.0, capacity=RENDER_CAPACITY, workspace=None):
+    """Render R rays (model space) to (rgb (R,3) without background, alpha (R,1) = 1 - T, n_samples (R,) int32, rounds).
+    Each ray composites the samples ngp_march gives it under the jitter layout of `jitter_tile`-ray tiles, in order, and stops after the
+    first sample that brings its transmittance below `min_transmittance` (0: never).  `rng` is not advanced here: the caller moves it
+    on by ceil(R / jitter_tile) * 2^32, as the tiled renderer would.  One 4-byte read-back per round."""
+    import ctypes
+    R, dev = rays_o.shape[0], rays_o.device
+    nbytes, off_rows, off_net, off_cnt = render_workspace_layout(R, capacity)
+    if workspace is None or workspace.numel() < nbytes:
+        workspace = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
+    rows = workspace[off_rows:off_rows + 28 * capacity].view(torch.float32).view(capacity, 7)
+    net = workspace[off_net:off_net + 8 * capacity].view(torch.float16).view(capacity, 4)
+    n_rows = workspace[off_cnt:off_cnt + 4].view(torch.int32)
+    rgb = torch.empty((R, 3), dtype=torch.float32, device=dev)
+    alpha = torch.empty((R, 1), dtype=torch.float32, device=dev)
+    n_samples = torch.empty(R, dtype=torch.int32, device=dev)
+    alive = np.zeros(1, np.uint32)
+    ap = alive.ctypes.data_as(ctypes.c_void_p)
+    lib.call("ngp_render_init", _stream(), R, int(capacity), _p(workspace), float(aabb[0]), float(aabb[1]), _p(rays_o), _p(rays_d), float(cone_angle),
+             float(near), int(cascades), int(const_dt), int(rng[0]), int(rng[1]), int(jitter_tile), _p(rgb), _p(alpha), _p(n_samples), ap)
+    rounds = 0
+    while int(alive[0]):
+        n_alive = int(alive[0])
+        k = render_k_steps(capacity, n_alive)
+        lib.call("ngp_render_march_round", _stream(), R, int(capacity), _p(workspace), n_alive, k, float(aabb[0]), float(aabb[1]), _p(rays_o),
+                 _p(rays_d), _p(bitfield), float(cone_angle), int(cascades), int(const_dt))
+        bound = min(n_alive, int(capacity) // k) * k                  # rows this round can hold: the network's grid covers no more
+        network_fwd(rows[:bound], grid, levels, wd, wr, n_dev=n_rows, save_enc=False, out=net[:bound])
+        lib.call("ngp_render_composite_round", _stream(), R, int(capacity), _p(workspace), n_alive, k, float(min_transmittance), int(cascades),
+                 _p(rgb), _p(alpha), _p(n_samples), ap)
+        rounds += 1
+    return rgb, alpha, n_samples, rounds
+
+
 def march(rays_o, rays_d, bitfield, aabb, max_samples, cone_angle, near, cascades, const_dt, rng, coords=None, workspace=None):
     R = rays_o.shape[0]
     dev = rays_o.device

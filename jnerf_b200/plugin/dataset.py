@@ -110,7 +110,8 @@ class NerfDataset(_RayBatcher):
         assert json_data is not None, f"dataset is not found at {root_dir}"
         self.H, self.W = int(json_data.get("h", H)), int(json_data.get("w", W))
         frames = json_data["frames"][::10] if mode == "val" else json_data["frames"]
-        imgs, self._xforms = [], []
+        imgs, self._xforms, self.poses = [], [], []
+        self.correct_pose = tuple(correct_pose)
         for fr in frames:
             p = os.path.join(root_dir, fr["file_path"])
             if not os.path.exists(p):
@@ -125,6 +126,7 @@ class NerfDataset(_RayBatcher):
             if self.H == 0 or self.W == 0:
                 self.H, self.W = im.shape[0], im.shape[1]
             imgs.append(im)
+            self.poses.append(np.array(fr["transform_matrix"], np.float32))                           # NeRF camera-to-world, as in the file
             self._xforms.append(matrix_nerf2ngp(fr["transform_matrix"], self.scale, self.offset, correct_pose))
         self.image_data = torch.from_numpy(np.stack(imgs)).to(DEVICE).reshape(len(imgs), -1, 4)
         def read_focal_length(resolution, axis):                                                   # dataset.py:125-131
@@ -213,6 +215,8 @@ class SyntheticNerfDataset(_RayBatcher):
             fx = fov_to_focal_length(W, camera_angle_x * 180 / math.pi)
             self._focal = (fx, fx)
             self._cx, self._cy = W / 2, H / 2
+        self.poses = [np.array(m, np.float32) for m in mats]                                    # NeRF camera-to-world
+        self.correct_pose = (1, -1, -1)
         self._xforms = [matrix_nerf2ngp(m, self.scale, self.offset) for m in mats]
         self.have_img = True
         self._finish_init()

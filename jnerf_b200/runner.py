@@ -54,6 +54,7 @@ class Runner:
         # state the evaluation / checkpoint code reads on EVERY kind of model (fused or the nn.Linear fallback)
         self._table_work, self._pending_epoch = None, None
         self._host_stage = None
+        self._render_ws = None                                       # workspace of the whole-frame renderer (render_rays)
         self._dev_state = None                                       # device-resident step state + CUDA graphs (single-GPU fast path)
         self._pipe = None                                            # march of step i+1 under the optimizer sweep of step i (single GPU)
         self._st = {id(s.p): s for s in self.optimizer._nested_optimizer.state}
@@ -694,6 +695,146 @@ class Runner:
         tar = ds.rgba_for(torch.arange(n_pix, device="cuda", dtype=torch.int32) + int(img_id) * n_pix)
         tar = tar[:, :3] * tar[:, 3:] + bgc * (1 - tar[:, 3:])
         return img.reshape(H, W, 3), tar.reshape(H, W, 3)
+
+    # ------------------------------------------------------------------------------------------ rendering (runner.py:86-121, 162-264)
+    @torch.no_grad()
+    def render_rays(self, rays_o, rays_d, min_transmittance=1e-4):
+        """Whole-frame renderer (ops.render_rays): every ray at once in rounds, each ray dropped after the first sample that brings its
+        transmittance below min_transmittance (0: never, and then every ray composites the samples render_img_nosync gives it).  The
+        jitter and the sampler rng advance exactly as render_img_nosync's n_rays_per_batch tiles would have them.
+        Returns (rgb (R,3) without background, alpha (R,1), n_samples (R,), rounds).
+        The renderer's workspace (per-ray state, and 144 MB of round rows and network outputs at the default capacity) is kept for the
+        next frame; render() and test() release it when they finish, and release_render_workspace() does so at any time."""
+        assert self.fast, "render_rays drives the fused network kernel"
+        self._table_ready()
+        self._sync_front()
+        s, m = self.sampler, self.model
+        R, tile = rays_o.shape[0], int(self.cfg.n_rays_per_batch)
+        self._render_ws = ops.render_workspace(R, self._render_ws)
+        out = ops.render_rays(rays_o.contiguous(), rays_d.contiguous(), s.density_grid_bitfield, s.aabb_range, s.cone_angle_constant, s.near_distance,
+                              s.NERF_CASCADES, s.const_dt, s.rng, m.pos_encoder.m_grid, m.pos_encoder.levels, m.density_mlp.con_weights,
+                              m.rgb_mlp.con_weights, tile, min_transmittance=min_transmittance, workspace=self._render_ws)
+        ops.pcg32_advance(s.rng, ((R + tile - 1) // tile) << 32)       # one rng.advance() per tile (ray_sampler.py:61)
+        return out
+
+    def release_render_workspace(self):
+        """Free the whole-frame renderer's workspace (the next render_rays allocates a new one), e.g. before training on."""
+        self._render_ws = None
+
+    def _render_frame(self, rays_o, rays_d, W, H, min_transmittance):
+        """(img (H,W,3) with the background blended in unless alpha_image, alpha (H,W,1), n_samples (H,W), rounds)"""
+        rgb, alpha, n, rounds = self.render_rays(rays_o, rays_d, min_transmittance)
+        if not getattr(self.cfg, "alpha_image", False):
+            rgb = rgb + torch.tensor(self.background_color, dtype=torch.float32, device=rgb.device) * (1 - alpha)
+        return rgb.reshape(H, W, 3), alpha.reshape(H, W, 1), n.reshape(H, W), rounds
+
+    def pose_rays(self, pose):
+        """generate_rays_with_pose (dataset.py:236-253): the rays of every pixel, row-major, of a camera at `pose` (3x4 or 4x4 NeRF
+        camera-to-world) with the train split's image-0 intrinsics and its true [W, H] (DESIGN.md section 7)."""
+        from .plugin.dataset import matrix_nerf2ngp
+        ds = self.dataset["train"]
+        W, H = ds.resolution
+        xf = matrix_nerf2ngp(np.asarray(pose, np.float32)[:3, :4], ds.scale, ds.offset, getattr(ds, "correct_pose", (1, -1, -1)))
+        dev = ds.transforms_gpu.device
+        xforms = torch.from_numpy(np.ascontiguousarray(xf.T).reshape(1, 12)).to(dev)   # one-entry table, column-major like transforms_gpu
+        pix = torch.arange(H * W, dtype=torch.int32, device=dev)
+        _, o, d = ops.raygen(pix, W, H, xforms, ds.focal_lengths[:1].contiguous(), ds.principal[:1].contiguous())
+        return o, d
+
+    @torch.no_grad()
+    def render_img_with_pose(self, pose, min_transmittance=1e-4):
+        """runner.py:238-264 on the whole-frame renderer: the (H, W, 3) image of a camera at `pose`, background blended in unless
+        alpha_image is set."""
+        W, H = self.dataset["train"].resolution
+        o, d = self.pose_rays(pose)
+        return self._render_frame(o, d, W, H, min_transmittance)[0]
+
+    def _save_path(self):
+        return os.path.join(self.cfg.log_dir or ".", self.cfg.exp_name or "exp")
+
+    @staticmethod
+    def save_img(path, img, alpha=None):
+        """runner.py:180-188: an (H, W, 3) image in [0, 1] (+ (H, W, 1) alpha: RGBA) as an 8-bit PNG."""
+        from PIL import Image
+        img = img.detach().cpu().numpy() if torch.is_tensor(img) else np.asarray(img)
+        if alpha is not None:
+            alpha = alpha.detach().cpu().numpy() if torch.is_tensor(alpha) else np.asarray(alpha)
+            img = np.concatenate([img, alpha], axis=-1)
+        Image.fromarray((img * 255 + 0.5).clip(0, 255).astype(np.uint8)).save(path)
+
+    @torch.no_grad()
+    def render(self, save_path=None, load_ckpt=False, min_transmittance=1e-4):
+        """runner.py:101-121: the 80-frame spherical camera path (utils/camera_path.py) as an mp4 (OpenCV, mp4v, 28 fps), by default
+        log_dir/exp_name/demo.mp4.  Returns the path."""
+        try:
+            import cv2
+        except ImportError as e:
+            raise RuntimeError("Runner.render writes the video with OpenCV: install opencv-python (cv2) to use it") from e
+        from .utils.camera_path import path_spherical
+        if load_ckpt:
+            self.load_ckpt(self.cfg.ckpt_path)
+        if not save_path:
+            save_path = os.path.join(self._save_path(), "demo.mp4")
+        elif not str(save_path).endswith(".mp4"):
+            raise ValueError(f"Runner.render: the video path must end in .mp4, got {save_path}")
+        os.makedirs(os.path.dirname(os.path.abspath(save_path)), exist_ok=True)
+        W, H = self.dataset["train"].resolution
+        writer = cv2.VideoWriter(str(save_path), cv2.VideoWriter_fourcc(*"mp4v"), 28, (W, H))
+        try:
+            for pose in path_spherical():
+                img = self.render_img_with_pose(pose, min_transmittance)
+                u8 = (img.cpu().numpy() * 255 + 0.5).clip(0, 255).astype(np.uint8)
+                writer.write(np.ascontiguousarray(u8[..., ::-1]))    # OpenCV takes BGR: the file shows the true colours (DESIGN.md section 7)
+        finally:
+            writer.release()
+            self.release_render_workspace()
+        return save_path
+
+    @torch.no_grad()
+    def render_test(self, save_img=True, save_path=None, min_transmittance=1e-4):
+        """runner.py:162-178: every view of the test split on the whole-frame renderer; saves {exp_name}_r_{i}.png (RGBA when
+        alpha_image is set) and, when the split has images, {exp_name}_gt_{i}.png; returns the per-view mse against the target with the
+        background blended in (an empty list for a split without images, as the reference computes no PSNR then)."""
+        ds = self.dataset["test"]
+        save_path = self._save_path() if save_path is None else save_path
+        if save_img:
+            os.makedirs(save_path, exist_ok=True)
+        exp = self.cfg.exp_name
+        W, H = ds.resolution
+        bgc = torch.tensor(self.background_color, dtype=torch.float32, device=ds.transforms_gpu.device)
+        have_img = getattr(ds, "have_img", True)
+        mse = []
+        for i in range(ds.n_images):
+            o, d = ds.generate_rays_total_test(i)
+            img, alpha, _, _ = self._render_frame(o, d, W, H, min_transmittance)
+            if save_img:
+                self.save_img(os.path.join(save_path, f"{exp}_r_{i}.png"), img, alpha if getattr(self.cfg, "alpha_image", False) else None)
+            if not have_img:                                          # runner.py:173: no target, no gt image, no mse
+                continue
+            tar = ds.rgba_for(torch.arange(H * W, device=bgc.device, dtype=torch.int32) + i * H * W)
+            tar = (tar[:, :3] * tar[:, 3:] + bgc * (1 - tar[:, 3:])).reshape(H, W, 3)
+            if save_img:
+                self.save_img(os.path.join(save_path, f"{exp}_gt_{i}.png"), tar)
+            mse.append(float(L.img2mse(img, tar).item()))
+        return mse
+
+    @torch.no_grad()
+    def test(self, load_ckpt=False, min_transmittance=1e-4):
+        """runner.py:86-99: render the test split into log_dir/exp_name/test and print the mean test PSNR, which is returned (None for
+        a split without images, as the reference prints none then).  Releases the renderer's workspace when done."""
+        if load_ckpt:
+            self.load_ckpt(self.cfg.ckpt_path)
+        if self.dataset["test"] is None:
+            self.dataset["test"] = build_from_cfg(self.cfg.dataset.test, DATASETS)
+        try:
+            mse = self.render_test(save_path=os.path.join(self._save_path(), "test"), min_transmittance=min_transmittance)
+        finally:
+            self.release_render_workspace()
+        if not getattr(self.dataset["test"], "have_img", True):
+            return None
+        psnr = sum(float(L.mse2psnr(torch.tensor(v)).item()) for v in mse) / len(mse)
+        print(f"TOTAL TEST PSNR===={psnr}", flush=True)
+        return psnr
 
     @torch.no_grad()
     def extract_mesh(self, out_dir, resolution=512):
