@@ -101,6 +101,15 @@ int ngp_network_fwd(void* stream, uint32_t n_max, const uint32_t* n_dev, const f
 int ngp_network_bwd(void* stream, uint32_t n_max, const uint32_t* n_dev, const float* coords, const void* enc_save,
                     const void* levels_dev, const void* w_density, const void* w_rgb, const void* dout,
                     void* grid_grad, float* dw_density, float* dw_rgb);
+/* The same backward into caller-owned scratch, for ngp_train_sweep: the hash-grid gradient ACCUMULATES into fx, 16 bytes per table
+ * entry (two signed 64-bit fixed-point sums in units of 2^-32, all zero before the first call: ngp_train_sweep clears what it reads),
+ * and every CTA STORES its weight-gradient sums into its slot of w_part.  Nothing is reduced, rounded, allocated or read back, so the
+ * call is deterministic inside CUDA-graph capture too.  n_entries is the level table's entry count (offset + size of its last
+ * level); buffers smaller than ngp_network_bwd_fx_bytes(n_entries) gives are refused. */
+int ngp_network_bwd_fx_bytes(uint64_t n_entries, uint64_t* fx_bytes, uint64_t* part_bytes);
+int ngp_network_bwd_fx(void* stream, uint32_t n_max, const uint32_t* n_dev, const float* coords, const void* enc_save,
+                       const void* levels_dev, const void* w_density, const void* w_rgb, const void* dout, uint32_t n_entries,
+                       void* fx, uint64_t fx_bytes, float* w_part, uint64_t part_bytes);
 /* NGPNetworks.density (ngp_network.py:86-89): pos (n,3) f32 -> sigma_raw (n) fp16 */
 int ngp_density_fwd(void* stream, uint32_t n, const float* pos, const void* grid, const void* levels_dev,
                     const void* w_density, void* sigma_out);
@@ -209,8 +218,15 @@ int ngp_grid_update_bitfield(void* stream, const float* grid, float* mean_out, u
 int ngp_adam_ema(void* stream, uint64_t n, void* param, int param_dtype, void* grad, int grad_dtype, float grad_scale,
                  float* m, float* v, float* master, float lr, float beta1, float beta2, float eps, uint32_t step,
                  float ema_decay, int zero_grad);
+/* The optimizer tail of a single-GPU training step after ngp_network_bwd_fx(n_max = bwd_rows, fx, w_part), one launch: the weight
+ * gradients summed from the slots, the table gradient rounded from the fixed-point sums, fx cleared again, and Adam+EMA (grad_scale 1)
+ * on the fp16 table (2 * n_entries parameters) and both fp16 MLP weight vectors.  Bit for bit what ngp_network_bwd into zeroed
+ * gradients followed by ngp_adam_ema(zero_grad) on each of the three gives. */
+int ngp_train_sweep(void* stream, uint64_t n_entries, void* table, float* m, float* v, float* master, void* fx, const float* w_part,
+                    uint32_t bwd_rows, void* w_density, float* wd_m, float* wd_v, float* wd_master, void* w_rgb, float* wr_m,
+                    float* wr_v, float* wr_master, float lr, float beta1, float beta2, float eps, uint32_t step, float ema_decay);
 
-/* ---- 8e  data-parallel exchange fused with the optimizer, over NVLink peer memory ------------------------------------
+/* ---- 8e data-parallel exchange fused with the optimizer, over NVLink peer memory ------------------------------------
  * The reference has no multi-GPU path for NGP (SURVEY.md 8e; its only exchange is jt.mpi all-reduce inside nn optimizers,
  * python/jnerf/optims/adam.py:8-16 via jt.nn.Adam).  One launch per step replaces gradient all-reduce + Adam + EMA:
  * reduce-scatter by pulling the peers' gradient slices, Adam+EMA on this rank's slice of the padded hash table, all-gather
@@ -266,6 +282,10 @@ int ngp_march_dev(void* stream, uint32_t n_rays, float aabb_lo, float aabb_hi, u
 /* ngp_adam_ema with lr / betas / eps / step / decay / grad_scale folded into the step state's factors */
 int ngp_adam_ema_dev(void* stream, uint64_t n, void* param, int param_dtype, void* grad, int grad_dtype, float* m, float* v,
                      float* master, const void* state_dev, int zero_grad);
+/* ngp_train_sweep with the step state's factors */
+int ngp_train_sweep_dev(void* stream, uint64_t n_entries, void* table, float* m, float* v, float* master, void* fx, const float* w_part,
+                        uint32_t bwd_rows, void* w_density, float* wd_m, float* wd_v, float* wd_master, void* w_rgb, float* wr_m,
+                        float* wr_v, float* wr_master, const void* state_dev);
 
 /* pcg32 helpers (ops/op_include/pcg32/pcg32.h): host-side, pure integer */
 void ngp_pcg32_seed(uint64_t initstate, uint64_t initseq, uint64_t* state_inc);

@@ -11,6 +11,7 @@
 // Roofline (DESIGN.md): forward is bound by the gather (524 B algorithmic per sample, L2-resident table);
 // the tensor work is 20 480 flop/sample forward, 61 440 with dgrad+wgrad.
 #include "mlp_tc.cuh"
+#include "train_common.cuh"
 #include <cstdlib>
 #include <cstdio>
 #include <mutex>
@@ -20,11 +21,6 @@ int* ngp_err_flag();
 
 namespace {
 using namespace mlp;
-
-// flat weight offsets (halfs) inside the two parameter vectors (OPS/fully_fused_mlp.py:26-40)
-constexpr int WD_W0 = 0, WD_WOUT = 64 * 32, WD_N = 64 * 32 + 16 * 64;
-constexpr int WR_W0 = 0, WR_W1 = 64 * 32, WR_WOUT = 64 * 32 + 64 * 64, WR_N = 64 * 32 + 64 * 64 + 16 * 64;
-constexpr int W_PART = WD_N + WR_N;   // one CTA's weight-gradient sums: [dwd | dwr]
 
 // ---- shared-memory maps -------------------------------------------------------------------------------
 // activation slab groups
@@ -277,7 +273,8 @@ network_fwd_kernel(uint32_t n_max, const uint32_t* __restrict__ n_dev, const flo
 // Both gradient sums are independent of scheduling, so that a training run is reproducible: each CTA stores its weight-gradient sums
 // in its own slot (layout [dwd | dwr]) and wgrad_reduce_kernel adds the slots in CTA order; the scatter adds into a 64-bit fixed-point
 // copy of the hash-grid gradient (integer sums do not depend on their order) that grid_grad_flush_kernel rounds once into the fp16
-// gradient and clears again.  Without that scratch (see ngp_network_bwd) the kernel reduces straight into the outputs instead, with
+// gradient and clears again -- or, after ngp_network_bwd_fx, the training sweep of optimizer.cu reads both straight from the slots
+// and the scratch.  Without that scratch (see ngp_network_bwd) the kernel reduces straight into the outputs instead, with
 // fp32 / f16x2 reductions whose rounding depends on their order.
 constexpr uint32_t B3_G_GX = 32, B3_G_DY = 40, B3_G_DENC = 42, B3_GROUPS = 46;   // slab groups of one tile after the 32 activation groups
 constexpr uint32_t B3_EPI_THREADS = 256, B3_SCATTER_WARPS = 8, B3_THREADS = B3_EPI_THREADS + 32 * B3_SCATTER_WARPS;
@@ -302,10 +299,7 @@ struct SmemBwd3 {
 static_assert(SmemBwd3::total <= 227 * 1024, "backward CTA does not fit");
 constexpr uint32_t B3_STAGE = 1, B3_FULL = 2, B3_EMPTY = 3;         // named barriers (4 + T: the 128 threads of tile T)
 
-// Fixed-point hash-grid gradient: feature f of entry e is the signed 64-bit integer fx[2e + f] in units of 2^-32.  The unit is below
-// the smallest fp16 spacing (2^-24), so every contribution keeps more precision than an fp16 reduction gives it, and a sum cannot wrap
-// while it is within the fp16 range: a contribution is clamped to +-65504 first, and 2^31 units of 1 are 2^31 / 65504 > 32 000 of them.
-constexpr float FX_SCALE = 4294967296.0f, FX_INV = 1.0f / 4294967296.0f;
+// a contribution to the fixed-point hash-grid gradient (train_common.cuh)
 __device__ __forceinline__ void red_add_fx(unsigned long long* p, float v) {
     const long long q = __float2ll_rn(fminf(fmaxf(v, -65504.f), 65504.f) * FX_SCALE);
     if (q) asm volatile("red.global.add.u64 [%0], %1;" ::"l"(__cvta_generic_to_global(p)), "l"((unsigned long long)q) : "memory");
@@ -664,6 +658,25 @@ int bwd_scratch(cudaStream_t s, const void* levels_dev, BwdScratch** out) {
     return 0;
 }
 
+// One launch of network_bwd256_kernel: with fx / w_part into the fixed-point scratch and the per-CTA slots, without them straight
+// into grid_grad / dwd / dwr.
+int bwd_launch(cudaStream_t s, uint32_t n_max, const uint32_t* n_dev, const float* coords, const void* enc_save, const void* levels_dev,
+               const void* w_density, const void* w_rgb, const void* dout, void* grid_grad, float* dw_density, float* dw_rgb,
+               unsigned long long* fx, uint32_t fx_entries, float* w_part) {
+    // timing experiments only (results are wrong with any bit set): 1 = no atomics, 2 = no scatter, 4 = no weight-gradient MMAs
+    static const uint32_t dbg = getenv("NGP_BWD_DEBUG") ? (uint32_t)atoi(getenv("NGP_BWD_DEBUG")) : 0u;
+    if (ngp_first_use((const void*)network_bwd256_kernel)) NGP_CHECK_CUDA(cudaFuncSetAttribute(network_bwd256_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SmemBwd3::total));
+    NgpTensorMap enc_map{};
+    static const bool no_tma = getenv("NGP_NO_TMA") != nullptr;           // A/B switch
+    const uint32_t enc_tma = (!no_tma && ngp_make_rows32_tensormap(&enc_map, enc_save, n_max)) ? 1u : 0u;
+    network_bwd256_kernel<<<bwd_ctas(n_max), B3_THREADS, SmemBwd3::total, s>>>(n_max, n_dev, coords, (const __half*)enc_save, (const NgpLevel*)levels_dev,
+                                                                              (const __half*)w_density, (const __half*)w_rgb, (const __half*)dout,
+                                                                              (__half*)grid_grad, dw_density, dw_rgb, fx, fx_entries, w_part,
+                                                                              ngp_err_flag(), dbg, enc_map, enc_tma);
+    NGP_LAUNCH_CHECK();
+    return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -715,29 +728,37 @@ int ngp_network_bwd(void* stream, uint32_t n_max, const uint32_t* n_dev, const f
                     const void* w_density, const void* w_rgb, const void* dout, void* grid_grad, float* dw_density, float* dw_rgb) {
     if (n_max == 0) return 0;
     cudaStream_t s = (cudaStream_t)stream;
-    const uint32_t ntiles = (n_max + ROWS - 1) / ROWS;
-    // timing experiments only (results are wrong with any bit set): 1 = no atomics, 2 = no scatter, 4 = no weight-gradient MMAs
-    static const uint32_t dbg = getenv("NGP_BWD_DEBUG") ? (uint32_t)atoi(getenv("NGP_BWD_DEBUG")) : 0u;
-    if (ngp_first_use((const void*)network_bwd256_kernel)) NGP_CHECK_CUDA(cudaFuncSetAttribute(network_bwd256_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SmemBwd3::total));
-    const uint32_t grid_dim = min((ntiles + 1) / 2, (uint32_t)ngp_num_sms());
-    NgpTensorMap enc_map{};
-    static const bool no_tma = getenv("NGP_NO_TMA") != nullptr;           // A/B switch
-    const uint32_t enc_tma = (!no_tma && ngp_make_rows32_tensormap(&enc_map, enc_save, n_max)) ? 1u : 0u;
     BwdScratch* b = nullptr;
     if (int rc = bwd_scratch(s, levels_dev, &b)) return rc;
-    network_bwd256_kernel<<<grid_dim, B3_THREADS, SmemBwd3::total, s>>>(n_max, n_dev, coords, (const __half*)enc_save, (const NgpLevel*)levels_dev,
-                                                                       (const __half*)w_density, (const __half*)w_rgb, (const __half*)dout,
-                                                                       (__half*)grid_grad, dw_density, dw_rgb, b ? b->fx : nullptr,
-                                                                       b ? b->fx_entries : 0u, b ? b->part : nullptr, ngp_err_flag(), dbg, enc_map, enc_tma);
-    NGP_LAUNCH_CHECK();
+    if (int rc = bwd_launch(s, n_max, n_dev, coords, enc_save, levels_dev, w_density, w_rgb, dout, grid_grad, dw_density, dw_rgb, b ? b->fx : nullptr,
+                            b ? b->fx_entries : 0u, b ? b->part : nullptr))
+        return rc;
     if (b) {
-        wgrad_reduce_kernel<<<(W_PART + 255) / 256, 256, 0, s>>>(b->part, grid_dim, dw_density, dw_rgb);
+        wgrad_reduce_kernel<<<(W_PART + 255) / 256, 256, 0, s>>>(b->part, bwd_ctas(n_max), dw_density, dw_rgb);
         NGP_LAUNCH_CHECK();
         grid_grad_flush_kernel<<<ngp_num_sms() * 8, 256, 0, s>>>((const NgpLevel*)levels_dev, b->fx_entries, reinterpret_cast<longlong2*>(b->fx),
                                                                  (__half2*)grid_grad);
         NGP_LAUNCH_CHECK();
     }
     return 0;
+}
+
+int ngp_network_bwd_fx_bytes(uint64_t n_entries, uint64_t* fx_bytes, uint64_t* part_bytes) {
+    *fx_bytes = 16 * n_entries;
+    *part_bytes = sizeof(float) * W_PART * (uint64_t)ngp_num_sms();
+    return 0;
+}
+
+int ngp_network_bwd_fx(void* stream, uint32_t n_max, const uint32_t* n_dev, const float* coords, const void* enc_save, const void* levels_dev,
+                       const void* w_density, const void* w_rgb, const void* dout, uint32_t n_entries, void* fx, uint64_t fx_bytes,
+                       float* w_part, uint64_t part_bytes) {
+    // every entry must be held by the scratch: the kernel's fallback for the others would reduce into a gradient this call has not got
+    NGP_REQUIRE(fx != nullptr && fx_bytes >= 16 * (uint64_t)n_entries, "ngp_network_bwd_fx: the fixed-point scratch must hold 16 bytes per table entry");
+    NGP_REQUIRE(w_part != nullptr && part_bytes >= sizeof(float) * W_PART * (uint64_t)ngp_num_sms(),
+                "ngp_network_bwd_fx: the weight-gradient slots are smaller than ngp_network_bwd_fx_bytes gives");
+    if (n_max == 0) return 0;
+    return bwd_launch((cudaStream_t)stream, n_max, n_dev, coords, enc_save, levels_dev, w_density, w_rgb, dout, nullptr, nullptr, nullptr,
+                      (unsigned long long*)fx, n_entries, w_part);
 }
 
 }  // extern "C"

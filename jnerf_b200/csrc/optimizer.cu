@@ -6,22 +6,11 @@
 //   read  grad(2|4) + m(4) + v(4) + master(4)   write m(4) + v(4) + master(4) + param(2|4) [+ grad zero]
 // = 30 B/param for the fp16 table -> HBM-bound (DESIGN.md).  Optimizer state is fp32; `master` is the EMA's
 // `values` buffer and doubles as the fp32 master copy of fp16 parameters (documented deviation, SURVEY.md 8c).
-#include "ngp_common.cuh"
+#include "train_common.cuh"
 #include <cmath>
 #include <cstring>
 
 namespace {
-
-// Every operation is spelled out (no compiler-chosen FMA contraction) so that all kernels that inline this -- the single-GPU
-// sweep, its scalar tail and the data-parallel exchange kernel -- produce bit-identical parameters from identical inputs.
-__device__ __forceinline__ float adam_one(float g, float& m, float& v, float& master, const AdamArgs& a) {
-    g = __fmul_rn(g, a.grad_scale);
-    m = __fmaf_rn(a.b1, m, __fmul_rn(1.f - a.b1, g));
-    v = __fmaf_rn(a.b2, v, __fmul_rn(__fmul_rn(1.f - a.b2, g), g));
-    const float p = __fsub_rn(master, __fdiv_rn(__fmul_rn(m, a.step_size), __fadd_rn(sqrtf(v), a.eps)));          // jt.nn.Adam.step
-    master = __fmul_rn(__fmaf_rn(1.f - a.decay, p, __fmul_rn(__fmul_rn(a.decay, master), a.debias_old)), a.debias_new);   // ema.py:33-36
-    return master;
-}
 
 // Each thread handles 4 consecutive parameters per slot, so that every 16-byte (fp32) / 8-byte (fp16) access of a warp is one
 // fully coalesced 512 B / 256 B request; UNROLL slots are issued back to back to keep ~100 B per thread in flight.
@@ -87,6 +76,86 @@ __global__ void __launch_bounds__(256) adam_ema_kernel(uint64_t n, PT* __restric
         if (zero_grad) grad[i] = (GT)0.f;
         const float p = adam_one(g1, m1, v1, s1, a);
         m[i] = m1; v[i] = v1; master[i] = s1; param[i] = (PT)p;
+    }
+}
+
+// The training step's whole optimizer tail in one launch, after ngp_network_bwd_fx.  It computes exactly what the backward's slot
+// reduction and fixed-point flush (ngp_network_bwd) followed by adam_ema_kernel on the three gradients compute, without the fp16
+// table gradient in between: per table parameter 8 + 26 bytes plus 8 for every touched one, against 8 + 12 f + 30 for that sequence.
+//  * blocks [0, SWEEP_W_BLOCKS), scheduled first: one MLP weight each thread -- the sum of the backward's per-CTA slots in CTA order,
+//    formed as wgrad_reduce_kernel forms it and added to a zero gradient, then Adam+EMA;
+//  * the other blocks stream the hash table, one entry (2 parameters) per slot: the fixed-point sums rounded once to fp16, as the
+//    flush rounds them into a zeroed gradient, nonzero scratch entries cleared for the next backward, then Adam+EMA.
+constexpr uint32_t SWEEP_THREADS = 256, SWEEP_W_BLOCKS = (W_PART + SWEEP_THREADS - 1) / SWEEP_THREADS;
+struct SweepTensor { __half* param; float *m, *v, *master; };
+
+// the gradient of one table entry, as the flush leaves it in a zeroed fp16 gradient (the product is exact: FX_INV is a power of two)
+__device__ __forceinline__ float2 fx_grad(longlong2 q) {
+    if (!(q.x | q.y)) return make_float2(0.f, 0.f);
+    return __half22float2(__floats2half2_rn(__fmul_rn(__ll2float_rn(q.x), FX_INV), __fmul_rn(__ll2float_rn(q.y), FX_INV)));
+}
+
+__global__ void __launch_bounds__(SWEEP_THREADS) train_sweep_kernel(uint64_t n_entries, SweepTensor tab, longlong2* __restrict__ fx,
+                                                                    const float* __restrict__ part, uint32_t nparts, SweepTensor wd, SweepTensor wr,
+                                                                    AdamArgs a, const NgpStepState* __restrict__ st) {
+    if (st) a = st->adam;
+    if (blockIdx.x < SWEEP_W_BLOCKS) {
+        const uint32_t e = blockIdx.x * SWEEP_THREADS + threadIdx.x;
+        if (e >= (uint32_t)W_PART) return;
+        float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
+        uint32_t k = 0;
+#pragma unroll 4
+        for (; k + 4 <= nparts; k += 4) {
+            a0 += part[(size_t)k * W_PART + e];
+            a1 += part[(size_t)(k + 1) * W_PART + e];
+            a2 += part[(size_t)(k + 2) * W_PART + e];
+            a3 += part[(size_t)(k + 3) * W_PART + e];
+        }
+        for (; k < nparts; ++k) a0 += part[(size_t)k * W_PART + e];
+        const float g = __fadd_rn(0.f, (a0 + a1) + (a2 + a3));
+        const bool d = e < (uint32_t)WD_N;
+        const uint32_t j = d ? e : e - WD_N;
+        float* wm = (d ? wd.m : wr.m) + j;
+        float* wv = (d ? wd.v : wr.v) + j;
+        float* ws = (d ? wd.master : wr.master) + j;
+        float m1 = *wm, v1 = *wv, s1 = *ws;
+        const float p = adam_one(g, m1, v1, s1, a);
+        *wm = m1; *wv = v1; *ws = s1;
+        (d ? wd.param : wr.param)[j] = __float2half_rn(p);
+        return;
+    }
+    // one entry (2 parameters) per thread and slot: every access of a warp -- 16 B of scratch, 8 B of m / v / master, 4 B of
+    // parameters per lane -- is one contiguous request whose sectors are used whole
+    constexpr int UNROLL = 4;
+    const uint64_t T = (uint64_t)(gridDim.x - SWEEP_W_BLOCKS) * SWEEP_THREADS;
+    const uint64_t g0 = (uint64_t)(blockIdx.x - SWEEP_W_BLOCKS) * SWEEP_THREADS + threadIdx.x;
+    for (uint64_t i0 = g0; i0 < n_entries; i0 += UNROLL * T) {
+        longlong2 q[UNROLL];
+        float2 mm[UNROLL], vv[UNROLL], ms[UNROLL];
+#pragma unroll
+        for (int u = 0; u < UNROLL; ++u) {
+            const uint64_t i = i0 + u * T;
+            if (i < n_entries) {
+                q[u] = fx[i];
+                mm[u] = reinterpret_cast<const float2*>(tab.m)[i];
+                vv[u] = reinterpret_cast<const float2*>(tab.v)[i];
+                ms[u] = reinterpret_cast<const float2*>(tab.master)[i];
+            }
+        }
+#pragma unroll
+        for (int u = 0; u < UNROLL; ++u) {
+            const uint64_t i = i0 + u * T;
+            if (i < n_entries) {
+                const float2 g = fx_grad(q[u]);
+                if (q[u].x | q[u].y) fx[i] = make_longlong2(0, 0);
+                const float px = adam_one(g.x, mm[u].x, vv[u].x, ms[u].x, a);
+                const float py = adam_one(g.y, mm[u].y, vv[u].y, ms[u].y, a);
+                reinterpret_cast<float2*>(tab.m)[i] = mm[u];
+                reinterpret_cast<float2*>(tab.v)[i] = vv[u];
+                reinterpret_cast<float2*>(tab.master)[i] = ms[u];
+                reinterpret_cast<__half2*>(tab.param)[i] = __floats2half2_rn(px, py);
+            }
+        }
     }
 }
 
@@ -315,6 +384,35 @@ int ngp_adam_ema_dev(void* stream, uint64_t n, void* param, int param_dtype, voi
                      const void* state_dev, int zero_grad) {
     NGP_REQUIRE(state_dev != nullptr, "ngp_adam_ema_dev: state_dev is required");
     return adam_launch(stream, n, param, param_dtype, grad, grad_dtype, m, v, master, AdamArgs{}, zero_grad, (const NgpStepState*)state_dev);
+}
+
+static int sweep_launch(void* stream, uint64_t n_entries, void* table, float* m, float* v, float* master, void* fx, const float* w_part,
+                        uint32_t bwd_rows, void* w_density, float* wd_m, float* wd_v, float* wd_master, void* w_rgb, float* wr_m, float* wr_v,
+                        float* wr_master, AdamArgs a, const NgpStepState* st) {
+    NGP_REQUIRE(fx != nullptr && w_part != nullptr, "ngp_train_sweep: the backward's fixed-point scratch and weight-gradient slots are required");
+    const uint32_t blocks = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((n_entries + 4 * SWEEP_THREADS - 1) / (4 * SWEEP_THREADS),
+                                                                           (uint64_t)ngp_num_sms() * 32));
+    train_sweep_kernel<<<SWEEP_W_BLOCKS + blocks, SWEEP_THREADS, 0, (cudaStream_t)stream>>>(
+        n_entries, SweepTensor{(__half*)table, m, v, master}, (longlong2*)fx, w_part, bwd_ctas(bwd_rows),
+        SweepTensor{(__half*)w_density, wd_m, wd_v, wd_master}, SweepTensor{(__half*)w_rgb, wr_m, wr_v, wr_master}, a, st);
+    NGP_LAUNCH_CHECK();
+    return 0;
+}
+
+int ngp_train_sweep(void* stream, uint64_t n_entries, void* table, float* m, float* v, float* master, void* fx, const float* w_part,
+                    uint32_t bwd_rows, void* w_density, float* wd_m, float* wd_v, float* wd_master, void* w_rgb, float* wr_m, float* wr_v,
+                    float* wr_master, float lr, float beta1, float beta2, float eps, uint32_t step, float ema_decay) {
+    NGP_REQUIRE(step >= 1, "ngp_train_sweep: step is 1-based");
+    return sweep_launch(stream, n_entries, table, m, v, master, fx, w_part, bwd_rows, w_density, wd_m, wd_v, wd_master, w_rgb, wr_m, wr_v,
+                        wr_master, make_adam_args(lr, beta1, beta2, eps, step, ema_decay, 1.0f), nullptr);
+}
+
+int ngp_train_sweep_dev(void* stream, uint64_t n_entries, void* table, float* m, float* v, float* master, void* fx, const float* w_part,
+                        uint32_t bwd_rows, void* w_density, float* wd_m, float* wd_v, float* wd_master, void* w_rgb, float* wr_m, float* wr_v,
+                        float* wr_master, const void* state_dev) {
+    NGP_REQUIRE(state_dev != nullptr, "ngp_train_sweep_dev: state_dev is required");
+    return sweep_launch(stream, n_entries, table, m, v, master, fx, w_part, bwd_rows, w_density, wd_m, wd_v, wd_master, w_rgb, wr_m, wr_v,
+                        wr_master, AdamArgs{}, (const NgpStepState*)state_dev);
 }
 
 static AdamArgs make_adam_args(float lr, float beta1, float beta2, float eps, uint32_t step, float ema_decay, float grad_scale) {

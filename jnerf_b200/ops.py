@@ -115,6 +115,40 @@ def network_bwd(coords, enc, levels, wd, wr, dout, grid_grad, dwd, dwr, n_dev=No
              _p(grid_grad), _p(dwd), _p(dwr))
 
 
+_network_bwd = network_bwd        # the Runner folds its optimizer tail into train_sweep only while network_bwd is this function
+
+
+def network_bwd_scratch(levels, device="cuda"):
+    """(fx, w_part): zeroed caller-owned scratch of network_bwd_fx / train_sweep for this level table -- the fixed-point hash-grid
+    gradient (int64, two per entry) and the per-CTA weight-gradient slots (fp32)."""
+    b = np.zeros(2, np.uint64)
+    lib.call("ngp_network_bwd_fx_bytes", levels.n_entries, b.ctypes.data, b[1:].ctypes.data)
+    return (torch.zeros(int(b[0]) // 8, dtype=torch.int64, device=device), torch.zeros(int(b[1]) // 4, dtype=torch.float32, device=device))
+
+
+def network_bwd_fx(coords, enc, levels, wd, wr, dout, fx, w_part, n_dev=None):
+    """network_bwd into the scratch of network_bwd_scratch; train_sweep(bwd_rows=coords.shape[0]) turns it into the optimizer step."""
+    lib.call("ngp_network_bwd_fx", _stream(), coords.shape[0], _p(n_dev), _p(coords), _p(enc), _p(levels.table), _p(wd), _p(wr), _p(dout),
+             levels.n_entries, _p(fx), fx.numel() * fx.element_size(), _p(w_part), w_part.numel() * w_part.element_size())
+
+
+def _sweep_args(table, table_state, fx, w_part, bwd_rows, wd, wd_state, wr, wr_state):
+    assert table.dtype == wd.dtype == wr.dtype == torch.float16 and table.numel() % 2 == 0
+    return (_stream(), table.numel() // 2, _p(table), *map(_p, table_state), _p(fx), _p(w_part), int(bwd_rows), _p(wd), *map(_p, wd_state), _p(wr),
+            *map(_p, wr_state))
+
+
+def train_sweep(table, table_state, fx, w_part, bwd_rows, wd, wd_state, wr, wr_state, lr, step, beta1=0.9, beta2=0.99, eps=1e-15, ema_decay=0.95):
+    """The optimizer tail after network_bwd_fx(rows = bwd_rows) in one launch: Adam+EMA of the fp16 hash table and both fp16 MLP weight
+    vectors from the backward's scratch, which it clears.  *_state = (m, v, master).  Same bits as network_bwd + three adam_ema calls."""
+    lib.call("ngp_train_sweep", *_sweep_args(table, table_state, fx, w_part, bwd_rows, wd, wd_state, wr, wr_state), float(lr), float(beta1),
+             float(beta2), float(eps), int(step), float(ema_decay))
+
+
+def train_sweep_dev(table, table_state, fx, w_part, bwd_rows, wd, wd_state, wr, wr_state, state):
+    lib.call("ngp_train_sweep_dev", *_sweep_args(table, table_state, fx, w_part, bwd_rows, wd, wd_state, wr, wr_state), _p(state))
+
+
 def density_fwd(pos, grid, levels, wd):
     out = torch.empty(pos.shape[0], dtype=torch.float16, device=pos.device)
     lib.call("ngp_density_fwd", _stream(), pos.shape[0], _p(pos), _p(grid), _p(levels.table), _p(wd), _p(out))

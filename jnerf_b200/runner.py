@@ -81,6 +81,13 @@ class Runner:
         self.dnet = torch.zeros((cap, 4), dtype=torch.float16, device=dev)
         self.last_loss = None
         self.last_rgb = None
+        # One GPU: the backward leaves its gradients in caller-owned scratch (fixed-point table gradient, per-CTA weight-gradient slots)
+        # and ONE sweep turns them into the optimizer step of all three tensors (ops.train_sweep, same bits as the backward's own
+        # reduction + three adam_ema sweeps, about 80 MB less traffic a step).  Only with the library's own network_bwd: a stand-in
+        # operator layer keeps the per-tensor calls.  Data parallelism exchanges the fp16 table gradient and keeps them too.
+        self._fx = self._w_part = None
+        if self.world_size == 1 and ops.network_bwd is ops._network_bwd:
+            self._fx, self._w_part = ops.network_bwd_scratch(m.pos_encoder.levels, device=dev)
         if self.world_size == 1:
             # Device-resident step state (include/ngp_b200.h: ngp_step_state_*): the sampler rng, the pixel cursor and Adam's step
             # factors live on the device, so every launch of a training step has the same arguments and the step can be captured in
@@ -94,9 +101,10 @@ class Runner:
             self._graph_after = int(os.environ.get("NGP_GRAPH_AFTER", "20"))     # occurrences of a ray-batch size before it gets a graph
         # Software pipeline over steps (default): nothing the march reads is written by the network kernels -- rays, jitter and the
         # occupancy bitfield only -- so the "front" of step i+1 (background colours, ray generation, march, compaction) is enqueued
-        # on a second stream while step i's backward / Adam+EMA sweep still run.  The sweep is HBM-bound and the march is
+        # on a second stream while step i's network kernels / Adam+EMA sweep still run.  The sweep is HBM-bound and the march is
         # latency-bound: side by side they share the SMs instead of queueing (DESIGN.md section 5).  NGP_PIPE_AT picks the point of
-        # step i the front of step i+1 may start at: after its network forward ("fwd"), backward ("bwd") or at once ("front").
+        # step i the front of step i+1 may start at: after its network forward ("fwd"), backward ("bwd") or at once ("front", the
+        # fastest on the H100: DESIGN.md section 5).
         if os.environ.get("NGP_PIPELINE", "1") == "1" and not getattr(self, "_graphs_enabled", False):
             at = os.environ.get("NGP_PIPE_AT", "front")
             assert at in ("front", "fwd", "bwd")
@@ -241,9 +249,12 @@ class Runner:
         rgb, loss, _ = ops.composite_loss_bwd(self.net_out, coords, s._rays_numsteps, s._rays_numsteps_compacted, bg, target,
                                               s.density_grid_mean, delta=self.loss_func.delta, cascades=s.NERF_CASCADES, dnet=self.dnet)
         self.net_backward(coords, n_dev)
-        for p, g in ((m.pos_encoder.m_grid, self.grid_grad), (m.density_mlp.con_weights, self.dwd), (m.rgb_mlp.con_weights, self.dwr)):
-            stp = self._st[id(p)]
-            ops.adam_ema_dev(p.data, g, stp.m, stp.v, stp.master, st, zero_grad=True)
+        if self._fx is not None:
+            ops.train_sweep_dev(*self._sweep_tensors(), st)
+        else:
+            for p, g in ((m.pos_encoder.m_grid, self.grid_grad), (m.density_mlp.con_weights, self.dwd), (m.rgb_mlp.con_weights, self.dwr)):
+                stp = self._st[id(p)]
+                ops.adam_ema_dev(p.data, g, stp.m, stp.v, stp.master, st, zero_grad=True)
         ops.step_state_tick(st, R, lr_next, adam.betas[0], adam.betas[1], adam.eps, self.ema_optimizer.decay, 1.0)
         self.last_loss, self.last_rgb = loss, rgb
         return loss
@@ -431,8 +442,8 @@ class Runner:
         # cost a launch latency each -- on a third stream they run beside the table's sweep instead of after it
         m = self.model
         hyper = (lr, adam.n_step, adam.betas[0], adam.betas[1], adam.eps, self.ema_optimizer.decay)
-        if self.world_size > 1:
-            self._optimizer_step(lr, adam.n_step)                    # gradient exchange fused with the sliced sweep (section 6)
+        if self.world_size > 1 or self._fx is not None:
+            self._optimizer_step(lr, adam.n_step)                    # the one sweep, or the gradient exchange fused with the sliced sweep
             return self._pipe_finish(F, loss, rgb, batch, next_batch)
         P["bwd_done"].record(main)
         P["aux"].wait_event(P["bwd_done"])
@@ -565,14 +576,29 @@ class Runner:
     def net_backward(self, coords, n_dev):
         """self.dnet -> gradients of the hash table (self.grid_grad) and of both weight vectors (self.dwd, self.dwr)."""
         m = self.model
+        if self._fx is not None:                                     # into the scratch the next sweep reads and clears
+            ops.network_bwd_fx(coords, self.enc, m.pos_encoder.levels, m.density_mlp.con_weights, m.rgb_mlp.con_weights, self.dnet,
+                               self._fx, self._w_part, n_dev=n_dev)
+            self._bwd_rows = coords.shape[0]                         # the sweep reads as many weight-gradient slots as this fills
+            return
         ops.network_bwd(coords, self.enc, m.pos_encoder.levels, m.density_mlp.con_weights, m.rgb_mlp.con_weights, self.dnet,
                         self.grid_grad, self.dwd, self.dwr, n_dev=n_dev)
+
+    def _sweep_tensors(self):
+        """Arguments of ops.train_sweep(_dev) after net_backward."""
+        m = self.model
+        st = [self._st[id(p)] for p in (m.pos_encoder.m_grid, m.density_mlp.con_weights, m.rgb_mlp.con_weights)]
+        return (m.pos_encoder.m_grid.data, (st[0].m, st[0].v, st[0].master), self._fx, self._w_part, self._bwd_rows,
+                m.density_mlp.con_weights.data, (st[1].m, st[1].v, st[1].master), m.rgb_mlp.con_weights.data, (st[2].m, st[2].v, st[2].master))
 
     def _optimizer_step(self, lr, n_step):
         """Gradient exchange + fused Adam/EMA sweep(s) (optims/adam.py + ema.py; runner.py:75-76)."""
         m = self.model
         adam = self.optimizer._nested_optimizer
         hyper = (lr, n_step, adam.betas[0], adam.betas[1], adam.eps, self.ema_optimizer.decay)
+        if self._fx is not None:
+            ops.train_sweep(*self._sweep_tensors(), lr, n_step, adam.betas[0], adam.betas[1], adam.eps, self.ema_optimizer.decay)
+            return
         if self.world_size > 1 and self.dp_mode == "p2p":
             st = self._st[id(m.pos_encoder.m_grid)]
             self._epoch += 1
