@@ -138,6 +138,17 @@ int ngp_mesh_largest_component(void* stream, uint64_t n_verts, uint64_t n_tris, 
  * sum stays zero).  normals (n_verts,3). */
 int ngp_mesh_vertex_normals(void* stream, uint64_t n_verts, uint64_t n_tris, const float* verts, const int32_t* tris, void* workspace,
                             float* normals);
+/* M5/M6: mcubes.smooth(sigma) of --mcube_smooth (:27-31, 74-78), to be marched at iso 0 (DESIGN.md section 7 states the contract).
+ * method: 0 auto (constrained for n <= 512, gaussian above), 1 constrained (signed distance from an exact EDT, then a bounded fp64 Jacobi
+ * solve on the band |D| < 4, at most max_iters iterations, stopping early on the energy test every 10), 2 gaussian (sigma 3 of
+ * field - 0.5 in fp64, mode 'reflect'; max_iters is ignored).  max_iters = 0 with the constrained method gives D itself.
+ * field and field_out are separate n^3 fp32 lattices.  info_host[0..2] = method used, iterations run, band variables (the constrained
+ * method reads them back once and synchronises; the gaussian one does not synchronise).  Bit-reproducible.
+ * M5 workspace, each part rounded up to 256 bytes: constrained 8 n^3 (two int32 lattices) + 4 ceil(n^3 / 2048) + 24 + 8 * 1024
+ *   + 64 n^3 (neighbour table, x, Qx and bound of up to n^3 band variables), about 9.7 GB at n = 512; gaussian 8 n^3 (one fp64 lattice). */
+int ngp_mesh_smooth_workspace_bytes(uint32_t n, uint32_t method, uint64_t* bytes_out);
+int ngp_mesh_smooth(void* stream, uint32_t n, const float* field, uint32_t method, uint32_t max_iters, void* workspace,
+                    uint64_t workspace_bytes, float* field_out, uint32_t* info_host);
 
 /* ---- R6  ray march (DGS/ray_sampler.py:20-72 -> DGS/op_header/ray_sampler.h:4-114) -------------------
  * counters[0] = rays accepted, counters[1] = total samples (both zeroed here, ray_sampler.py:29).

@@ -19,6 +19,7 @@ SOURCES = {
     "sampler.cu": ["-fmad=false"],
     "grid_update.cu": ["-fmad=false"],
     "mesh.cu": ["-fmad=false"],
+    "mesh_smooth.cu": ["-fmad=false"],
     "render.cu": ["-fmad=false"],
     "optimizer.cu": [],
     "compat_tcnn.cu": [],

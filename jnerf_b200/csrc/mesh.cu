@@ -6,11 +6,15 @@
 // Built with -fmad=false (like sampler.cu): the interpolation and the cross products match the oracle bit for bit.
 #include "ngp_common.cuh"
 #include "mc_table.cuh"
+#include "mesh_scan.cuh"
+
+using ngp_mesh::scan_u32;
 
 namespace {
 
 constexpr uint32_t MC_THREADS = 256, MC_PPT = 8, MC_BLOCK = MC_THREADS * MC_PPT;   // lattice points per block (8 consecutive per thread)
 constexpr uint32_t SC_THREADS = 256, SC_PPT = 8, SC_BLOCK = SC_THREADS * SC_PPT;   // elements per block of the u32 scans
+static_assert(SC_BLOCK == ngp_mesh::SCAN_BLOCK, "mesh_scan.cuh states the scan's block size");
 constexpr uint32_t TOP_THREADS = 1024;                                              // the single-CTA scan over block sums
 constexpr uint32_t LOCAL_BITS = 13;   // per point: vertex offset inside its block (< 3 * MC_BLOCK = 6144) | crossing mask << 13
 
@@ -399,8 +403,10 @@ struct MeshWs {
 
 inline uint32_t blocks(uint64_t n, uint32_t per) { return (uint32_t)((n + per - 1) / per); }
 
+}  // namespace
+
 // exclusive scan of a[0..len) in place, sum -> *total (device)
-int scan_u32(cudaStream_t s, uint32_t* a, uint32_t len, uint32_t* bsum, uint32_t* total) {
+int ngp_mesh::scan_u32(cudaStream_t s, uint32_t* a, uint32_t len, uint32_t* bsum, uint32_t* total) {
     const uint32_t nb = blocks(len, SC_BLOCK);
     if (nb == 0) return 0;
     scan_part_kernel<<<nb, SC_THREADS, 0, s>>>(a, len, bsum);
@@ -411,6 +417,8 @@ int scan_u32(cudaStream_t s, uint32_t* a, uint32_t len, uint32_t* bsum, uint32_t
     NGP_LAUNCH_CHECK();
     return 0;
 }
+
+namespace {
 
 // vertex -> triangle incidence lists, each ascending; status bit 0 = a triangle index out of range (that corner is ignored)
 int build_csr(cudaStream_t s, uint32_t nv, uint32_t nt, const int32_t* tris, const MeshWs& w) {

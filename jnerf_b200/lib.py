@@ -34,6 +34,8 @@ SIGNATURES = {
     "ngp_marching_cubes": (_i32, [_vp, _u32, _vp, _f32, _vp, _vp, _u64, _vp, _u64, _vp]),
     "ngp_mesh_largest_component": (_i32, [_vp, _u64, _u64, _vp, _vp, _vp, _vp, _vp, _vp]),
     "ngp_mesh_vertex_normals": (_i32, [_vp, _u64, _u64, _vp, _vp, _vp, _vp]),
+    "ngp_mesh_smooth_workspace_bytes": (_i32, [_u32, _u32, _vp]),
+    "ngp_mesh_smooth": (_i32, [_vp, _u32, _vp, _u32, _u32, _vp, _u64, _vp, _vp]),
     "ngp_render_workspace_bytes": (_i32, [_u32, _u32, _vp]),
     "ngp_render_init": (_i32, [_vp, _u32, _u32, _vp, _f32, _f32, _vp, _vp, _f32, _f32, _u32, _i32, _u64, _u64, _u32, _vp, _vp, _vp, _vp]),
     "ngp_render_march_round": (_i32, [_vp, _u32, _u32, _vp, _u32, _u32, _f32, _f32, _vp, _vp, _vp, _f32, _u32, _i32]),

@@ -155,7 +155,7 @@ def density_fwd(pos, grid, levels, wd):
     return out
 
 
-# ---- mesh extraction (include/ngp_b200.h M1-M4; tools/extract_mesh.py of the reference) ----
+# ---- mesh extraction (include/ngp_b200.h M1-M6; tools/extract_mesh.py of the reference) ----
 def _mesh_workspace(device, n=0, n_verts=0, n_tris=0):
     b = np.zeros(1, np.uint64)
     lib.call("ngp_mesh_workspace_bytes", int(n), int(n_verts), int(n_tris), b.ctypes.data)
@@ -210,6 +210,32 @@ def mesh_vertex_normals(verts, tris, workspace=None):
     normals = torch.empty_like(verts)
     lib.call("ngp_mesh_vertex_normals", _stream(), V, T, _p(verts), _p(tris) if T else None, _p(workspace), _p(normals))
     return normals
+
+
+SMOOTH_METHODS = ("auto", "constrained", "gaussian")
+
+
+def mesh_smooth_workspace(n, method="auto", device="cuda"):
+    b = np.zeros(1, np.uint64)
+    lib.call("ngp_mesh_smooth_workspace_bytes", int(n), SMOOTH_METHODS.index(method), b.ctypes.data)
+    return torch.empty(int(b[0]), dtype=torch.uint8, device=device)
+
+
+def mesh_smooth(field, method="auto", max_iters=250, workspace=None):
+    """PyMCubes' smooth() of an (n, n, n) fp32 lattice, to be marched at iso 0: "constrained" (signed distance, then a bounded Jacobi
+    solve on the band |D| < 4), "gaussian" (sigma 3 of field - 0.5) or "auto" (constrained up to 512^3).  Returns (field_out, info) with
+    info = {"method", "iterations", "band_variables"}."""
+    n = field.shape[0]
+    if method not in SMOOTH_METHODS:
+        raise ValueError(f"mesh_smooth: method must be one of {SMOOTH_METHODS}, got {method!r}")
+    assert field.dim() == 3 and field.shape == (n, n, n) and field.dtype == torch.float32
+    if workspace is None:
+        workspace = mesh_smooth_workspace(n, method, field.device)
+    out = torch.empty_like(field)
+    info = np.zeros(3, np.uint32)
+    lib.call("ngp_mesh_smooth", _stream(), n, _p(field), SMOOTH_METHODS.index(method), int(max_iters), _p(workspace), workspace.numel(), _p(out),
+             info.ctypes.data)
+    return out, dict(method=SMOOTH_METHODS[int(info[0])], iterations=int(info[1]), band_variables=int(info[2]))
 
 
 # ---- whole-frame renderer with early ray termination (include/ngp_b200.h V1-V4) ----

@@ -863,12 +863,14 @@ class Runner:
         return psnr
 
     @torch.no_grad()
-    def extract_mesh(self, out_dir, resolution=512):
+    def extract_mesh(self, out_dir, resolution=512, mcube_smooth=False):
         """tools/extract_mesh.py of the reference on the device: the density lattice of the unit cube (:42-70), marching cubes at 0.5
         (:78) in the PLY frame (:80-84) -> out_dir/mesh-origin.ply, the largest edge-connected component (:92-97), area-weighted vertex
         normals (:106), one colour ray per vertex through the march / network / inference-composite kernels (:108-135) ->
         out_dir/mesh-color.ply.  The colour ray starts 0.2 outside the vertex and runs along the unit normal into the object (towards
-        higher density), in model space (DESIGN.md section 7).  Returns the arrays, the counts and the device time of each stage."""
+        higher density), in model space (DESIGN.md section 7).  mcube_smooth (:74-78): the lattice is smoothed (ops.mesh_smooth, method
+        auto) and marched at 0 instead, which removes the terraces of the integer density field; the result then also holds the
+        smoothing's info under "smooth".  Returns the arrays, the counts and the device time of each stage."""
         import os
         from .utils.ply import write_ply
         assert self.fast, "extract_mesh drives the fused network kernels"
@@ -879,19 +881,25 @@ class Runner:
             raise ValueError(f"extract_mesh: resolution {N} is outside [2, 1024]")
         os.makedirs(out_dir, exist_ok=True)
         s, m = self.sampler, self.model
-        ev = [torch.cuda.Event(enable_timing=True) for _ in range(6)]
-        ev[0].record()
+        names = ("density_lattice",) + (("smooth",) if mcube_smooth else ()) + ("marching_cubes", "write_origin", "component_normals", "colour")
+        ev = [torch.cuda.Event(enable_timing=True) for _ in range(len(names) + 1)]
+        stamps = iter(ev)                                             # one event after each stage, in the order of `names`
+        next(stamps).record()
         field = ops.density_lattice(N, m.pos_encoder.m_grid, m.pos_encoder.levels, m.density_mlp.con_weights)
-        ev[1].record()
-        verts0, tris0 = ops.marching_cubes(field, 0.5)
-        ev[2].record()
+        next(stamps).record()
+        smooth = None
+        if mcube_smooth:
+            field, smooth = ops.mesh_smooth(field)
+            next(stamps).record()
+        verts0, tris0 = ops.marching_cubes(field, 0.0 if mcube_smooth else 0.5)
+        next(stamps).record()
         del field
         v0_host, t0_host = verts0.cpu().numpy(), tris0.cpu().numpy()
         write_ply(os.path.join(out_dir, "mesh-origin.ply"), v0_host, t0_host)
-        ev[3].record()
+        next(stamps).record()
         verts, tris = ops.mesh_largest_component(verts0, tris0)
         normals = ops.mesh_vertex_normals(verts, tris)
-        ev[4].record()
+        next(stamps).record()
         # back to model space (x/y swapped again); the ray runs against the outward normal, into the object
         perm = torch.tensor([1, 0, 2], device=verts.device)
         v_model, n_model = verts[:, perm], normals[:, perm]
@@ -914,18 +922,20 @@ class Runner:
                             n_dev=counters[1:2], save_enc=False, out=self._infer_net_out)
             c, a = ops.composite_infer(self._infer_net_out, coords, numsteps, s.NERF_CASCADES)
             rgb[p:p + tile], alpha[p:p + tile] = c, a
-        ev[5].record()
+        next(stamps).record()
         # :136-137 in float64, as numpy promotes the reference's integer background colour
         img = rgb.cpu().numpy().astype(np.float64) + np.asarray(self.background_color, np.float64) * (1 - alpha.cpu().numpy().astype(np.float64))
         colors = (img * 255 + 0.5).clip(0, 255).astype(np.uint8)
         v_host, t_host = verts.cpu().numpy(), tris.cpu().numpy()
         write_ply(os.path.join(out_dir, "mesh-color.ply"), v_host, t_host, colors)
         torch.cuda.synchronize()
-        names = ("density_lattice", "marching_cubes", "write_origin", "component_normals", "colour")
         times = {k: round(ev[i].elapsed_time(ev[i + 1]), 3) for i, k in enumerate(names)}
-        return dict(vertices=v_host, triangles=t_host, normals=normals.cpu().numpy(), colors=colors, origins=origins.cpu().numpy(),
-                    dirs=dirs.cpu().numpy(), n_verts_origin=int(v0_host.shape[0]), n_tris_origin=int(t0_host.shape[0]),
-                    n_verts=int(v_host.shape[0]), n_tris=int(t_host.shape[0]), stage_ms=times)
+        res = dict(vertices=v_host, triangles=t_host, normals=normals.cpu().numpy(), colors=colors, origins=origins.cpu().numpy(),
+                   dirs=dirs.cpu().numpy(), n_verts_origin=int(v0_host.shape[0]), n_tris_origin=int(t0_host.shape[0]),
+                   n_verts=int(v_host.shape[0]), n_tris=int(t_host.shape[0]), stage_ms=times)
+        if mcube_smooth:
+            res["smooth"] = smooth
+        return res
 
     @torch.no_grad()
     def psnr(self, dataset_mode="val", max_images=None):
