@@ -100,8 +100,14 @@ class DensityGridSampler(Module):
     def sample(self, img_ids, rays_o, rays_d, rgb_target=None, is_training=False, ray_index_offset=0):
         """ray_index_offset: index of rays_o[0] in the global (all-rank) ray batch -- the per-ray jitter stream is indexed by the
         global ray id so that a data-parallel shard reproduces the single-GPU samples (ray_sampler.h:30)."""
-        if is_training and self.cfg.m_training_step % self.update_den_freq == 0:
-            self.update_density_grid()
+        if is_training:
+            if self.cfg.m_training_step % self.update_den_freq == 0:
+                self.update_density_grid()
+            self._rays_numsteps, self._rays_numsteps_compacted, self._counters_compacted, self._coords = self.sample_front(
+                rays_o, rays_d, self._coords_raw, ray_index_offset)
+            if self.cfg.m_training_step % self.update_den_freq == self.update_den_freq - 1:
+                self.update_batch_rays()
+            return self._coords[:, :3], self._coords[:, 4:]
         if rays_o.shape[0] > self._march_ws_rays:
             self._ensure_march_ws(2 * rays_o.shape[0])
         coords, rays_index, rays_numsteps, counters = ops.march(
@@ -110,26 +116,17 @@ class DensityGridSampler(Module):
             ops.pcg32_advance(self.rng.copy(), ray_index_offset * 8) if ray_index_offset else self.rng, coords=self._coords_raw, workspace=self._march_ws)
         ops.pcg32_advance(self.rng)                                    # rng.advance(), ray_sampler.py:61
         self._rays_numsteps = rays_numsteps
-        if not is_training:
-            samples = int(counters[1].item())                          # ray_sampler.py:70 (inference only here)
-            samples = min(samples, self.max_samples)
-            self._coords = coords[:samples]
-            self._rays_numsteps_compacted = rays_numsteps
-            return self._coords[:, :3], self._coords[:, 4:]
-        cap = self.target_batch_size
-        _, ns_c, cnt_c = ops.compact(coords, rays_numsteps, cap, alias=True)
-        self.measured_batch_size += cnt_c[0:1]
-        if self.cfg.m_training_step % self.update_den_freq == self.update_den_freq - 1:
-            self.update_batch_rays()
-        self._coords = coords[:cap]
-        self._rays_numsteps_compacted = ns_c
-        self._counters_compacted = cnt_c
+        samples = int(counters[1].item())                              # ray_sampler.py:70 (inference only here)
+        samples = min(samples, self.max_samples)
+        self._coords = coords[:samples]
+        self._rays_numsteps_compacted = rays_numsteps
         return self._coords[:, :3], self._coords[:, 4:]
 
     def sample_front(self, rays_o, rays_d, coords_raw, ray_index_offset=0):
-        """Training-mode march + compaction into a caller-owned coordinate buffer, returning the step's bookkeeping instead of
-        keeping it on the sampler: the runner's software pipeline runs this for step i+1 (on a second stream) while step i still
-        reads its own rows.  The caller runs the occupancy-grid update and the ray-batch adaptation around it."""
+        """Training-mode march + compaction into a caller-owned coordinate buffer, returning the step's bookkeeping
+        (rays_numsteps, rays_numsteps_compacted, counters_compacted, coords) instead of keeping it on the sampler: the runner's
+        software pipeline runs this for step i+1 (on a second stream) while step i still reads its own rows; sample() keeps it.
+        The caller runs the occupancy-grid update and the ray-batch adaptation around it."""
         if rays_o.shape[0] > self._march_ws_rays:
             self._ensure_march_ws(2 * rays_o.shape[0])
         coords, _, rays_numsteps, _ = ops.march(rays_o.contiguous(), rays_d.contiguous(), self.density_grid_bitfield, self.aabb_range,

@@ -1,7 +1,7 @@
 """The Runner's folded optimizer tail (ops.network_bwd_fx + one ops.train_sweep per step) without a GPU: the CPU stand-in of
 tests/cpu_backend.py, extended by stand-ins of the two new operators.  Checks the call sequence of the sequential and the pipelined
-step, where the next step's front may start with NGP_PIPE_AT=bwd, that the folded step trains exactly as the per-tensor sweeps do, and that under the
-plain stand-in (no stand-ins for the new operators) the Runner makes the per-tensor calls."""
+step, where the next step's front may start with the step in flight, that the folded step trains exactly as the per-tensor sweeps
+do, and that under the plain stand-in (no stand-ins for the new operators) the Runner makes the per-tensor calls."""
 import pytest
 import torch
 
@@ -88,19 +88,15 @@ def test_folded_sequential_step_is_one_backward_and_one_sweep(monkeypatch, fold_
     assert not r._fx.any() and not r._w_part.any()                 # the sweep leaves the scratch cleared
 
 
-def test_folded_pipelined_step_starts_the_next_front_after_the_backward(monkeypatch, fold_backend):
+def test_folded_pipelined_step_starts_the_next_front_with_the_step(monkeypatch, fold_backend):
     r, fake = make_runner(monkeypatch, pipeline=True)
-    assert r._fx is not None and r._pipe["at"] == "front"            # the default: the next front may start with the step
-    monkeypatch.setenv("NGP_PIPE_AT", "bwd")
-    r, fake = make_runner(monkeypatch, pipeline=True)
-    assert r._pipe["at"] == "bwd"
+    assert r._fx is not None and r._pipe["at"] == "front"            # the next front may start as soon as the step in flight does
     r.train_step()
     r._pipe["mid"] = _MarkEvent(fake.calls)
     fake.calls.clear()
     r.train_step()
-    back = ["network_fwd", "composite_loss_bwd", "network_bwd_fx", "front may start", "train_sweep"]
-    assert fake.calls[:len(back)] == back, fake.calls
-    assert fake.calls[len(back):][:2] == ["prepare_batch", "march"]   # the front of the next step, enqueued behind the mark
+    step = ["front may start", "network_fwd", "composite_loss_bwd", "network_bwd_fx", "train_sweep", "prepare_batch", "march", "compact"]
+    assert fake.calls == step, fake.calls                           # this step's back, then the front of the next step behind the mark
     assert fake.calls.count("train_sweep") == 1 and "adam_ema" not in fake.calls and "network_bwd" not in fake.calls
 
 
