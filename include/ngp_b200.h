@@ -114,6 +114,24 @@ int ngp_network_bwd_fx(void* stream, uint32_t n_max, const uint32_t* n_dev, cons
 int ngp_density_fwd(void* stream, uint32_t n, const float* pos, const void* grid, const void* levels_dev,
                     const void* w_density, void* sigma_out);
 
+/* ---- F1-F4  vanilla NeRF: FrequencyEncoder + OriginNeRFNetworks (position_encoders/freq_encoder/freq_encoder.py:22-50,
+ * models/networks/ori_nerf_network.py:10-70), csrc/nerf_mlp.cu, DESIGN.md section 10 ---------------------------------------------
+ * params: ONE flat fp16 vector of *count_out (ngp_nerf_param_count) entries, 16-byte aligned, in the kernels' padded layout (DESIGN.md
+ * section 10; jnerf_b200/plugin/nerf.py maps it to the reference's parameter names).
+ * F1: the sizes of the forward's saved activations and of the backward's scratch for n_max rows (~5 KB a row each). */
+int ngp_nerf_param_count(uint64_t* count_out);
+int ngp_nerf_workspace_bytes(uint32_t n_max, uint64_t* saved_bytes, uint64_t* scratch_bytes);
+/* F2: OriginNeRFNetworks.execute (ori_nerf_network.py:34-56) on NerfCoordinate rows coords (n_max,7) f32: pos = row[0:3],
+ * dir = row[4:7] -> out (n_max,4) fp16 {rgb, alpha}, the layout the composite kernels read.  n_dev as for ngp_network_fwd: rows at
+ * or past it are not written.  saved (may be NULL): every layer's input, what ngp_nerf_bwd reads. */
+int ngp_nerf_fwd(void* stream, uint32_t n_max, const uint32_t* n_dev, const float* coords, const void* params, void* out, void* saved);
+/* F3: OriginNeRFNetworks.density (ori_nerf_network.py:58-67): pos (n,3) f32 -> alpha (n) fp16, bit for bit column 3 of ngp_nerf_fwd */
+int ngp_nerf_density(void* stream, uint32_t n, const float* pos, const void* params, void* sigma_out);
+/* F4: backward of F2 from dout (n_max,4) fp16 and F2's saved activations -> grad (one fp32 per parameter, OVERWRITTEN) of every
+ * weight and bias.  No gradient into the encoding or the coordinates.  Deterministic: no float atomics, sums in a fixed order. */
+int ngp_nerf_bwd(void* stream, uint32_t n_max, const uint32_t* n_dev, const void* params, const void* saved, const void* dout, void* scratch,
+                 float* grad);
+
 /* ---- M1-M4  mesh extraction (tools/extract_mesh.py of the reference: a trained model -> mesh-origin.ply / mesh-color.ply) --------
  * Resolution n must be in [2, 1024]; vertices are (V,3) f32, triangles (T,3) int32 (V, T < 2^31); counts are 64-bit.
  * workspace: *bytes_out of ngp_mesh_workspace_bytes(n, 0, 0, .) for ngp_marching_cubes, of (0, V, T, .) for the other two.

@@ -16,6 +16,7 @@ SOURCES = {
     "hash_encode.cu": [],
     "mlp_tc.cu": [],
     "fused_net.cu": [],
+    "nerf_mlp.cu": [],
     "sampler.cu": ["-fmad=false"],
     "grid_update.cu": ["-fmad=false"],
     "mesh.cu": ["-fmad=false"],

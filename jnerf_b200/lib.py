@@ -29,6 +29,11 @@ SIGNATURES = {
     "ngp_network_bwd_fx_bytes": (_i32, [_u64, _vp, _vp]),
     "ngp_network_bwd_fx": (_i32, [_vp, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _u32, _vp, _u64, _vp, _u64]),
     "ngp_density_fwd": (_i32, [_vp, _u32, _vp, _vp, _vp, _vp, _vp]),
+    "ngp_nerf_param_count": (_i32, [_vp]),
+    "ngp_nerf_workspace_bytes": (_i32, [_u32, _vp, _vp]),
+    "ngp_nerf_fwd": (_i32, [_vp, _u32, _vp, _vp, _vp, _vp, _vp]),
+    "ngp_nerf_density": (_i32, [_vp, _u32, _vp, _vp, _vp]),
+    "ngp_nerf_bwd": (_i32, [_vp, _u32, _vp, _vp, _vp, _vp, _vp, _vp]),
     "ngp_mesh_workspace_bytes": (_i32, [_u32, _u64, _u64, _vp]),
     "ngp_density_lattice": (_i32, [_vp, _u32, _vp, _vp, _vp, _vp]),
     "ngp_marching_cubes": (_i32, [_vp, _u32, _vp, _f32, _vp, _vp, _u64, _vp, _u64, _vp]),
@@ -84,6 +89,7 @@ KERNELS_PER_CALL = {
     "ngp_blend_target": 1, "ngp_step_state_set": 1, "ngp_step_state_tick": 1, "ngp_prepare_batch_dev": 1, "ngp_march_dev": 3, "ngp_adam_ema_dev": 1,
     "ngp_density_lattice": 1, "ngp_marching_cubes": 3, "ngp_mesh_largest_component": 18, "ngp_mesh_vertex_normals": 7,
     "ngp_render_init": 3, "ngp_render_march_round": 3, "ngp_render_composite_round": 3,
+    "ngp_nerf_fwd": 1, "ngp_nerf_density": 1, "ngp_nerf_bwd": 3,
 }
 launch_count = 0
 _lib = None

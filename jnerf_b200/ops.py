@@ -155,6 +155,45 @@ def density_fwd(pos, grid, levels, wd):
     return out
 
 
+# ---- vanilla NeRF (include/ngp_b200.h F1-F4; the parameter layout is plugin/nerf.py's) ----
+def nerf_param_count():
+    b = np.zeros(1, np.uint64)
+    lib.call("ngp_nerf_param_count", b.ctypes.data)
+    return int(b[0])
+
+
+def nerf_workspace_bytes(n):
+    """(bytes of the forward's saved activations, bytes of the backward's scratch) for n rows."""
+    b = np.zeros(2, np.uint64)
+    lib.call("ngp_nerf_workspace_bytes", int(n), b.ctypes.data, b[1:].ctypes.data)
+    return int(b[0]), int(b[1])
+
+
+def nerf_fwd(coords, params, n_dev=None, save=False, out=None):
+    """(N,7) NerfCoordinate rows -> ((N,4) fp16 {rgb, alpha}, saved activations for nerf_bwd or None)."""
+    n = coords.shape[0]
+    if out is None:
+        out = torch.empty((n, 4), dtype=torch.float16, device=coords.device)
+    saved = torch.empty(max(nerf_workspace_bytes(n)[0], 16), dtype=torch.uint8, device=coords.device) if save else None
+    lib.call("ngp_nerf_fwd", _stream(), n, _p(n_dev), _p(coords), _p(params), _p(out), _p(saved))
+    return out, saved
+
+
+def nerf_density(pos, params):
+    out = torch.empty(pos.shape[0], dtype=torch.float16, device=pos.device)
+    lib.call("ngp_nerf_density", _stream(), pos.shape[0], _p(pos), _p(params), _p(out))
+    return out
+
+
+def nerf_bwd(params, saved, dout, n_dev=None):
+    """dout (N,4) fp16 + nerf_fwd's saved activations -> fp32 gradient of the flat parameter vector."""
+    n = dout.shape[0]
+    scratch = torch.empty(nerf_workspace_bytes(n)[1], dtype=torch.uint8, device=dout.device)
+    grad = torch.empty(params.numel(), dtype=torch.float32, device=dout.device)
+    lib.call("ngp_nerf_bwd", _stream(), n, _p(n_dev), _p(params), _p(saved), _p(dout), _p(scratch), _p(grad))
+    return grad
+
+
 # ---- mesh extraction (include/ngp_b200.h M1-M6; tools/extract_mesh.py of the reference) ----
 def _mesh_workspace(device, n=0, n_verts=0, n_tris=0):
     b = np.zeros(1, np.uint64)
@@ -266,18 +305,19 @@ def render_workspace(n_rays, workspace=None, capacity=RENDER_CAPACITY):
 
 
 def render_rays(rays_o, rays_d, bitfield, aabb, cone_angle, near, cascades, const_dt, rng, grid, levels, wd, wr, jitter_tile,
-                min_transmittance=0.0, capacity=RENDER_CAPACITY, workspace=None):
+                min_transmittance=0.0, capacity=RENDER_CAPACITY, workspace=None, net=None):
     """Render R rays (model space) to (rgb (R,3) without background, alpha (R,1) = 1 - T, n_samples (R,) int32, rounds).
     Each ray composites the samples ngp_march gives it under the jitter layout of `jitter_tile`-ray tiles, in order, and stops after the
     first sample that brings its transmittance below `min_transmittance` (0: never).  `rng` is not advanced here: the caller moves it
-    on by ceil(R / jitter_tile) * 2^32, as the tiled renderer would.  One 4-byte read-back per round."""
+    on by ceil(R / jitter_tile) * 2^32, as the tiled renderer would.  One 4-byte read-back per round.
+    net: the network as net(rows, n_dev, out) instead of the fused NGP network of (grid, levels, wd, wr), e.g. OriginNeRFNetworks.infer."""
     import ctypes
     R, dev = rays_o.shape[0], rays_o.device
     nbytes, off_rows, off_net, off_cnt = render_workspace_layout(R, capacity)
     if workspace is None or workspace.numel() < nbytes:
         workspace = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
     rows = workspace[off_rows:off_rows + 28 * capacity].view(torch.float32).view(capacity, 7)
-    net = workspace[off_net:off_net + 8 * capacity].view(torch.float16).view(capacity, 4)
+    out_rows = workspace[off_net:off_net + 8 * capacity].view(torch.float16).view(capacity, 4)
     n_rows = workspace[off_cnt:off_cnt + 4].view(torch.int32)
     rgb = torch.empty((R, 3), dtype=torch.float32, device=dev)
     alpha = torch.empty((R, 1), dtype=torch.float32, device=dev)
@@ -293,7 +333,10 @@ def render_rays(rays_o, rays_d, bitfield, aabb, cone_angle, near, cascades, cons
         lib.call("ngp_render_march_round", _stream(), R, int(capacity), _p(workspace), n_alive, k, float(aabb[0]), float(aabb[1]), _p(rays_o),
                  _p(rays_d), _p(bitfield), float(cone_angle), int(cascades), int(const_dt))
         bound = min(n_alive, int(capacity) // k) * k                  # rows this round can hold: the network's grid covers no more
-        network_fwd(rows[:bound], grid, levels, wd, wr, n_dev=n_rows, save_enc=False, out=net[:bound])
+        if net is None:
+            network_fwd(rows[:bound], grid, levels, wd, wr, n_dev=n_rows, save_enc=False, out=out_rows[:bound])
+        else:
+            net(rows[:bound], n_rows, out_rows[:bound])
         lib.call("ngp_render_composite_round", _stream(), R, int(capacity), _p(workspace), n_alive, k, float(min_transmittance), int(cascades),
                  _p(rgb), _p(alpha), _p(n_samples), ap)
         rounds += 1

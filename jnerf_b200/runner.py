@@ -53,6 +53,8 @@ class Runner:
         cfg.m_training_step = 0
         self.val_freq = 4096
         self.fast = bool(getattr(self.model, "fused", False))
+        # the march / network / composite renderers drive the fused NGP kernels or a model with its own inference forward (infer)
+        self._can_infer = self.fast or hasattr(self.model, "infer")
         # state the evaluation / checkpoint code reads on EVERY kind of model (fused or the nn.Linear fallback)
         self._table_work, self._pending_epoch = None, None
         self._host_stage = None
@@ -656,7 +658,7 @@ class Runner:
         """(rgb (R,3) without background, alpha (R,1)) of the rays through march -> fused network -> inference composite, in tiles of
         n_rays_per_batch rays (the last one as short as the rays leave it); one rng.advance() per tile.  The march's device-side
         counter bounds the network kernel: nothing is read back."""
-        s, m = self.sampler, self.model
+        s = self.sampler
         tile = self.cfg.n_rays_per_batch
         rgb = torch.empty((rays_o.shape[0], 3), device=rays_o.device)
         alpha = torch.empty((rays_o.shape[0], 1), device=rays_o.device)
@@ -668,10 +670,18 @@ class Runner:
                 rays_o[p:p + tile].contiguous(), rays_d[p:p + tile].contiguous(), s.density_grid_bitfield, s.aabb_range, s.max_samples,
                 s.cone_angle_constant, s.near_distance, s.NERF_CASCADES, s.const_dt, s.rng, coords=s._coords_raw, workspace=s._march_ws)
             ops.pcg32_advance(s.rng)                                   # rng.advance(), ray_sampler.py:61
-            ops.network_fwd(coords, m.pos_encoder.m_grid, m.pos_encoder.levels, m.density_mlp.con_weights, m.rgb_mlp.con_weights,
-                            n_dev=counters[1:2], save_enc=False, out=self._infer_net_out)
+            self._net_infer(coords, counters[1:2], self._infer_net_out)
             rgb[p:p + tile], alpha[p:p + tile] = ops.composite_infer(self._infer_net_out, coords, numsteps, s.NERF_CASCADES)
         return rgb, alpha
+
+    def _net_infer(self, rows, n_dev, out):
+        """Inference forward of the model on (N,7) coordinate rows into out (N,4), bounded by the device row count n_dev."""
+        m = self.model
+        if self.fast:
+            ops.network_fwd(rows, m.pos_encoder.m_grid, m.pos_encoder.levels, m.density_mlp.con_weights, m.rgb_mlp.con_weights, n_dev=n_dev,
+                            save_enc=False, out=out)
+        else:
+            m.infer(rows, n_dev, out)
 
     @torch.no_grad()
     def render_img_nosync(self, dataset_mode="train", img_id=0):
@@ -679,7 +689,7 @@ class Runner:
         sample count back with .item() and copies every tile to the host; 157 tiles per 800x800 image).  The march's device-side
         counter bounds the fused network kernel (n_dev), ngp_composite_infer writes into the image buffer, nothing is read back
         before the caller uses the result.  Same kernels, same RNG consumption, same pixels as render_img."""
-        assert self.fast, "render_img_nosync drives the fused network kernel"
+        assert self._can_infer, "render_img_nosync needs the fused NGP model or a model with an inference forward (infer)"
         self._table_ready()
         self._sync_front()
         ds = self.dataset[dataset_mode]
@@ -705,15 +715,20 @@ class Runner:
         Returns (rgb (R,3) without background, alpha (R,1), n_samples (R,), rounds).
         The renderer's workspace (per-ray state, and 144 MB of round rows and network outputs at the default capacity) is kept for the
         next frame; render() and test() release it when they finish, and release_render_workspace() does so at any time."""
-        assert self.fast, "render_rays drives the fused network kernel"
+        assert self._can_infer, "render_rays needs the fused NGP model or a model with an inference forward (infer)"
         self._table_ready()
         self._sync_front()
         s, m = self.sampler, self.model
         R, tile = rays_o.shape[0], int(self.cfg.n_rays_per_batch)
         self._render_ws = ops.render_workspace(R, self._render_ws)
-        out = ops.render_rays(rays_o.contiguous(), rays_d.contiguous(), s.density_grid_bitfield, s.aabb_range, s.cone_angle_constant, s.near_distance,
-                              s.NERF_CASCADES, s.const_dt, s.rng, m.pos_encoder.m_grid, m.pos_encoder.levels, m.density_mlp.con_weights,
-                              m.rgb_mlp.con_weights, tile, min_transmittance=min_transmittance, workspace=self._render_ws)
+        args = (rays_o.contiguous(), rays_d.contiguous(), s.density_grid_bitfield, s.aabb_range, s.cone_angle_constant, s.near_distance,
+                s.NERF_CASCADES, s.const_dt, s.rng)
+        if self.fast:
+            out = ops.render_rays(*args, m.pos_encoder.m_grid, m.pos_encoder.levels, m.density_mlp.con_weights, m.rgb_mlp.con_weights, tile,
+                                  min_transmittance=min_transmittance, workspace=self._render_ws)
+        else:
+            out = ops.render_rays(*args, None, None, None, None, tile, min_transmittance=min_transmittance, workspace=self._render_ws,
+                                  net=m.infer)
         ops.pcg32_advance(s.rng, ((R + tile - 1) // tile) << 32)       # one rng.advance() per tile (ray_sampler.py:61)
         return out
 
@@ -845,7 +860,9 @@ class Runner:
         smoothing's info under "smooth".  Returns the arrays, the counts and the device time of each stage."""
         import os
         from .utils.ply import write_ply
-        assert self.fast, "extract_mesh drives the fused network kernels"
+        if not self.fast:
+            raise NotImplementedError(f"extract_mesh: mesh extraction runs on the fused NGPNetworks kernels; {type(self.model).__name__} "
+                                      "(fp16 / use_fully off, or another model) has no density lattice kernel")
         self._table_ready()
         self._sync_front()
         N = int(resolution)
@@ -925,9 +942,9 @@ class Runner:
             sampler_state["rng"] = torch.from_numpy(self._pipe["pending"]["rng_before"].astype(np.int64))
         ck = {"global_step": self.cfg.m_training_step, "model": self.model.state_dict(), "sampler": sampler_state,
               "optimizer": self.optimizer.state_dict(), "nested_optimizer": nested, "ema_optimizer": self.ema_optimizer.state_dict()}
-        if str(path).endswith(".pkl") and not hasattr(self.model.density_mlp, "con_weights"):
-            raise NotImplementedError("the .pkl interchange format is written for the fused-MLP parameter layout (con_weights); "
-                                      "save the nn.Linear fallback model to a .pt path")
+        if str(path).endswith(".pkl") and not hasattr(getattr(self.model, "density_mlp", None), "con_weights"):
+            raise NotImplementedError(f"the .pkl interchange format is written for the fused-MLP parameter layout (con_weights) of "
+                                      f"NGPNetworks; save {type(self.model).__name__} to a .pt path")
         if str(path).endswith(".pkl"):
             # the reference's params.pkl wire format (runner/runner.py:123-131), readable by its load_ckpt (:133-151)
             from .utils import ckpt_compat as cc
@@ -949,7 +966,7 @@ class Runner:
         if self.world_size > 1:
             import torch.distributed as dist
             dist.barrier(group=self.pg)                              # no peer may still push into this rank's table while it is overwritten
-        if str(path).endswith(".pkl") and not hasattr(self.model.density_mlp, "con_weights"):
+        if str(path).endswith(".pkl") and not hasattr(getattr(self.model, "density_mlp", None), "con_weights"):
             raise NotImplementedError("the .pkl interchange format carries the fused-MLP parameter layout; load a .pt checkpoint instead")
         if str(path).endswith(".pkl"):
             from .utils import ckpt_compat as cc
@@ -1005,5 +1022,28 @@ def fox_cfg(fp16=True, synthetic=True, **over):
     c.update(dataset=dict(train=dict(type=ds_type, root_dir="data/fox", batch_size=4096, mode="train", **extra),
                           test=dict(type=ds_type, root_dir="data/fox", batch_size=4096, mode="test", preload_shuffle=False, **extra)),
              exp_name="fox", const_dt=False)
+    c.update(over)
+    return c
+
+
+def nerf_cfg(fp16=True, synthetic=True, **over):
+    """projects/nerf/configs/nerf_base.py key for key (vanilla NeRF: FrequencyEncoder(10) / FrequencyEncoder(4), OriginNeRFNetworks, Adam
+    lr 1e-2, 512 rays a batch, 200 000 steps); `synthetic` swaps data/lego for the procedural stand-in."""
+    ds_type = "SyntheticNerfDataset" if synthetic else "NerfDataset"
+    c = dict(
+        sampler=dict(type="DensityGridSampler", update_den_freq=16),
+        encoder=dict(pos_encoder=dict(type="FrequencyEncoder", multires=10), dir_encoder=dict(type="FrequencyEncoder", multires=4)),
+        model=dict(type="OriginNeRFNetworks"),
+        loss=dict(type="HuberLoss", delta=0.1),
+        optim=dict(type="Adam", lr=1e-2, eps=1e-15, betas=(0.9, 0.99)),
+        ema=dict(type="EMA", decay=0.95),
+        expdecay=dict(type="ExpDecay", decay_start=20_000, decay_interval=10_000, decay_base=0.33, decay_end=None),
+        dataset_type=ds_type, dataset_dir="data/lego",
+        dataset=dict(train=dict(type=ds_type, root_dir="data/lego", batch_size=512, mode="train"),
+                     val=dict(type=ds_type, root_dir="data/lego", batch_size=512, mode="val", preload_shuffle=False),
+                     test=dict(type=ds_type, root_dir="data/lego", batch_size=512, mode="test", preload_shuffle=False)),
+        exp_name="lego", log_dir="./logs", tot_train_steps=200000, background_color=[0, 0, 0], cone_angle_constant=0.00390625,
+        near_distance=0.2, n_rays_per_batch=512, n_training_steps=16, target_batch_size=1 << 18, const_dt=True, fp16=fp16,
+    )
     c.update(over)
     return c
