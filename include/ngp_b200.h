@@ -132,6 +132,46 @@ int ngp_nerf_density(void* stream, uint32_t n, const float* pos, const void* par
 int ngp_nerf_bwd(void* stream, uint32_t n_max, const uint32_t* n_dev, const void* params, const void* saved, const void* dout, void* scratch,
                  float* grad);
 
+/* ---- P1-P7  Mip-NeRF (contrib/mipnerf of the reference: models/samplers/mip_sampler/mip_sampler.py, utils/miputils.py,
+ * models/networks/mip_network.py, dataset/nerf_datasets.py:22-235), csrc/mip_sampler.cu + csrc/mip_mlp.cu, DESIGN.md section 11 --------
+ * A ray row is 12 floats: origin[3], direction[3] (unnormalised), viewdir[3], base radius, near, far.  t holds S + 1 fenceposts a ray
+ * (S = n_samples <= 128 for the per-ray kernels).  Network rows are (ray, interval) pairs, row r = interval r % S of ray r / S.  The
+ * kernels that draw uniforms give ray g the pcg32 draws [g (S + 1), (g + 1)(S + 1)) of the stream at (rng_state, rng_inc), in fencepost
+ * order; the caller advances its stream by n_rays (S + 1) after such a call.  ray_shape: 0 cone, 1 cylinder.
+ * P1: rays and targets of pixels pix (img * H + y) * W + x: c2w (n_img, 12) row-major 3x4 NeRF camera-to-world, images_rgba
+ * (n_img * H * W, 4) uint8, target = rgb / 255 (n, 3).  Bit for bit the reference's fp32 numpy ray generation. */
+int ngp_mip_rays(void* stream, uint32_t n, const uint32_t* pix, uint32_t W, uint32_t H, const float* c2w, float focal, float near, float far,
+                 const uint8_t* images_rgba, float* rays_out, float* target_out);
+/* P2: sample_along_rays (miputils.py:324-362): t_out (n_rays, S + 1), linear in depth or in disparity, jittered when randomized. */
+int ngp_mip_sample(void* stream, uint32_t n_rays, uint32_t n_samples, const float* rays, int lindisp, int randomized, uint64_t rng_state,
+                   uint64_t rng_inc, float* t_out);
+/* P3: resample_along_rays (:365-408): blur-pool of weights (n_rays, S) + resample_padding, inverse-CDF sampling of S + 1 sorted new
+ * fenceposts within [t_0, t_S] into t_out (not aliasing t). */
+int ngp_mip_resample(void* stream, uint32_t n_rays, uint32_t n_samples, const float* t, const float* weights, float resample_padding,
+                     int randomized, uint64_t rng_state, uint64_t rng_inc, float* t_out);
+/* P4: cast_rays + integrated_pos_enc of degrees [min_deg, min_deg + 8) (:215-275) -> enc_out (N, 48), and pos_enc(viewdir, 0, 4)
+ * (:120-127) -> view_out (N, 27), fp32, the reference's column orders; integrate = 0 is disable_integration.  N = n_rays * S. */
+int ngp_mip_encode(void* stream, uint32_t n_rays, uint32_t n_samples, const float* rays, const float* t, int ray_shape, int integrate, int min_deg,
+                   float* enc_out, float* view_out);
+/* P5: MipNerfMLP.execute on the fused kernels of F1-F4: the encodings of P4 computed on chip, params in the layout of
+ * ngp_nerf_param_count (jnerf_b200/plugin/mip.py maps it to the reference's names), out (N, 4) fp16 {raw rgb, raw density}; saved (may
+ * be NULL, ngp_nerf_workspace_bytes(N) bytes) is what ngp_nerf_bwd reads.  Two calls whose rows are multiples of 128 may save into
+ * consecutive parts of one buffer and share one ngp_nerf_bwd. */
+int ngp_mip_fwd(void* stream, uint32_t n_rays, uint32_t n_samples, const float* rays, const float* t, int ray_shape, int integrate, int min_deg,
+                const void* params, void* out, void* saved);
+/* P6: rays2rgb + volumetric_rendering (mip_sampler.py:83-96, miputils.py:278-321) of raw (n_rays * S, 4) of dtype: rgb (n_rays, 3), acc,
+ * distance (clipped to [t_0, t_S]; t_0 where acc = 0) and, unless NULL, the weights (n_rays, S). */
+int ngp_mip_composite_fwd(void* stream, uint32_t n_rays, uint32_t n_samples, const void* raw, int dtype, const float* t, const float* rays,
+                          float rgb_padding, float density_bias, int white_bkgd, float* rgb_out, float* acc_out, float* distance_out,
+                          float* weights_out);
+/* P7: the training loss of both levels (runner.py:83-92) and its backward in one launch: raw (2 n_rays * S, 4) and t (2 n_rays, S + 1)
+ * hold the coarse level, then the fine level, of the n_rays rays.  loss = coarse_loss_mult L_coarse + L_fine with
+ * L = sum_r mask_r |rgb_r - target_r|^2 / sum_r mask_r (mask NULL: all ones).  rgb_out (2 n_rays, 3), loss_out (2 n_rays) the per-ray
+ * terms of that sum, draw_out (2 n_rays * S, 4) of dtype = grad_scale * dloss / draw. */
+int ngp_mip_composite_loss_bwd(void* stream, uint32_t n_rays, uint32_t n_samples, const void* raw, int dtype, const float* t, const float* rays,
+                               const float* target, const float* mask, float rgb_padding, float density_bias, int white_bkgd, float coarse_loss_mult,
+                               float grad_scale, float* rgb_out, float* loss_out, void* draw_out);
+
 /* ---- M1-M4  mesh extraction (tools/extract_mesh.py of the reference: a trained model -> mesh-origin.ply / mesh-color.ply) --------
  * Resolution n must be in [2, 1024]; vertices are (V,3) f32, triangles (T,3) int32 (V, T < 2^31); counts are 64-bit.
  * workspace: *bytes_out of ngp_mesh_workspace_bytes(n, 0, 0, .) for ngp_marching_cubes, of (0, V, T, .) for the other two.

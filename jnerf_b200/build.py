@@ -10,13 +10,15 @@ LIB = os.path.join(HERE, "libngp_b200.so")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 EXTRA = os.environ.get("NGP_NVCC_FLAGS", "").split()          # extra nvcc flags for experiments
 COMMON = EXTRA + ["-O3", "-std=c++17", "-lineinfo", "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC", "-I", os.path.join(HERE, "..", "include")]
-# per-file extra flags: the sampler / grid / mesh / render code must not contract multiply-adds on its own (bit-exact sample indices)
+# per-file extra flags: the sampler / grid / mesh / render / Mip-NeRF ray code must not contract multiply-adds on its own (bit-exact sample indices)
 SOURCES = {
     "capi.cu": [],
     "hash_encode.cu": [],
     "mlp_tc.cu": [],
     "fused_net.cu": [],
     "nerf_mlp.cu": [],
+    "mip_mlp.cu": [],
+    "mip_sampler.cu": ["-fmad=false"],
     "sampler.cu": ["-fmad=false"],
     "grid_update.cu": ["-fmad=false"],
     "mesh.cu": ["-fmad=false"],

@@ -34,6 +34,13 @@ SIGNATURES = {
     "ngp_nerf_fwd": (_i32, [_vp, _u32, _vp, _vp, _vp, _vp, _vp]),
     "ngp_nerf_density": (_i32, [_vp, _u32, _vp, _vp, _vp]),
     "ngp_nerf_bwd": (_i32, [_vp, _u32, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "ngp_mip_rays": (_i32, [_vp, _u32, _vp, _u32, _u32, _vp, _f32, _f32, _f32, _vp, _vp, _vp]),
+    "ngp_mip_sample": (_i32, [_vp, _u32, _u32, _vp, _i32, _i32, _u64, _u64, _vp]),
+    "ngp_mip_resample": (_i32, [_vp, _u32, _u32, _vp, _vp, _f32, _i32, _u64, _u64, _vp]),
+    "ngp_mip_encode": (_i32, [_vp, _u32, _u32, _vp, _vp, _i32, _i32, _i32, _vp, _vp]),
+    "ngp_mip_fwd": (_i32, [_vp, _u32, _u32, _vp, _vp, _i32, _i32, _i32, _vp, _vp, _vp]),
+    "ngp_mip_composite_fwd": (_i32, [_vp, _u32, _u32, _vp, _i32, _vp, _vp, _f32, _f32, _i32, _vp, _vp, _vp, _vp]),
+    "ngp_mip_composite_loss_bwd": (_i32, [_vp, _u32, _u32, _vp, _i32, _vp, _vp, _vp, _vp, _f32, _f32, _i32, _f32, _f32, _vp, _vp, _vp]),
     "ngp_mesh_workspace_bytes": (_i32, [_u32, _u64, _u64, _vp]),
     "ngp_density_lattice": (_i32, [_vp, _u32, _vp, _vp, _vp, _vp]),
     "ngp_marching_cubes": (_i32, [_vp, _u32, _vp, _f32, _vp, _vp, _u64, _vp, _u64, _vp]),
@@ -90,6 +97,8 @@ KERNELS_PER_CALL = {
     "ngp_density_lattice": 1, "ngp_marching_cubes": 3, "ngp_mesh_largest_component": 18, "ngp_mesh_vertex_normals": 7,
     "ngp_render_init": 3, "ngp_render_march_round": 3, "ngp_render_composite_round": 3,
     "ngp_nerf_fwd": 1, "ngp_nerf_density": 1, "ngp_nerf_bwd": 3,
+    "ngp_mip_rays": 1, "ngp_mip_sample": 1, "ngp_mip_resample": 1, "ngp_mip_encode": 1, "ngp_mip_fwd": 1, "ngp_mip_composite_fwd": 1,
+    "ngp_mip_composite_loss_bwd": 1,
 }
 launch_count = 0
 _lib = None

@@ -194,6 +194,81 @@ def nerf_bwd(params, saved, dout, n_dev=None):
     return grad
 
 
+# ---- Mip-NeRF (include/ngp_b200.h P1-P7; rays (R, 12): origin, direction, viewdir, radius, near, far; t (R, S + 1) fenceposts) ----
+RAY_SHAPES = ("cone", "cylinder")
+
+
+def mip_rays(pix, W, H, c2w, focal, near, far, images):
+    """Blender rays of pixel ids pix ((img * H + y) * W + x) -> (rays (n, 12), target rgb (n, 3)).  images: (n_img * H * W, 4) uint8."""
+    n = pix.numel()
+    rays = torch.empty((n, 12), dtype=torch.float32, device=pix.device)
+    target = torch.empty((n, 3), dtype=torch.float32, device=pix.device)
+    assert images.dtype == torch.uint8
+    lib.call("ngp_mip_rays", _stream(), n, _p(pix), int(W), int(H), _p(c2w), float(focal), float(near), float(far), _p(images), _p(rays), _p(target))
+    return rays, target
+
+
+def mip_sample(rays, n_samples, lindisp, randomized, rng):
+    """(R, S + 1) stratified fenceposts; ray g takes the draws [g (S + 1), (g + 1)(S + 1)) of the pcg32 stream `rng` (not advanced here)."""
+    t = torch.empty((rays.shape[0], n_samples + 1), dtype=torch.float32, device=rays.device)
+    lib.call("ngp_mip_sample", _stream(), rays.shape[0], int(n_samples), _p(rays), int(bool(lindisp)), int(bool(randomized)), int(rng[0]), int(rng[1]), _p(t))
+    return t
+
+
+def mip_resample(t, weights, resample_padding, randomized, rng):
+    """(R, S + 1) fenceposts resampled from the blurred weights (R, S); same pcg32 offsets as mip_sample."""
+    out = torch.empty_like(t)
+    lib.call("ngp_mip_resample", _stream(), t.shape[0], t.shape[1] - 1, _p(t), _p(weights), float(resample_padding), int(bool(randomized)), int(rng[0]),
+             int(rng[1]), _p(out))
+    return out
+
+
+def mip_encode(rays, t, ray_shape="cone", integrate=True, min_deg=0):
+    """fp32 (IPE (N, 48), view encoding (N, 27)) of the N = R * S intervals, in the reference's column orders."""
+    R, S = t.shape[0], t.shape[1] - 1
+    enc = torch.empty((R * S, 48), dtype=torch.float32, device=t.device)
+    view = torch.empty((R * S, 27), dtype=torch.float32, device=t.device)
+    lib.call("ngp_mip_encode", _stream(), R, S, _p(rays), _p(t), RAY_SHAPES.index(ray_shape), int(bool(integrate)), int(min_deg), _p(enc), _p(view))
+    return enc, view
+
+
+def mip_fwd(rays, t, params, ray_shape="cone", integrate=True, min_deg=0, out=None, saved=None):
+    """The fused MipNerfMLP forward: (R * S, 4) fp16 {raw rgb, raw density}.  saved: None, or a uint8 buffer of at least
+    nerf_workspace_bytes(R * S)[0] bytes for nerf_bwd."""
+    R, S = t.shape[0], t.shape[1] - 1
+    if out is None:
+        out = torch.empty((R * S, 4), dtype=torch.float16, device=t.device)
+    lib.call("ngp_mip_fwd", _stream(), R, S, _p(rays), _p(t), RAY_SHAPES.index(ray_shape), int(bool(integrate)), int(min_deg), _p(params), _p(out),
+             _p(saved))
+    return out
+
+
+def mip_composite_fwd(raw, t, rays, rgb_padding, density_bias, white_bkgd, weights=True):
+    """(rgb (R, 3), acc (R,), distance (R,), weights (R, S) or None)."""
+    R, S = t.shape[0], t.shape[1] - 1
+    dev = t.device
+    rgb = torch.empty((R, 3), dtype=torch.float32, device=dev)
+    acc = torch.empty(R, dtype=torch.float32, device=dev)
+    dist = torch.empty(R, dtype=torch.float32, device=dev)
+    w = torch.empty((R, S), dtype=torch.float32, device=dev) if weights else None
+    lib.call("ngp_mip_composite_fwd", _stream(), R, S, _p(raw), _dt(raw), _p(t), _p(rays), float(rgb_padding), float(density_bias), int(bool(white_bkgd)),
+             _p(rgb), _p(acc), _p(dist), _p(w))
+    return rgb, acc, dist, w
+
+
+def mip_composite_loss_bwd(raw, t, rays, target, mask, rgb_padding, density_bias, white_bkgd, coarse_loss_mult, grad_scale=1.0):
+    """Both levels (coarse rows, then fine rows, of the R rays) -> (rgb (2R, 3), per-ray loss terms (2R,), grad_scale * dloss/draw like raw)."""
+    R, S = rays.shape[0], t.shape[1] - 1
+    assert t.shape[0] == 2 * R and raw.shape[0] == 2 * R * S
+    dev = t.device
+    rgb = torch.empty((2 * R, 3), dtype=torch.float32, device=dev)
+    loss = torch.empty(2 * R, dtype=torch.float32, device=dev)
+    draw = torch.empty_like(raw)
+    lib.call("ngp_mip_composite_loss_bwd", _stream(), R, S, _p(raw), _dt(raw), _p(t), _p(rays), _p(target), _p(mask), float(rgb_padding), float(density_bias),
+             int(bool(white_bkgd)), float(coarse_loss_mult), float(grad_scale), _p(rgb), _p(loss), _p(draw))
+    return rgb, loss, draw
+
+
 # ---- mesh extraction (include/ngp_b200.h M1-M6; tools/extract_mesh.py of the reference) ----
 def _mesh_workspace(device, n=0, n_verts=0, n_tris=0):
     b = np.zeros(1, np.uint64)

@@ -44,30 +44,30 @@ REF_LAYERS.update({
 REF_ORDER = [f"pts_linears.{i}" for i in range(8)] + ["views_linears.0", "feature_linear", "alpha_linear", "rgb_linear"]
 
 
-def _kernel_views(flat, name):
-    (o, _), l, r0, cols = REF_LAYERS[name]
+def _kernel_views(flat, name, layers=REF_LAYERS):
+    (o, _), l, r0, cols = layers[name]
     W = flat[W_OFF[l]:W_OFF[l] + OUT[l] * IN[l]].view(OUT[l], IN[l])
     b = flat[W_OFF[l] + OUT[l] * IN[l]:W_OFF[l + 1]]
     return W[r0:r0 + o], b[r0:r0 + o], cols
 
 
-def pack(ref):
-    """{reference name: (weight (out, in), bias (out,))} -> the flat fp16 vector of the kernels."""
+def pack(ref, layers=REF_LAYERS):
+    """{reference name: (weight (out, in), bias (out,))} -> the flat fp16 vector of the kernels (layers: the name table, e.g. plugin/mip.py's)."""
     dev = next(iter(ref.values()))[0].device
     flat = torch.zeros(N_PARAMS, dtype=torch.float16, device=dev)
     for name, (W, b) in ref.items():
-        Wk, bk, cols = _kernel_views(flat, name)
+        Wk, bk, cols = _kernel_views(flat, name, layers)
         for rc, kc, n in cols:
             Wk[:, kc:kc + n] = W[:, rc:rc + n].to(torch.float16)
         bk.copy_(b.to(torch.float16))
     return flat
 
 
-def unpack(flat):
+def unpack(flat, layers=REF_LAYERS):
     """The flat vector (parameters or gradients) -> {reference name: (weight (out, in), bias (out,))} in fp32."""
     out = {}
-    for name, ((o, i), _, _, _) in REF_LAYERS.items():
-        Wk, bk, cols = _kernel_views(flat, name)
+    for name, ((o, i), _, _, _) in layers.items():
+        Wk, bk, cols = _kernel_views(flat, name, layers)
         W = torch.empty((o, i), dtype=torch.float32, device=flat.device)
         for rc, kc, n in cols:
             W[:, rc:rc + n] = Wk[:, kc:kc + n].float()
@@ -75,11 +75,11 @@ def unpack(flat):
     return out
 
 
-def init_reference_params(gen):
+def init_reference_params(gen, layers=REF_LAYERS, order=REF_ORDER):
     """Jittor's nn.Linear initialisation, restated: weight invariant_uniform((out, in)), bias U(+-1/sqrt(in)); fp32."""
     ref = {}
-    for name in REF_ORDER:
-        (o, i) = REF_LAYERS[name][0]
+    for name in order:
+        (o, i) = layers[name][0]
         W = invariant_uniform((o, i), gen)
         b = (torch.rand(o, device="cuda", generator=gen) * 2 - 1) / math.sqrt(i)
         ref[name] = (W, b)

@@ -1,10 +1,11 @@
-"""Adam / ExpDecay / EMA mirrors (optims/{adam,expdecay,ema}.py) on top of ONE fused kernel (ngp_adam_ema).
+"""Adam / ExpDecay / EMA / LinearLog mirrors (optims/{adam,expdecay,ema}.py, contrib/mipnerf optims/linearlog.py) on top of ONE fused kernel (ngp_adam_ema).
 
 Reference step order (runner/runner.py:75-76): optimizer.step(loss) [ExpDecay -> jt.nn.Adam] then
 ema_optimizer.ema_step(), which overwrites the live parameters with the debiased EMA (ema.py:26-37).
 Here `Adam.step` runs backward and, when an EMA is attached to the same parameters, defers the parameter update so
 that `EMA.ema_step` can apply Adam + EMA + gradient zeroing in a single streaming pass.  Without an EMA the same
 kernel runs with decay 0 (pure Adam)."""
+import numpy as np
 import torch
 
 from .. import ops
@@ -129,6 +130,47 @@ class EMA:
 
     def state_dict(self):
         return {"steps": self.steps, "decay": self.decay}
+
+    def load_state_dict(self, sd):
+        self.steps = sd["steps"]
+
+
+@OPTIMS.register_module()
+class LinearLog:
+    """contrib/mipnerf optims/linearlog.py:8-38: lr = delay * exp(log(start_lr) (1 - t) + log(end_lr) t), t = clip(step / max_steps, 0, 1),
+    delay = lr_delay_mult + (1 - lr_delay_mult) sin(pi/2 clip(step / lr_delay_steps, 0, 1)) (1 without a delay), in fp32 as Jittor
+    evaluates it.  start_lr is the nested optimizer's lr, as in the reference (its start_lr argument is not read)."""
+
+    def __init__(self, nested_optimizer, start_lr=5e-4, end_lr=5e-6, max_steps=40000, lr_delay_steps=0, lr_delay_mult=1):
+        self._nested_optimizer = nested_optimizer
+        self.start_lr, self.end_lr, self.max_steps = nested_optimizer.lr, end_lr, max_steps
+        self.lr_delay_steps, self.lr_delay_mult = lr_delay_steps, lr_delay_mult
+        self.steps = 0
+
+    def lr_at(self, step):
+        f = np.float32
+        if self.lr_delay_steps > 0:
+            x = f(np.clip(f(step / self.lr_delay_steps), 0, 1))
+            delay = f(self.lr_delay_mult) + f(1 - self.lr_delay_mult) * np.sin(f(0.5) * f(np.pi) * x)
+        else:
+            delay = f(1.0)
+        t = f(np.clip(f(step / self.max_steps), 0, 1))
+        return float(f(delay * np.exp(np.log(f(self.start_lr)) * (f(1) - t) + np.log(f(self.end_lr)) * t)))
+
+    def advance_lr(self):
+        self._nested_optimizer.lr = self.lr_at(self.steps)
+        self.steps += 1
+        return self._nested_optimizer.lr
+
+    def step(self, loss=None):
+        self.advance_lr()
+        self._nested_optimizer.step(loss)
+
+    def zero_grad(self):
+        return self._nested_optimizer.zero_grad()
+
+    def state_dict(self):
+        return {"steps": self.steps}
 
     def load_state_dict(self, sd):
         self.steps = sd["steps"]
