@@ -328,34 +328,6 @@ int ngp_prepare_batch(void* stream, uint32_t n, const uint32_t* pix_index, uint3
 /* target = rgb*a + bg*(1-a) (runner/runner.py:68) for a batch whose RGBA (n,4) f32 is already gathered (host-fed ray batches) */
 int ngp_blend_target(void* stream, uint32_t n, const float* rgba, const float* bg, float* target);
 
-/* ---- device-resident step state: everything a CUDA-graph replay of one training step must not take as a launch argument ------------
- * The reference passes the sampler's rng state (ops/code_ops/global_vars.py:5-27), the position in the shuffled pixel list
- * (dataset/dataset.py:172) and Adam's step count (optims/adam.py) from the host on every call.  The *_dev entry points below read
- * them from a small device struct instead (ngp_step_state_bytes() bytes, caller-owned), and ngp_step_state_tick advances it on the
- * device exactly as the host would: rng.advance() (ray_sampler.py:61), cursor += pix_advance, step += 1 with the bias-correction /
- * EMA-debias factors of the next step.  ngp_step_state_set (re)loads it from host values. */
-uint64_t ngp_step_state_bytes(void);
-int ngp_step_state_set(void* stream, void* state_dev, uint64_t rng_state, uint64_t rng_inc, uint32_t pix_cursor, uint32_t adam_steps_done,
-                       float lr, float beta1, float beta2, float eps, float ema_decay, float grad_scale);
-int ngp_step_state_tick(void* stream, void* state_dev, uint32_t pix_advance, float lr, float beta1, float beta2, float eps,
-                        float ema_decay, float grad_scale);
-/* ngp_prepare_batch with pix_index = pix_list + state.pix_cursor + pix_offset */
-int ngp_prepare_batch_dev(void* stream, uint32_t n, const uint32_t* pix_list, const void* state_dev, uint32_t pix_offset, uint32_t W,
-                          uint32_t H, const float* xforms, const float* focal, const float* principal, const void* images_rgba,
-                          int image_is_u8, const float* bg, uint32_t* img_id_out, float* rays_o, float* rays_d, float* target);
-/* ngp_march with the rng of the step state; ray_offset = index of ray 0 in the global (all-rank) ray batch */
-int ngp_march_dev(void* stream, uint32_t n_rays, float aabb_lo, float aabb_hi, uint32_t max_samples, const float* rays_o,
-                  const float* rays_d, const uint8_t* bitfield, float cone_angle, float near_distance, uint32_t cascades, int const_dt,
-                  const void* state_dev, uint32_t ray_offset, uint32_t* counters, uint32_t* ray_indices, uint32_t* numsteps,
-                  float* coords, void* workspace);
-/* ngp_adam_ema with lr / betas / eps / step / decay / grad_scale folded into the step state's factors */
-int ngp_adam_ema_dev(void* stream, uint64_t n, void* param, int param_dtype, void* grad, int grad_dtype, float* m, float* v,
-                     float* master, const void* state_dev, int zero_grad);
-/* ngp_train_sweep with the step state's factors */
-int ngp_train_sweep_dev(void* stream, uint64_t n_entries, void* table, float* m, float* v, float* master, void* fx, const float* w_part,
-                        uint32_t bwd_rows, void* w_density, float* wd_m, float* wd_v, float* wd_master, void* w_rgb, float* wr_m,
-                        float* wr_v, float* wr_master, const void* state_dev);
-
 /* pcg32 helpers (ops/op_include/pcg32/pcg32.h): host-side, pure integer */
 void ngp_pcg32_seed(uint64_t initstate, uint64_t initseq, uint64_t* state_inc);
 void ngp_pcg32_advance(uint64_t* state_inc, int64_t delta);

@@ -102,16 +102,14 @@ __device__ __forceinline__ float ray_tmin(float lo, float hi, const float o[3], 
 struct RayState {
     float o[3], d[3], id[3], startt;
 };
-// rng: the kernel arguments, or -- ngp_march_dev -- the device-resident step state (ngp_common.cuh); `ray_offset` = index of ray 0 in
-// the global ray batch (data-parallel shards draw the jitter of the global ray id)
-struct MarchRng { uint64_t state, inc; const NgpStepState* st; uint32_t ray_offset; };
+// `ray_offset` = index of ray 0 in the global ray batch (data-parallel shards draw the jitter of the global ray id)
+struct MarchRng { uint64_t state, inc; uint32_t ray_offset; };
 __device__ __forceinline__ RayState ray_setup(uint32_t i, const float* __restrict__ rays_o, const float* __restrict__ rays_d, float lo,
                                               float hi, float near_distance, float cone, const MarchCfg& c, const MarchRng& mr) {
-    const uint64_t rng_state = mr.st ? mr.st->rng_state : mr.state, rng_inc = mr.st ? mr.st->rng_inc : mr.inc;
     RayState r;
 #pragma unroll
     for (int k = 0; k < 3; ++k) { r.o[k] = rays_o[3 * (size_t)i + k]; r.d[k] = rays_d[3 * (size_t)i + k]; r.id[k] = 1.0f / r.d[k]; }
-    Pcg32 rng{rng_state, rng_inc};
+    Pcg32 rng{mr.state, mr.inc};
     rng.advance((int64_t)(uint32_t)((i + mr.ray_offset) * 8u));               // ray_sampler.h:30, N_MAX_RANDOM_SAMPLES_PER_RAY = 8
     float tmin = fmaxf(ray_tmin(lo, hi, r.o, r.d), near_distance);           // :41-44
     r.startt = __fmaf_rn(calc_dt(c, tmin, cone), rng.next_float(), tmin);    // :48

@@ -206,20 +206,8 @@ struct Pcg32 {
     }
 };
 
-// ---- device-resident step state ---------------------------------------------------------------------
-// Everything that changes from one training step to the next and used to travel as kernel ARGUMENTS -- the pcg32 state of the
-// sampler's jitter stream, the read position in the shuffled pixel list, Adam's step count with the bias-correction factors derived
-// from it -- also lives in this small device struct.  Kernels launched through the *_dev entry points read it instead of their
-// arguments and ngp_step_state_tick advances it on the device, so a whole training step has the same launch parameters every time:
-// it can be captured once in a CUDA graph and replayed (runner.py).
 struct AdamArgs {
     float step_size, b1, b2, eps, decay, debias_old, debias_new, grad_scale;
-};
-struct NgpStepState {
-    uint64_t rng_state, rng_inc;      // sampler rng (global_vars.py:17) BEFORE this step's march
-    uint32_t pix_cursor;              // index of this step's first pixel in the shuffled pixel list (dataset.py:172)
-    uint32_t adam_steps_done;         // Adam / EMA steps applied so far
-    AdamArgs adam;                    // factors for step adam_steps_done + 1
 };
 
 // ---- morton (ray_sampler_header.h:642-667) ----------------------------------------------------------

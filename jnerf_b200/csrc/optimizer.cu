@@ -18,9 +18,7 @@ namespace {
 //  were used per request and the kernel stalled on the LSU queue.)
 template <typename PT, typename GT>
 __global__ void __launch_bounds__(256) adam_ema_kernel(uint64_t n, PT* __restrict__ param, GT* __restrict__ grad, float* __restrict__ m,
-                                                       float* __restrict__ v, float* __restrict__ master, AdamArgs a, int zero_grad,
-                                                       const NgpStepState* __restrict__ st) {
-    if (st) a = st->adam;                                         // *_dev entry point: factors of the current step from device memory
+                                                       float* __restrict__ v, float* __restrict__ master, AdamArgs a, int zero_grad) {
     constexpr int UNROLL = 2;
     const uint64_t n4 = n / 4, T = (uint64_t)gridDim.x * blockDim.x, g = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
     for (uint64_t i0 = g; i0 < n4; i0 += UNROLL * T) {
@@ -97,8 +95,7 @@ __device__ __forceinline__ float2 fx_grad(longlong2 q) {
 
 __global__ void __launch_bounds__(SWEEP_THREADS) train_sweep_kernel(uint64_t n_entries, SweepTensor tab, longlong2* __restrict__ fx,
                                                                     const float* __restrict__ part, uint32_t nparts, SweepTensor wd, SweepTensor wr,
-                                                                    AdamArgs a, const NgpStepState* __restrict__ st) {
-    if (st) a = st->adam;
+                                                                    AdamArgs a) {
     if (blockIdx.x < SWEEP_W_BLOCKS) {
         const uint32_t e = blockIdx.x * SWEEP_THREADS + threadIdx.x;
         if (e >= (uint32_t)W_PART) return;
@@ -180,11 +177,10 @@ template <typename IMG>
 __global__ void prepare_batch_kernel(uint32_t n, const uint32_t* __restrict__ pix, uint32_t W, uint32_t H, const float* __restrict__ xforms,
                                      const float* __restrict__ focal, const float* __restrict__ principal, const IMG* __restrict__ images,
                                      const float* __restrict__ bg, uint32_t* __restrict__ img_id, float* __restrict__ rays_o,
-                                     float* __restrict__ rays_d, float* __restrict__ target, const NgpStepState* __restrict__ st,
-                                     uint32_t pix_offset) {
+                                     float* __restrict__ rays_d, float* __restrict__ target) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const uint32_t px = pix[(st ? st->pix_cursor : 0u) + pix_offset + i];          // *_dev: `pix` is the whole shuffled list
+    const uint32_t px = pix[i];
     const uint32_t id = px / (H * W), off = px % (H * W);
     const float* m = xforms + 12 * (size_t)id;
     const float x = ((off % W) + 0.5f) / W, y = ((off / W) + 0.5f) / H;
@@ -357,64 +353,6 @@ __global__ void dp_wait_kernel(const uint32_t* my_flags, int W, uint32_t epoch) 
 
 extern "C" {
 
-static AdamArgs make_adam_args(float lr, float beta1, float beta2, float eps, uint32_t step, float ema_decay, float grad_scale);
-
-static int adam_launch(void* stream, uint64_t n, void* param, int param_dtype, void* grad, int grad_dtype, float* m, float* v, float* master,
-                       AdamArgs a, int zero_grad, const NgpStepState* st) {
-    if (n == 0) return 0;
-    cudaStream_t s = (cudaStream_t)stream;
-    const uint64_t n4 = (n + 3) / 4;
-    const uint32_t blocks = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((n4 + 511) / 512, (uint64_t)ngp_num_sms() * 32));
-    if (param_dtype == 1 && grad_dtype == 1) adam_ema_kernel<__half, __half><<<blocks, 256, 0, s>>>(n, (__half*)param, (__half*)grad, m, v, master, a, zero_grad, st);
-    else if (param_dtype == 1 && grad_dtype == 0) adam_ema_kernel<__half, float><<<blocks, 256, 0, s>>>(n, (__half*)param, (float*)grad, m, v, master, a, zero_grad, st);
-    else if (param_dtype == 0 && grad_dtype == 0) adam_ema_kernel<float, float><<<blocks, 256, 0, s>>>(n, (float*)param, (float*)grad, m, v, master, a, zero_grad, st);
-    else NGP_REQUIRE(false, "ngp_adam_ema: unsupported dtype combination");
-    NGP_LAUNCH_CHECK();
-    return 0;
-}
-
-int ngp_adam_ema(void* stream, uint64_t n, void* param, int param_dtype, void* grad, int grad_dtype, float grad_scale, float* m, float* v,
-                 float* master, float lr, float beta1, float beta2, float eps, uint32_t step, float ema_decay, int zero_grad) {
-    NGP_REQUIRE(step >= 1, "ngp_adam_ema: step is 1-based");
-    return adam_launch(stream, n, param, param_dtype, grad, grad_dtype, m, v, master, make_adam_args(lr, beta1, beta2, eps, step, ema_decay, grad_scale),
-                       zero_grad, nullptr);
-}
-
-int ngp_adam_ema_dev(void* stream, uint64_t n, void* param, int param_dtype, void* grad, int grad_dtype, float* m, float* v, float* master,
-                     const void* state_dev, int zero_grad) {
-    NGP_REQUIRE(state_dev != nullptr, "ngp_adam_ema_dev: state_dev is required");
-    return adam_launch(stream, n, param, param_dtype, grad, grad_dtype, m, v, master, AdamArgs{}, zero_grad, (const NgpStepState*)state_dev);
-}
-
-static int sweep_launch(void* stream, uint64_t n_entries, void* table, float* m, float* v, float* master, void* fx, const float* w_part,
-                        uint32_t bwd_rows, void* w_density, float* wd_m, float* wd_v, float* wd_master, void* w_rgb, float* wr_m, float* wr_v,
-                        float* wr_master, AdamArgs a, const NgpStepState* st) {
-    NGP_REQUIRE(fx != nullptr && w_part != nullptr, "ngp_train_sweep: the backward's fixed-point scratch and weight-gradient slots are required");
-    const uint32_t blocks = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((n_entries + 4 * SWEEP_THREADS - 1) / (4 * SWEEP_THREADS),
-                                                                           (uint64_t)ngp_num_sms() * 32));
-    train_sweep_kernel<<<SWEEP_W_BLOCKS + blocks, SWEEP_THREADS, 0, (cudaStream_t)stream>>>(
-        n_entries, SweepTensor{(__half*)table, m, v, master}, (longlong2*)fx, w_part, bwd_ctas(bwd_rows),
-        SweepTensor{(__half*)w_density, wd_m, wd_v, wd_master}, SweepTensor{(__half*)w_rgb, wr_m, wr_v, wr_master}, a, st);
-    NGP_LAUNCH_CHECK();
-    return 0;
-}
-
-int ngp_train_sweep(void* stream, uint64_t n_entries, void* table, float* m, float* v, float* master, void* fx, const float* w_part,
-                    uint32_t bwd_rows, void* w_density, float* wd_m, float* wd_v, float* wd_master, void* w_rgb, float* wr_m, float* wr_v,
-                    float* wr_master, float lr, float beta1, float beta2, float eps, uint32_t step, float ema_decay) {
-    NGP_REQUIRE(step >= 1, "ngp_train_sweep: step is 1-based");
-    return sweep_launch(stream, n_entries, table, m, v, master, fx, w_part, bwd_rows, w_density, wd_m, wd_v, wd_master, w_rgb, wr_m, wr_v,
-                        wr_master, make_adam_args(lr, beta1, beta2, eps, step, ema_decay, 1.0f), nullptr);
-}
-
-int ngp_train_sweep_dev(void* stream, uint64_t n_entries, void* table, float* m, float* v, float* master, void* fx, const float* w_part,
-                        uint32_t bwd_rows, void* w_density, float* wd_m, float* wd_v, float* wd_master, void* w_rgb, float* wr_m, float* wr_v,
-                        float* wr_master, const void* state_dev) {
-    NGP_REQUIRE(state_dev != nullptr, "ngp_train_sweep_dev: state_dev is required");
-    return sweep_launch(stream, n_entries, table, m, v, master, fx, w_part, bwd_rows, w_density, wd_m, wd_v, wd_master, w_rgb, wr_m, wr_v,
-                        wr_master, AdamArgs{}, (const NgpStepState*)state_dev);
-}
-
 static AdamArgs make_adam_args(float lr, float beta1, float beta2, float eps, uint32_t step, float ema_decay, float grad_scale) {
     AdamArgs a;
     const double n1 = 1.0 - std::pow((double)beta1, (double)step), n2 = 1.0 - std::pow((double)beta2, (double)step);
@@ -423,6 +361,37 @@ static AdamArgs make_adam_args(float lr, float beta1, float beta2, float eps, ui
     a.debias_old = (float)(1.0 - std::pow((double)ema_decay, (double)step - 1.0));
     a.debias_new = (float)(1.0 / (1.0 - std::pow((double)ema_decay, (double)step)));
     return a;
+}
+
+int ngp_adam_ema(void* stream, uint64_t n, void* param, int param_dtype, void* grad, int grad_dtype, float grad_scale, float* m, float* v,
+                 float* master, float lr, float beta1, float beta2, float eps, uint32_t step, float ema_decay, int zero_grad) {
+    NGP_REQUIRE(step >= 1, "ngp_adam_ema: step is 1-based");
+    if (n == 0) return 0;
+    const AdamArgs a = make_adam_args(lr, beta1, beta2, eps, step, ema_decay, grad_scale);
+    cudaStream_t s = (cudaStream_t)stream;
+    const uint64_t n4 = (n + 3) / 4;
+    const uint32_t blocks = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((n4 + 511) / 512, (uint64_t)ngp_num_sms() * 32));
+    if (param_dtype == 1 && grad_dtype == 1) adam_ema_kernel<__half, __half><<<blocks, 256, 0, s>>>(n, (__half*)param, (__half*)grad, m, v, master, a, zero_grad);
+    else if (param_dtype == 1 && grad_dtype == 0) adam_ema_kernel<__half, float><<<blocks, 256, 0, s>>>(n, (__half*)param, (float*)grad, m, v, master, a, zero_grad);
+    else if (param_dtype == 0 && grad_dtype == 0) adam_ema_kernel<float, float><<<blocks, 256, 0, s>>>(n, (float*)param, (float*)grad, m, v, master, a, zero_grad);
+    else NGP_REQUIRE(false, "ngp_adam_ema: unsupported dtype combination");
+    NGP_LAUNCH_CHECK();
+    return 0;
+}
+
+int ngp_train_sweep(void* stream, uint64_t n_entries, void* table, float* m, float* v, float* master, void* fx, const float* w_part,
+                    uint32_t bwd_rows, void* w_density, float* wd_m, float* wd_v, float* wd_master, void* w_rgb, float* wr_m, float* wr_v,
+                    float* wr_master, float lr, float beta1, float beta2, float eps, uint32_t step, float ema_decay) {
+    NGP_REQUIRE(step >= 1, "ngp_train_sweep: step is 1-based");
+    NGP_REQUIRE(fx != nullptr && w_part != nullptr, "ngp_train_sweep: the backward's fixed-point scratch and weight-gradient slots are required");
+    const uint32_t blocks = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((n_entries + 4 * SWEEP_THREADS - 1) / (4 * SWEEP_THREADS),
+                                                                           (uint64_t)ngp_num_sms() * 32));
+    train_sweep_kernel<<<SWEEP_W_BLOCKS + blocks, SWEEP_THREADS, 0, (cudaStream_t)stream>>>(
+        n_entries, SweepTensor{(__half*)table, m, v, master}, (longlong2*)fx, w_part, bwd_ctas(bwd_rows),
+        SweepTensor{(__half*)w_density, wd_m, wd_v, wd_master}, SweepTensor{(__half*)w_rgb, wr_m, wr_v, wr_master},
+        make_adam_args(lr, beta1, beta2, eps, step, ema_decay, 1.0f));
+    NGP_LAUNCH_CHECK();
+    return 0;
 }
 
 int ngp_dp_exchange_step(void* stream, int world, int rank, uint64_t slice_len, uint32_t n_w, void* const* peer_table,
@@ -490,69 +459,13 @@ int ngp_ipc_close(void* dev_ptr, uint64_t offset) {
     return 0;
 }
 
-static int prepare_batch_launch(void* stream, uint32_t n, const uint32_t* pix, uint32_t W, uint32_t H, const float* xforms, const float* focal,
-                                const float* principal, const void* images_rgba, int image_is_u8, const float* bg, uint32_t* img_id_out,
-                                float* rays_o, float* rays_d, float* target, const NgpStepState* st, uint32_t pix_offset) {
-    if (n == 0) return 0;
-    cudaStream_t s = (cudaStream_t)stream;
-    if (image_is_u8) prepare_batch_kernel<uint8_t><<<(n + 127) / 128, 128, 0, s>>>(n, pix, W, H, xforms, focal, principal, (const uint8_t*)images_rgba, bg, img_id_out, rays_o, rays_d, target, st, pix_offset);
-    else prepare_batch_kernel<float><<<(n + 127) / 128, 128, 0, s>>>(n, pix, W, H, xforms, focal, principal, (const float*)images_rgba, bg, img_id_out, rays_o, rays_d, target, st, pix_offset);
-    NGP_LAUNCH_CHECK();
-    return 0;
-}
-
 int ngp_prepare_batch(void* stream, uint32_t n, const uint32_t* pix_index, uint32_t W, uint32_t H, const float* xforms, const float* focal,
                       const float* principal, const void* images_rgba, int image_is_u8, const float* bg, uint32_t* img_id_out, float* rays_o,
                       float* rays_d, float* target) {
-    return prepare_batch_launch(stream, n, pix_index, W, H, xforms, focal, principal, images_rgba, image_is_u8, bg, img_id_out, rays_o, rays_d, target,
-                                nullptr, 0);
-}
-
-int ngp_prepare_batch_dev(void* stream, uint32_t n, const uint32_t* pix_list, const void* state_dev, uint32_t pix_offset, uint32_t W, uint32_t H,
-                          const float* xforms, const float* focal, const float* principal, const void* images_rgba, int image_is_u8,
-                          const float* bg, uint32_t* img_id_out, float* rays_o, float* rays_d, float* target) {
-    NGP_REQUIRE(state_dev != nullptr, "ngp_prepare_batch_dev: state_dev is required");
-    return prepare_batch_launch(stream, n, pix_list, W, H, xforms, focal, principal, images_rgba, image_is_u8, bg, img_id_out, rays_o, rays_d, target,
-                                (const NgpStepState*)state_dev, pix_offset);
-}
-
-// ---- device-resident step state (ngp_common.cuh: NgpStepState) ----
-__global__ void step_state_set_kernel(NgpStepState* st, uint64_t rng_state, uint64_t rng_inc, uint32_t pix_cursor, uint32_t steps_done, AdamArgs next) {
-    st->rng_state = rng_state; st->rng_inc = rng_inc; st->pix_cursor = pix_cursor; st->adam_steps_done = steps_done; st->adam = next;
-}
-// after a step: the sampler's rng.advance() (ray_sampler.py:61), the pixel cursor, Adam's step count and the factors of the next step
-// (same double-precision expressions as make_adam_args on the host)
-__global__ void step_state_tick_kernel(NgpStepState* st, uint32_t pix_advance, float lr, float beta1, float beta2, float eps, float ema_decay,
-                                       float grad_scale) {
-    Pcg32 rng{st->rng_state, st->rng_inc};
-    rng.advance((int64_t)1 << 32);
-    st->rng_state = rng.state;
-    st->pix_cursor += pix_advance;
-    const uint32_t done = st->adam_steps_done + 1;
-    st->adam_steps_done = done;
-    const double step = (double)done + 1.0;
-    const double n1 = 1.0 - pow((double)beta1, step), n2 = 1.0 - pow((double)beta2, step);
-    AdamArgs a;
-    a.step_size = (float)((double)lr * sqrt(n2) / n1);
-    a.b1 = beta1; a.b2 = beta2; a.eps = eps; a.decay = ema_decay; a.grad_scale = grad_scale;
-    a.debias_old = (float)(1.0 - pow((double)ema_decay, step - 1.0));
-    a.debias_new = (float)(1.0 / (1.0 - pow((double)ema_decay, step)));
-    st->adam = a;
-}
-
-uint64_t ngp_step_state_bytes(void) { return sizeof(NgpStepState); }
-
-int ngp_step_state_set(void* stream, void* state_dev, uint64_t rng_state, uint64_t rng_inc, uint32_t pix_cursor, uint32_t adam_steps_done, float lr,
-                       float beta1, float beta2, float eps, float ema_decay, float grad_scale) {
-    step_state_set_kernel<<<1, 1, 0, (cudaStream_t)stream>>>((NgpStepState*)state_dev, rng_state, rng_inc, pix_cursor, adam_steps_done,
-                                                              make_adam_args(lr, beta1, beta2, eps, adam_steps_done + 1, ema_decay, grad_scale));
-    NGP_LAUNCH_CHECK();
-    return 0;
-}
-
-int ngp_step_state_tick(void* stream, void* state_dev, uint32_t pix_advance, float lr, float beta1, float beta2, float eps, float ema_decay,
-                        float grad_scale) {
-    step_state_tick_kernel<<<1, 1, 0, (cudaStream_t)stream>>>((NgpStepState*)state_dev, pix_advance, lr, beta1, beta2, eps, ema_decay, grad_scale);
+    if (n == 0) return 0;
+    cudaStream_t s = (cudaStream_t)stream;
+    if (image_is_u8) prepare_batch_kernel<uint8_t><<<(n + 127) / 128, 128, 0, s>>>(n, pix_index, W, H, xforms, focal, principal, (const uint8_t*)images_rgba, bg, img_id_out, rays_o, rays_d, target);
+    else prepare_batch_kernel<float><<<(n + 127) / 128, 128, 0, s>>>(n, pix_index, W, H, xforms, focal, principal, (const float*)images_rgba, bg, img_id_out, rays_o, rays_d, target);
     NGP_LAUNCH_CHECK();
     return 0;
 }

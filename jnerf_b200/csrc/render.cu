@@ -84,7 +84,7 @@ __global__ void __launch_bounds__(RB) render_init_kernel(uint32_t n_rays, float 
         Pcg32 tile_rng{rng_state, rng_inc};
         tile_rng.advance((int64_t)((uint64_t)(g / tile) << 32));
         // ray_setup draws at (i + ray_offset) * 8: the wrapped offset makes that (g % tile) * 8
-        const MarchRng mr{tile_rng.state, rng_inc, nullptr, 0u - (g / tile) * tile};
+        const MarchRng mr{tile_rng.state, rng_inc, 0u - (g / tile) * tile};
         const RayState r = ray_setup(g, rays_o, rays_d, lo, hi, near_distance, cone, c, mr);
         hit = ray_tmin(lo, hi, r.o, r.d) != FLT_MAX ? 1u : 0u;
         ray_t[g] = r.startt;

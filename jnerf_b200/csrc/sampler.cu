@@ -720,14 +720,15 @@ uint64_t ngp_march_workspace_bytes(uint32_t n_rays) {
     return (uint64_t)n_rays * (8 + MARCH_RAY_BYTES) + 1024;
 }
 
-static int march_launch(void* stream, uint32_t n_rays, float aabb_lo, float aabb_hi, uint32_t max_samples, const float* rays_o, const float* rays_d,
-                        const uint8_t* bitfield, float cone_angle, float near_distance, uint32_t cascades, int const_dt, MarchRng mr,
-                        uint32_t* counters, uint32_t* ray_indices, uint32_t* numsteps, float* coords, void* workspace) {
+int ngp_march(void* stream, uint32_t n_rays, float aabb_lo, float aabb_hi, uint32_t max_samples, const float* rays_o, const float* rays_d,
+              const uint8_t* bitfield, float cone_angle, float near_distance, uint32_t cascades, int const_dt, uint64_t rng_state,
+              uint64_t rng_inc, uint32_t* counters, uint32_t* ray_indices, uint32_t* numsteps, float* coords, void* workspace) {
     cudaStream_t s = (cudaStream_t)stream;
     NGP_REQUIRE(cascades >= 1 && cascades <= 8, "ngp_march: cascades out of range");
     NGP_CHECK_CUDA(cudaMemsetAsync(counters, 0, 8, s));                                     // ray_sampler.py:29
     if (n_rays == 0) return 0;
     const MarchCfg c = make_cfg(cascades, const_dt);
+    const MarchRng mr{rng_state, rng_inc, 0u};
     uint32_t* counts = (uint32_t*)workspace;
     uint32_t* n_emit = counts + n_rays;
     uint8_t* ws = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(n_emit + n_rays) + 255) & ~(uintptr_t)255);
@@ -741,21 +742,6 @@ static int march_launch(void* stream, uint32_t n_rays, float aabb_lo, float aabb
                                              ws, n_emit);
     NGP_LAUNCH_CHECK();
     return 0;
-}
-
-int ngp_march(void* stream, uint32_t n_rays, float aabb_lo, float aabb_hi, uint32_t max_samples, const float* rays_o, const float* rays_d,
-              const uint8_t* bitfield, float cone_angle, float near_distance, uint32_t cascades, int const_dt, uint64_t rng_state,
-              uint64_t rng_inc, uint32_t* counters, uint32_t* ray_indices, uint32_t* numsteps, float* coords, void* workspace) {
-    return march_launch(stream, n_rays, aabb_lo, aabb_hi, max_samples, rays_o, rays_d, bitfield, cone_angle, near_distance, cascades, const_dt,
-                        MarchRng{rng_state, rng_inc, nullptr, 0u}, counters, ray_indices, numsteps, coords, workspace);
-}
-
-int ngp_march_dev(void* stream, uint32_t n_rays, float aabb_lo, float aabb_hi, uint32_t max_samples, const float* rays_o, const float* rays_d,
-                  const uint8_t* bitfield, float cone_angle, float near_distance, uint32_t cascades, int const_dt, const void* state_dev,
-                  uint32_t ray_offset, uint32_t* counters, uint32_t* ray_indices, uint32_t* numsteps, float* coords, void* workspace) {
-    NGP_REQUIRE(state_dev != nullptr, "ngp_march_dev: state_dev is required");
-    return march_launch(stream, n_rays, aabb_lo, aabb_hi, max_samples, rays_o, rays_d, bitfield, cone_angle, near_distance, cascades, const_dt,
-                        MarchRng{0, 0, (const NgpStepState*)state_dev, ray_offset}, counters, ray_indices, numsteps, coords, workspace);
 }
 
 int ngp_compact(void* stream, uint32_t n_rays, uint32_t max_compacted, const float* coords_in, const uint32_t* numsteps_in, float* coords_out,

@@ -67,7 +67,6 @@ SIGNATURES = {
     "ngp_adam_ema": (_i32, [_vp, _u64, _vp, _i32, _vp, _i32, _f32, _vp, _vp, _vp, _f32, _f32, _f32, _f32, _u32, _f32, _i32]),
     "ngp_train_sweep": (_i32, [_vp, _u64, _vp, _vp, _vp, _vp, _vp, _vp, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _f32, _f32, _f32, _f32, _u32,
                                _f32]),
-    "ngp_train_sweep_dev": (_i32, [_vp, _u64, _vp, _vp, _vp, _vp, _vp, _vp, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "ngp_dp_exchange_step": (_i32, [_vp, _i32, _i32, _u64, _u32, _vp, _vp, _vp, _vp, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _f32, _f32, _f32,
                                     _f32, _f32, _u32, _f32]),
     "ngp_dp_exchange_wait": (_i32, [_vp, _i32, _vp, _u32]),
@@ -77,12 +76,6 @@ SIGNATURES = {
     "ngp_raygen": (_i32, [_vp, _u32, _vp, _u32, _u32, _vp, _vp, _vp, _vp, _vp, _vp]),
     "ngp_prepare_batch": (_i32, [_vp, _u32, _vp, _u32, _u32, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp]),
     "ngp_blend_target": (_i32, [_vp, _u32, _vp, _vp, _vp]),
-    "ngp_step_state_bytes": (_u64, []),
-    "ngp_step_state_set": (_i32, [_vp, _vp, _u64, _u64, _u32, _u32, _f32, _f32, _f32, _f32, _f32, _f32]),
-    "ngp_step_state_tick": (_i32, [_vp, _vp, _u32, _f32, _f32, _f32, _f32, _f32, _f32]),
-    "ngp_prepare_batch_dev": (_i32, [_vp, _u32, _vp, _vp, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp]),
-    "ngp_march_dev": (_i32, [_vp, _u32, _f32, _f32, _u32, _vp, _vp, _vp, _f32, _f32, _u32, _i32, _vp, _u32, _vp, _vp, _vp, _vp, _vp]),
-    "ngp_adam_ema_dev": (_i32, [_vp, _u64, _vp, _i32, _vp, _i32, _vp, _vp, _vp, _vp, _i32]),
     "ngp_pcg32_seed": (None, [_u64, _u64, _vp]),
     "ngp_pcg32_advance": (None, [_vp, _i64]),
 }
@@ -90,10 +83,10 @@ SIGNATURES = {
 # kernels launched by each entry point (our own __global__ functions; memsets not counted) -- bench.py's gpu_launches
 KERNELS_PER_CALL = {
     "ngp_hash_level_table": 1, "ngp_hash_level_table_primes": 1, "ngp_hash_fwd": 1, "ngp_hash_bwd": 1, "ngp_sh_fwd": 1, "ngp_mlp_fwd": 1, "ngp_mlp_bwd": 1, "ngp_mlp_bwd_dgrad": 1,
-    "ngp_network_fwd": 1, "ngp_network_bwd": 1, "ngp_network_bwd_fx": 1, "ngp_train_sweep": 1, "ngp_train_sweep_dev": 1, "ngp_density_fwd": 1, "ngp_march": 3, "ngp_compact": 1, "ngp_composite_fwd": 1,
+    "ngp_network_fwd": 1, "ngp_network_bwd": 1, "ngp_network_bwd_fx": 1, "ngp_train_sweep": 1, "ngp_density_fwd": 1, "ngp_march": 3, "ngp_compact": 1, "ngp_composite_fwd": 1,
     "ngp_composite_bwd": 1, "ngp_composite_infer": 1, "ngp_composite_loss_bwd": 1, "ngp_grid_mark_untrained": 1,
     "ngp_grid_generate_samples": 1, "ngp_grid_splat": 1, "ngp_grid_ema": 1, "ngp_grid_update_bitfield": 7, "ngp_adam_ema": 1, "ngp_dp_exchange_step": 1, "ngp_dp_exchange_wait": 1, "ngp_raygen": 1, "ngp_prepare_batch": 1,
-    "ngp_blend_target": 1, "ngp_step_state_set": 1, "ngp_step_state_tick": 1, "ngp_prepare_batch_dev": 1, "ngp_march_dev": 3, "ngp_adam_ema_dev": 1,
+    "ngp_blend_target": 1,
     "ngp_density_lattice": 1, "ngp_marching_cubes": 3, "ngp_mesh_largest_component": 18, "ngp_mesh_vertex_normals": 7,
     "ngp_render_init": 3, "ngp_render_march_round": 3, "ngp_render_composite_round": 3,
     "ngp_nerf_fwd": 1, "ngp_nerf_density": 1, "ngp_nerf_bwd": 3,

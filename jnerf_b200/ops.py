@@ -132,21 +132,12 @@ def network_bwd_fx(coords, enc, levels, wd, wr, dout, fx, w_part, n_dev=None):
              levels.n_entries, _p(fx), fx.numel() * fx.element_size(), _p(w_part), w_part.numel() * w_part.element_size())
 
 
-def _sweep_args(table, table_state, fx, w_part, bwd_rows, wd, wd_state, wr, wr_state):
-    assert table.dtype == wd.dtype == wr.dtype == torch.float16 and table.numel() % 2 == 0
-    return (_stream(), table.numel() // 2, _p(table), *map(_p, table_state), _p(fx), _p(w_part), int(bwd_rows), _p(wd), *map(_p, wd_state), _p(wr),
-            *map(_p, wr_state))
-
-
 def train_sweep(table, table_state, fx, w_part, bwd_rows, wd, wd_state, wr, wr_state, lr, step, beta1=0.9, beta2=0.99, eps=1e-15, ema_decay=0.95):
     """The optimizer tail after network_bwd_fx(rows = bwd_rows) in one launch: Adam+EMA of the fp16 hash table and both fp16 MLP weight
     vectors from the backward's scratch, which it clears.  *_state = (m, v, master).  Same bits as network_bwd + three adam_ema calls."""
-    lib.call("ngp_train_sweep", *_sweep_args(table, table_state, fx, w_part, bwd_rows, wd, wd_state, wr, wr_state), float(lr), float(beta1),
-             float(beta2), float(eps), int(step), float(ema_decay))
-
-
-def train_sweep_dev(table, table_state, fx, w_part, bwd_rows, wd, wd_state, wr, wr_state, state):
-    lib.call("ngp_train_sweep_dev", *_sweep_args(table, table_state, fx, w_part, bwd_rows, wd, wd_state, wr, wr_state), _p(state))
+    assert table.dtype == wd.dtype == wr.dtype == torch.float16 and table.numel() % 2 == 0
+    lib.call("ngp_train_sweep", _stream(), table.numel() // 2, _p(table), *map(_p, table_state), _p(fx), _p(w_part), int(bwd_rows), _p(wd),
+             *map(_p, wd_state), _p(wr), *map(_p, wr_state), float(lr), float(beta1), float(beta2), float(eps), int(step), float(ema_decay))
 
 
 def density_fwd(pos, grid, levels, wd):
@@ -538,51 +529,6 @@ def blend_target(rgba, bg, target=None):
         target = torch.empty((n, 3), dtype=torch.float32, device=rgba.device)
     lib.call("ngp_blend_target", _stream(), n, _p(rgba), _p(bg), _p(target))
     return target
-
-
-# ---- device-resident step state (include/ngp_b200.h: ngp_step_state_*) -- what makes a training step replayable as a CUDA graph ----
-def step_state_new(device="cuda"):
-    return torch.zeros(int(lib.load().ngp_step_state_bytes()), dtype=torch.uint8, device=device)
-
-
-def step_state_set(state, rng, pix_cursor, adam_steps_done, lr, beta1=0.9, beta2=0.99, eps=1e-15, ema_decay=0.95, grad_scale=1.0):
-    lib.call("ngp_step_state_set", _stream(), _p(state), int(rng[0]), int(rng[1]), int(pix_cursor), int(adam_steps_done), float(lr), float(beta1),
-             float(beta2), float(eps), float(ema_decay), float(grad_scale))
-
-
-def step_state_tick(state, pix_advance, lr, beta1=0.9, beta2=0.99, eps=1e-15, ema_decay=0.95, grad_scale=1.0):
-    lib.call("ngp_step_state_tick", _stream(), _p(state), int(pix_advance), float(lr), float(beta1), float(beta2), float(eps), float(ema_decay),
-             float(grad_scale))
-
-
-def prepare_batch_dev(n, pix_list, state, pix_offset, W, H, xforms, focal, principal, images, bg):
-    dev = pix_list.device
-    img = torch.empty(n, dtype=torch.int32, device=dev)
-    o = torch.empty((n, 3), dtype=torch.float32, device=dev)
-    d = torch.empty((n, 3), dtype=torch.float32, device=dev)
-    target = torch.empty((n, 3), dtype=torch.float32, device=dev)
-    lib.call("ngp_prepare_batch_dev", _stream(), n, _p(pix_list), _p(state), int(pix_offset), W, H, _p(xforms), _p(focal), _p(principal), _p(images),
-             int(images.dtype == torch.uint8), _p(bg), _p(img), _p(o), _p(d), _p(target))
-    return img, o, d, target
-
-
-def march_dev(rays_o, rays_d, bitfield, aabb, max_samples, cone_angle, near, cascades, const_dt, state, ray_offset=0, coords=None, workspace=None):
-    R = rays_o.shape[0]
-    dev = rays_o.device
-    counters = torch.empty(2, dtype=torch.int32, device=dev)
-    ray_idx = torch.zeros(R, dtype=torch.int32, device=dev)
-    numsteps = torch.empty((R, 2), dtype=torch.int32, device=dev)
-    if coords is None:
-        coords = torch.empty((max_samples, 7), dtype=torch.float32, device=dev)
-    if workspace is None:
-        workspace = torch.empty(int(lib.load().ngp_march_workspace_bytes(R)), dtype=torch.uint8, device=dev)
-    lib.call("ngp_march_dev", _stream(), R, float(aabb[0]), float(aabb[1]), max_samples, _p(rays_o), _p(rays_d), _p(bitfield), float(cone_angle),
-             float(near), cascades, int(const_dt), _p(state), int(ray_offset), _p(counters), _p(ray_idx), _p(numsteps), _p(coords), _p(workspace))
-    return coords, ray_idx, numsteps, counters
-
-
-def adam_ema_dev(param, grad, m, v, master, state, zero_grad=True):
-    lib.call("ngp_adam_ema_dev", _stream(), param.numel(), _p(param), _dt(param), _p(grad), _dt(grad), _p(m), _p(v), _p(master), _p(state), int(zero_grad))
 
 
 def pcg32_seed(seed=1337, seq=1):

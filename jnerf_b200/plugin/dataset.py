@@ -52,20 +52,14 @@ class _RayBatcher:
         self._gen = torch.Generator(device=dev).manual_seed(int(self.seed))
         self.shuffle_index = torch.randperm(self.n_images * self.H * self.W, device=dev, generator=self._gen).int()
 
-    def reserve_pixels(self, n=None):
-        """Claim the next n entries of the shuffled pixel list; returns the index of the first.  The list is reshuffled IN PLACE when it
-        runs out, so its device address never changes (the Runner's CUDA graphs hold it)."""
+    def next_pixels(self, n=None):
+        """The next n entries of the shuffled pixel list; the list is reshuffled in place when it runs out."""
         n = self.batch_size if n is None else n
         if self.idx_now + n >= self.shuffle_index.shape[0]:
             self.shuffle_index.copy_(torch.randperm(self.n_images * self.H * self.W, device=DEVICE, generator=self._gen).int())
             self.idx_now = 0
         start = self.idx_now
         self.idx_now += n
-        return start
-
-    def next_pixels(self, n=None):
-        n = self.batch_size if n is None else n
-        start = self.reserve_pixels(n)
         return self.shuffle_index[start:start + n]
 
     def rays_for(self, pix):

@@ -140,21 +140,6 @@ class DensityGridSampler(Module):
         self.measured_batch_size += cnt_c[0:1]
         return rays_numsteps, ns_c, cnt_c, coords[:cap]
 
-    def sample_dev(self, rays_o, rays_d, state, ray_index_offset=0):
-        """Training-mode sample() with the rng taken from the device-resident step state (ops.march_dev): no host value changes from one
-        call to the next, so the call sequence can be captured in a CUDA graph.  The caller advances self.rng (host mirror), runs the
-        occupancy-grid update and the ray-batch adaptation around it."""
-        coords, _, rays_numsteps, _ = ops.march_dev(rays_o, rays_d, self.density_grid_bitfield, self.aabb_range, self.max_samples,
-                                                    self.cone_angle_constant, self.near_distance, self.NERF_CASCADES, self.const_dt, state,
-                                                    ray_offset=ray_index_offset, coords=self._coords_raw, workspace=self._march_ws)
-        cap = self.target_batch_size
-        _, ns_c, cnt_c = ops.compact(coords, rays_numsteps, cap, alias=True)
-        self.measured_batch_size += cnt_c[0:1]
-        self._rays_numsteps = rays_numsteps
-        self._coords = coords[:cap]
-        self._rays_numsteps_compacted = ns_c
-        self._counters_compacted = cnt_c
-
     @property
     def coords_compacted(self):
         """(target_batch_size, 7) NerfCoordinate rows of the last training sample() -- input of the fused network path."""

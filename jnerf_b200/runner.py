@@ -6,9 +6,9 @@ reference's own batch-size adaptation every 16 steps), one C-ABI call per stage:
     fused composite + Huber + composite bwd -> fused network bwd -> [NCCL all-reduce] -> fused Adam+EMA
 
 The steps are software-pipelined: raygen + march of step i+1 are enqueued on a second stream as soon as step i starts, and run beside
-its network kernels and Adam+EMA sweep (`_train_step_pipe`; NGP_PIPELINE=0 restores the strictly sequential step, NGP_GRAPHS=1 the
-CUDA-graph replay of it).  Every schedule runs the same pieces: `_batch` (background colours + ray batch), the sampler's march,
-`_net_pass` (network forward, composite + loss + its backward, network backward) and the optimizer tail.
+its network kernels and Adam+EMA sweep (`_train_step_pipe`; NGP_PIPELINE=0 restores the strictly sequential step).  Both schedules run
+the same pieces: `_batch` (background colours + ray batch), the sampler's march, `_net_pass` (network forward, composite + loss + its
+backward, network backward) and the optimizer tail.
 
 `train_step_autograd` runs the same step through the per-operator plugin classes and torch autograd, exactly as
 JNeRF's Runner.train does with Jittor; tests check that both give the same parameters."""
@@ -59,7 +59,6 @@ class Runner:
         self._table_work, self._pending_epoch = None, None
         self._host_stage = None
         self._render_ws = None                                       # workspace of the whole-frame renderer (render_rays)
-        self._dev_state = None                                       # device-resident step state + CUDA graphs (single-GPU fast path)
         self._pipe = None                                            # march of step i+1 beside step i (software pipeline over steps)
         self._st = {id(s.p): s for s in self.optimizer._nested_optimizer.state}
         if world_size > 1 and not self.fast:
@@ -92,23 +91,12 @@ class Runner:
         self._fx = self._w_part = None
         if self.world_size == 1 and ops.network_bwd is ops._network_bwd:
             self._fx, self._w_part = ops.network_bwd_scratch(m.pos_encoder.levels, device=dev)
-        if self.world_size == 1:
-            # Device-resident step state (include/ngp_b200.h: ngp_step_state_*): the sampler rng, the pixel cursor and Adam's step
-            # factors live on the device, so every launch of a training step has the same arguments and the step can be captured in
-            # a CUDA graph per ray-batch size.  Opt-in (NGP_GRAPHS=1): every ray-batch size of a run needs its own capture, and a
-            # capture at large batches allocates hundreds of MB.
-            self._dev_state = ops.step_state_new()
-            self._dev_expect = None
-            self._graphs, self._graph_seen, self._graph_pool, self._cap_stream = {}, {}, None, None
-            self._graphs_enabled = os.environ.get("NGP_GRAPHS", "0") == "1" and torch.cuda.is_available() and hasattr(torch.cuda, "CUDAGraph")
-            self.graph_replays = 0
-            self._graph_after = int(os.environ.get("NGP_GRAPH_AFTER", "20"))     # occurrences of a ray-batch size before it gets a graph
         # Software pipeline over steps (default): nothing the march reads is written by the network kernels -- rays, jitter and the
         # occupancy bitfield only -- so the "front" of step i+1 (background colours, ray generation, march, compaction) is enqueued
         # on a second stream while step i's network kernels / Adam+EMA sweep still run.  The sweep is HBM-bound and the march is
         # latency-bound: side by side they share the SMs instead of queueing.  The front of step i+1 may start as soon as step i does
         # (`at` = "front"): starting it after step i's forward or backward was measured slower on the H100 (DESIGN.md section 5).
-        if os.environ.get("NGP_PIPELINE", "1") == "1" and not getattr(self, "_graphs_enabled", False):
+        if os.environ.get("NGP_PIPELINE", "1") == "1":
             # both coordinate buffers are allocated (and zero-filled) HERE, on the constructor's stream: a fill enqueued lazily from inside
             # a step would land on the main stream behind that step's kernels and wipe what the side stream's march had just written
             raw = self.sampler._coords_raw
@@ -250,107 +238,6 @@ class Runner:
         bg = bg.contiguous()
         return img_ids, rays_o, rays_d, bg, ops.blend_target(rgba.contiguous(), bg)                # runner.py:68
 
-    # ------------------------------------------------------------------------------------------ device-state / CUDA-graph step
-    def _lr_for_step(self, k):
-        """ExpDecay's learning rate for its k-th call (optims/expdecay.py:20-25), without advancing it."""
-        dec = self.optimizer
-        f = dec.m_learning_rate_factor
-        for q in range(dec.steps, k + 1):
-            if q >= dec.decay_start and (q - dec.decay_start) % dec.decay_interval == 0 and q <= dec.decay_end:
-                f *= dec.decay_base
-        return dec.base_lr * f
-
-    def _step_body(self, R, lr_next):
-        """Every launch of one training step on R device-generated rays, with nothing step-dependent among the launch arguments (the
-        rng, the pixel cursor and Adam's factors come from the device step state): run eagerly or captured into a CUDA graph."""
-        s, m, ds, st = self.sampler, self.model, self.dataset["train"], self._dev_state
-        adam = self.optimizer._nested_optimizer
-        bg = torch.rand((R, 3), device="cuda", generator=self._bg_gen)                               # runner.py:66
-        img_ids, rays_o, rays_d, target = ops.prepare_batch_dev(R, ds.shuffle_index, st, 0, ds.W, ds.H, ds.transforms_gpu, ds.focal_lengths,
-                                                                ds.principal, ds.image_data, bg)      # dataset.py:172-188 + runner.py:68
-        s.sample_dev(rays_o, rays_d, st)                                                              # march, compaction bookkeeping
-        rgb, loss = self._net_pass(bg, target)
-        if self._fx is not None:
-            ops.train_sweep_dev(*self._sweep_tensors(), st)
-        else:
-            for p, g in ((m.pos_encoder.m_grid, self.grid_grad), (m.density_mlp.con_weights, self.dwd), (m.rgb_mlp.con_weights, self.dwr)):
-                stp = self._st[id(p)]
-                ops.adam_ema_dev(p.data, g, stp.m, stp.v, stp.master, st, zero_grad=True)
-        ops.step_state_tick(st, R, lr_next, adam.betas[0], adam.betas[1], adam.eps, self.ema_optimizer.decay, 1.0)
-        self.last_loss, self.last_rgb = loss, rgb
-        return loss
-
-    def _train_step_dev(self):
-        cfg, s, ds = self.cfg, self.sampler, self.dataset["train"]
-        adam, dec = self.optimizer._nested_optimizer, self.optimizer
-        i = cfg.m_training_step
-        R = s.n_rays_per_batch
-        edge = i % s.update_den_freq == 0 or i % s.update_den_freq == s.update_den_freq - 1
-        if i % s.update_den_freq == 0:
-            s.update_density_grid()                                  # evaluates the density network, advances the sampler rng
-        if R > s._march_ws_rays:
-            s._ensure_march_ws(2 * R)
-            self._graphs.clear()                                     # the captured launches hold the old workspace's address
-            self._graph_pool = None                                  # (the allocator drops a pool together with its last graph)
-        start = ds.reserve_pixels(R)
-        lr, lr_next = self._lr_for_step(dec.steps), self._lr_for_step(dec.steps + 1)
-        want = (int(s.rng[0]), int(s.rng[1]), start, adam.n_step, lr)
-        if self._dev_expect != want:                                 # first step, or the host changed something outside a step
-            ops.step_state_set(self._dev_state, s.rng, start, adam.n_step, lr, adam.betas[0], adam.betas[1], adam.eps, self.ema_optimizer.decay, 1.0)
-        key = (R, lr_next)
-        g = self._graphs.get(key) if self._graphs_enabled and not edge else None
-        if g is not None:
-            g[0].replay()
-            ops.lib.launch_count += g[1]
-            self.graph_replays += 1
-            loss = g[2]
-            self.last_loss, self.last_rgb = g[2], g[3]
-            s._rays_numsteps, s._rays_numsteps_compacted, s._counters_compacted, s._coords = g[4]
-        else:
-            seen = self._graph_seen.get(key, 0) + 1
-            self._graph_seen[key] = seen
-            # a capture costs about as much as 200 replays save: only ray-batch sizes that keep coming back (a second 16-step window)
-            # get a graph
-            if self._graphs_enabled and not edge and seen >= self._graph_after and len(self._graphs) < 64:
-                # capture on a side stream with the raw begin / end calls: torch.cuda.graph() would synchronise the device, run the
-                # Python garbage collector and empty the allocator cache on every capture (~10 ms each)
-                graph = torch.cuda.CUDAGraph()
-                if hasattr(graph, "register_generator_state"):
-                    graph.register_generator_state(self._bg_gen)
-                n0 = ops.lib.launch_count
-                if self._cap_stream is None:
-                    self._cap_stream = torch.cuda.Stream()
-                main = torch.cuda.current_stream()
-                self._cap_stream.wait_stream(main)
-                with torch.cuda.stream(self._cap_stream):
-                    if self._graph_pool is None:
-                        graph.capture_begin(capture_error_mode="thread_local")
-                    else:
-                        graph.capture_begin(pool=self._graph_pool, capture_error_mode="thread_local")
-                    loss = self._step_body(R, lr_next)
-                    graph.capture_end()
-                main.wait_stream(self._cap_stream)
-                if self._graph_pool is None:
-                    self._graph_pool = graph.pool()
-                self._graphs[key] = (graph, ops.lib.launch_count - n0, loss, self.last_rgb,
-                                     (s._rays_numsteps, s._rays_numsteps_compacted, s._counters_compacted, s._coords))
-                ops.lib.launch_count = n0
-                graph.replay()                                       # capture records the launches, the replay performs the step
-                ops.lib.launch_count += self._graphs[key][1]
-                self.graph_replays += 1
-            else:
-                loss = self._step_body(R, lr_next)
-        # host mirrors of what the step advanced on the device
-        ops.pcg32_advance(s.rng)                                     # rng.advance(), ray_sampler.py:61
-        dec.advance_lr()
-        adam.n_step += 1
-        self.ema_optimizer.steps += 1
-        self._dev_expect = (int(s.rng[0]), int(s.rng[1]), start + R, adam.n_step, lr_next)
-        if i % s.update_den_freq == s.update_den_freq - 1:
-            s.update_batch_rays()
-        cfg.m_training_step = i + 1
-        return loss
-
     # ------------------------------------------------------------------------------------------ software pipeline over steps
     def _front(self, step, batch, prefetch):
         """The part of training step `step` that does not read a network parameter: background colours, ray generation + target
@@ -441,8 +328,6 @@ class Runner:
     def train_step(self, batch=None, next_batch=None):
         if self._pipe is not None:
             return self._train_step_pipe(batch, next_batch)
-        if batch is None and self._dev_state is not None:
-            return self._train_step_dev()
         cfg, s = self.cfg, self.sampler
         i = cfg.m_training_step
         img_ids, rays_o, rays_d, bg, target = self._batch(batch)
@@ -541,13 +426,6 @@ class Runner:
         ops.network_bwd(coords, self.enc, m.pos_encoder.levels, m.density_mlp.con_weights, m.rgb_mlp.con_weights, self.dnet,
                         self.grid_grad, self.dwd, self.dwr, n_dev=n_dev)
 
-    def _sweep_tensors(self):
-        """Arguments of ops.train_sweep(_dev) after net_backward."""
-        m = self.model
-        st = [self._st[id(p)] for p in (m.pos_encoder.m_grid, m.density_mlp.con_weights, m.rgb_mlp.con_weights)]
-        return (m.pos_encoder.m_grid.data, (st[0].m, st[0].v, st[0].master), self._fx, self._w_part, self._bwd_rows,
-                m.density_mlp.con_weights.data, (st[1].m, st[1].v, st[1].master), m.rgb_mlp.con_weights.data, (st[2].m, st[2].v, st[2].master))
-
     def _optimizer_tail(self):
         """One optimizer step of the host-state training steps: ExpDecay's learning rate, Adam's and the EMA's step counters, then
         _optimizer_step."""
@@ -563,7 +441,10 @@ class Runner:
         adam = self.optimizer._nested_optimizer
         hyper = (lr, n_step, adam.betas[0], adam.betas[1], adam.eps, self.ema_optimizer.decay)
         if self._fx is not None:
-            ops.train_sweep(*self._sweep_tensors(), lr, n_step, adam.betas[0], adam.betas[1], adam.eps, self.ema_optimizer.decay)
+            st = [self._st[id(p)] for p in (m.pos_encoder.m_grid, m.density_mlp.con_weights, m.rgb_mlp.con_weights)]
+            ops.train_sweep(m.pos_encoder.m_grid.data, (st[0].m, st[0].v, st[0].master), self._fx, self._w_part, self._bwd_rows,
+                            m.density_mlp.con_weights.data, (st[1].m, st[1].v, st[1].master), m.rgb_mlp.con_weights.data,
+                            (st[2].m, st[2].v, st[2].master), *hyper)
             return
         if self.world_size > 1 and self.dp_mode == "p2p":
             st = self._st[id(m.pos_encoder.m_grid)]

@@ -248,42 +248,6 @@ class OracleOps:
         target = rgba[:, :3] * rgba[:, 3:] + bg * (1 - rgba[:, 3:])            # runner.py:68
         return img, o, d, target.contiguous()
 
-    # ---- device-resident step state: the CPU stand-in keeps it in a small Python object and forwards to the host-argument operators,
-    # logged under the same names (what is under test is the Runner's bookkeeping around them)
-    class _StepState:
-        rng = None
-        cursor = steps_done = 0
-        hyper = None
-
-    def step_state_new(self, device="cpu"):
-        return OracleOps._StepState()
-
-    def step_state_set(self, state, rng, pix_cursor, adam_steps_done, lr, beta1=0.9, beta2=0.99, eps=1e-15, ema_decay=0.95, grad_scale=1.0):
-        self._log("step_state_set")
-        state.rng = np.array([int(rng[0]), int(rng[1])], np.uint64)
-        state.cursor, state.steps_done = int(pix_cursor), int(adam_steps_done)
-        state.hyper = (float(lr), beta1, beta2, eps, ema_decay, grad_scale)
-
-    def step_state_tick(self, state, pix_advance, lr, beta1=0.9, beta2=0.99, eps=1e-15, ema_decay=0.95, grad_scale=1.0):
-        self._log("step_state_tick")
-        ol.pcg32_advance(state.rng)
-        state.cursor += int(pix_advance)
-        state.steps_done += 1
-        state.hyper = (float(lr), beta1, beta2, eps, ema_decay, grad_scale)
-
-    def prepare_batch_dev(self, n, pix_list, state, pix_offset, W, H, xforms, focal, principal, images, bg):
-        a = state.cursor + int(pix_offset)
-        return self.prepare_batch(pix_list[a:a + n], W, H, xforms, focal, principal, images, bg)
-
-    def march_dev(self, rays_o, rays_d, bitfield, aabb, max_samples, cone_angle, near, cascades, const_dt, state, ray_offset=0, coords=None,
-                  workspace=None):
-        rng = ol.pcg32_advance(state.rng.copy(), int(ray_offset) * 8) if ray_offset else state.rng
-        return self.march(rays_o, rays_d, bitfield, aabb, max_samples, cone_angle, near, cascades, const_dt, rng, coords=coords, workspace=workspace)
-
-    def adam_ema_dev(self, param, grad, m, v, master, state, zero_grad=True):
-        lr, b1, b2, eps, decay, gs = state.hyper
-        self.adam_ema(param, grad, m, v, master, lr, state.steps_done + 1, b1, b2, eps, decay, grad_scale=gs, zero_grad=zero_grad)
-
     def blend_target(self, rgba, bg, target=None):
         self._log("blend_target")
         t = (rgba[:, :3] * rgba[:, 3:] + bg * (1 - rgba[:, 3:])).contiguous()   # runner.py:68

@@ -1,6 +1,6 @@
-"""The single-GPU training tail: ngp_network_bwd_fx into caller-owned scratch + one ngp_train_sweep(_dev) must give the parameters and
-optimizer state that ngp_network_bwd + three ngp_adam_ema(_dev) sweeps give, bit for bit, and leave the scratch zeroed; a Runner
-that uses it trains identically pipelined, sequential and replayed from CUDA graphs."""
+"""The single-GPU training tail: ngp_network_bwd_fx into caller-owned scratch + one ngp_train_sweep must give the parameters and
+optimizer state that ngp_network_bwd + three ngp_adam_ema sweeps give, bit for bit, and leave the scratch zeroed; a Runner that uses
+it trains identically pipelined and sequential."""
 import pytest
 import torch
 
@@ -32,10 +32,9 @@ def _state(params):
     return [(torch.zeros(p.numel(), device="cuda"), torch.zeros(p.numel(), device="cuda"), p.float().clone()) for p in params]
 
 
-@pytest.mark.parametrize("dev", [False, True], ids=["host", "dev"])
 @pytest.mark.parametrize("aabb,n_max,n_live", [(1, 1 << 18, None), (4, 1 << 18, None), (1, 70001, None), (4, 70001, 41234)],
                          ids=["lego-2^18", "fox-2^18", "lego-70001", "fox-70001-live41234"])
-def test_bwd_fx_plus_sweep_equals_bwd_plus_three_sweeps(aabb, n_max, n_live, dev):
+def test_bwd_fx_plus_sweep_equals_bwd_plus_three_sweeps(aabb, n_max, n_live):
     from jnerf_b200 import ops
     lv, coords, enc, dout, n_dev, p0 = _inputs(aabb, n_max, n_live, seed=5 + n_max + aabb)
     pa, pb = [p.clone() for p in p0], [p.clone() for p in p0]
@@ -43,24 +42,12 @@ def test_bwd_fx_plus_sweep_equals_bwd_plus_three_sweeps(aabb, n_max, n_live, dev
     gg = torch.zeros(lv.n_params, dtype=torch.float16, device="cuda")
     dwd, dwr = torch.zeros(3072, device="cuda"), torch.zeros(7168, device="cuda")
     fx, part = ops.network_bwd_scratch(lv)
-    sta, stb = ops.step_state_new(), ops.step_state_new()
-    for st in (sta, stb):
-        ops.step_state_set(st, (0, 0), 0, 0, LR, HYPER["beta1"], HYPER["beta2"], HYPER["eps"], HYPER["ema_decay"], 1.0)
     for step in (1, 2):                                      # the second backward runs on the updated weights, into the cleared scratch
         ops.network_bwd(coords, enc, lv, pa[1], pa[2], dout, gg, dwd, dwr, n_dev=n_dev)
         for p, gr, (m, v, ms) in zip(pa, (gg, dwd, dwr), sa):
-            if dev:
-                ops.adam_ema_dev(p, gr, m, v, ms, sta, zero_grad=True)
-            else:
-                ops.adam_ema(p, gr, m, v, ms, LR, step, **HYPER, grad_scale=1.0, zero_grad=True)
+            ops.adam_ema(p, gr, m, v, ms, LR, step, **HYPER, grad_scale=1.0, zero_grad=True)
         ops.network_bwd_fx(coords, enc, lv, pb[1], pb[2], dout, fx, part, n_dev=n_dev)
-        args = (pb[0], sb[0], fx, part, n_max, pb[1], sb[1], pb[2], sb[2])
-        if dev:
-            ops.train_sweep_dev(*args, stb)
-        else:
-            ops.train_sweep(*args, LR, step, **HYPER)
-        for st in (sta, stb):
-            ops.step_state_tick(st, 0, LR, HYPER["beta1"], HYPER["beta2"], HYPER["eps"], HYPER["ema_decay"], 1.0)
+        ops.train_sweep(pb[0], sb[0], fx, part, n_max, pb[1], sb[1], pb[2], sb[2], LR, step, **HYPER)
         torch.cuda.synchronize()
         assert int(torch.count_nonzero(fx)) == 0, "the sweep must leave the scratch zeroed"
         for k, name in enumerate(("table", "density weights", "colour weights")):
@@ -100,19 +87,11 @@ def _train(monkeypatch, steps, **env):
 
 def test_runner_pipelined_equals_sequential_bit_for_bit(monkeypatch):
     """64 steps = four occupancy-grid updates: the deterministic backward and sweep make the two step orders train identically."""
-    ra, la, pa = _train(monkeypatch, 64, NGP_PIPELINE="1", NGP_GRAPHS="0")
+    ra, la, pa = _train(monkeypatch, 64, NGP_PIPELINE="1")
     assert ra._pipe is not None and ra._pipe["prefetched"] > 0
-    rb, lb, pb = _train(monkeypatch, 64, NGP_PIPELINE="0", NGP_GRAPHS="0")
+    rb, lb, pb = _train(monkeypatch, 64, NGP_PIPELINE="0")
     assert rb._pipe is None
     assert torch.equal(la, lb)
     for k in pa:
         assert torch.equal(pa[k], pb[k]), k
 
-
-def test_runner_cuda_graph_runs_are_reproducible(monkeypatch):
-    """A captured backward used to find no scratch and reduce in arbitrary order; with caller-owned scratch two graph runs agree."""
-    runs = [_train(monkeypatch, 48, NGP_GRAPHS="1", NGP_PIPELINE="0", NGP_GRAPH_AFTER="2") for _ in range(2)]
-    assert runs[0][0].graph_replays >= 10
-    assert torch.equal(runs[0][1], runs[1][1])
-    for k in runs[0][2]:
-        assert torch.equal(runs[0][2][k], runs[1][2][k]), k

@@ -80,9 +80,7 @@ def test_every_stub_in_integration_md_type_checks_against_the_header(tmp_path):
     # every compute entry point of the header has a stub in the document (host helpers and debug aids excepted)
     helpers = {"ngp_last_error", "ngp_version", "ngp_sm_count", "ngp_debug_timeout_flag", "ngp_hash_offsets", "ngp_hash_level_table", "ngp_hash_level_table_primes",
                "ngp_mlp_param_count", "ngp_march_workspace_bytes", "ngp_pcg32_seed", "ngp_pcg32_advance", "ngp_ipc_close", "ngp_raygen",
-               "ngp_prepare_batch", "ngp_composite_loss_bwd", "ngp_mlp_bwd_dgrad", "ngp_blend_target",
-               # the device-resident step state belongs to the Runner's CUDA-graph replay, not to the reference's operator classes
-               "ngp_step_state_bytes", "ngp_step_state_set", "ngp_step_state_tick", "ngp_prepare_batch_dev", "ngp_march_dev", "ngp_adam_ema_dev"}
+               "ngp_prepare_batch", "ngp_composite_loss_bwd", "ngp_mlp_bwd_dgrad", "ngp_blend_target"}
     for name in sorted(declared - helpers - used):
         assert name in text, f"{name} is declared in the header but INTEGRATION.md never mentions it"
     assert not (declared - helpers - used), declared - helpers - used

@@ -32,11 +32,10 @@ def make_runner(monkeypatch, cfg_fn="lego_cfg", images=4, H=24, W=24, rays=64, t
     return r, fake
 
 
-STEP_OPS = ["prepare_batch", "march", "compact", "network_fwd", "composite_loss_bwd", "network_bwd", "adam_ema", "adam_ema", "adam_ema",
-            "step_state_tick"]
+STEP_OPS = ["prepare_batch", "march", "compact", "network_fwd", "composite_loss_bwd", "network_bwd", "adam_ema", "adam_ema", "adam_ema"]
 
 
-def test_fast_path_step_sequence_and_bookkeeping(monkeypatch):
+def test_sequential_step_call_sequence_and_bookkeeping(monkeypatch):
     r, fake = make_runner(monkeypatch)
     m, s = r.model, r.sampler
     assert r.fast and m.pos_encoder.m_grid.numel() == 12196240 and s.max_samples == 64 * 1024
@@ -45,8 +44,7 @@ def test_fast_path_step_sequence_and_bookkeeping(monkeypatch):
     rng0 = s.rng.copy()
     fake.calls.clear()
     loss = r.train_step()
-    assert fake.calls == ["step_state_set"] + STEP_OPS              # first step: the device step state is loaded from the host mirrors;
-                                                                    # then one C-ABI call per stage, in the reference's order
+    assert fake.calls == STEP_OPS                                   # one C-ABI call per stage, in the reference's order
     assert torch.isfinite(loss).all() and loss.shape == (64,)
     assert r.cfg.m_training_step == 2 and r.optimizer._nested_optimizer.n_step == 1 and r.ema_optimizer.steps == 1 and r.optimizer.steps == 1
     assert not torch.equal(m.pos_encoder.m_grid.detach(), g0) and not torch.equal(m.rgb_mlp.con_weights.detach(), w0)
@@ -61,7 +59,7 @@ def test_fast_path_step_sequence_and_bookkeeping(monkeypatch):
     first = float(loss.mean())
     fake.calls.clear()
     loss = r.train_step()
-    assert fake.calls == STEP_OPS                                   # later steps: the state advanced on the "device", no reload
+    assert fake.calls == STEP_OPS
     for _ in range(12):
         loss = r.train_step()
     assert r.cfg.m_training_step == 15 and s.n_rays_per_batch == 64

@@ -10,7 +10,7 @@ from test_runner_cpu import make_runner
 
 
 class _FoldOps:
-    """Stand-ins of network_bwd_scratch / network_bwd_fx / train_sweep(_dev): the scratch holds the fp16-rounded table gradient as
+    """Stand-ins of network_bwd_scratch / network_bwd_fx / train_sweep: the scratch holds the fp16-rounded table gradient as
     fp32 and the weight gradients in one slot, and the sweep hands them to the stand-in adam_ema."""
 
     def __init__(self, fake):
@@ -26,21 +26,14 @@ class _FoldOps:
         fx += gg.float()
         w_part += torch.cat([dwd, dwr])
 
-    def _sweep(self, name, table, ts, fx, w_part, bwd_rows, wd, ws, wr, rs, hyper):
+    def train_sweep(self, table, ts, fx, w_part, bwd_rows, wd, ws, wr, rs, lr, step, beta1=0.9, beta2=0.99, eps=1e-15, ema_decay=0.95):
         n = len(self.fake.calls)
         for p, g, (m, v, ms) in ((table, fx.half(), ts), (wd, w_part[:3072].clone(), ws), (wr, w_part[3072:].clone(), rs)):
-            self.fake.adam_ema(p, g, m, v, ms, *hyper)
+            self.fake.adam_ema(p, g, m, v, ms, lr, step, beta1, beta2, eps, ema_decay)
         del self.fake.calls[n:]
-        self.fake.calls.append(name)
+        self.fake.calls.append("train_sweep")
         fx.zero_()
         w_part.zero_()
-
-    def train_sweep(self, table, ts, fx, w_part, bwd_rows, wd, ws, wr, rs, lr, step, beta1=0.9, beta2=0.99, eps=1e-15, ema_decay=0.95):
-        self._sweep("train_sweep", table, ts, fx, w_part, bwd_rows, wd, ws, wr, rs, (lr, step, beta1, beta2, eps, ema_decay))
-
-    def train_sweep_dev(self, table, ts, fx, w_part, bwd_rows, wd, ws, wr, rs, state):
-        lr, b1, b2, eps, decay, _ = state.hyper
-        self._sweep("train_sweep_dev", table, ts, fx, w_part, bwd_rows, wd, ws, wr, rs, (lr, state.steps_done + 1, b1, b2, eps, decay))
 
 
 def _install_fold(monkeypatch):
@@ -51,7 +44,7 @@ def _install_fold(monkeypatch):
         fake = real_install(mp)
         import jnerf_b200.ops as real_ops
         fold = _FoldOps(fake)
-        for name in ("network_bwd_scratch", "network_bwd_fx", "train_sweep", "train_sweep_dev"):
+        for name in ("network_bwd_scratch", "network_bwd_fx", "train_sweep"):
             mp.setattr(real_ops, name, getattr(fold, name), raising=False)
         mp.setattr(real_ops, "_network_bwd", real_ops.network_bwd)
         return fake
@@ -73,15 +66,15 @@ class _MarkEvent:
         self.calls.append("front may start")
 
 
-SEQ_OPS = ["prepare_batch", "march", "compact", "network_fwd", "composite_loss_bwd", "network_bwd_fx", "train_sweep_dev", "step_state_tick"]
+SEQ_OPS = ["prepare_batch", "march", "compact", "network_fwd", "composite_loss_bwd", "network_bwd_fx", "train_sweep"]
 
 
-def test_folded_sequential_step_is_one_backward_and_one_sweep(monkeypatch, fold_backend):
+def test_folded_sequential_step_is_one_backward_and_one_host_argument_sweep(monkeypatch, fold_backend):
     r, fake = make_runner(monkeypatch)
     assert r._fx is not None
     fake.calls.clear()
     r.train_step()
-    assert fake.calls == ["step_state_set"] + SEQ_OPS
+    assert fake.calls == SEQ_OPS
     fake.calls.clear()
     r.train_step()
     assert fake.calls == SEQ_OPS
