@@ -308,6 +308,47 @@ void orc_hash_bwd_f16_acc32(uint32_t n, const float* x, const half_t* dy, const 
         }
     }
 }
+/* The exact scatter of an fp32 dL/dy, for error bounds: w is the fp32 corner weight formed as above, dy * w is exact in double
+ * (24 + 24 significant bits), and per feature of every entry it returns g = sum dy * w, a = sum |dy * w| and cnt = the number of
+ * nonzero contributions.  g is summed in double in row order: its own error, at most cnt * 2^-53 * a, is far below the fp32 error
+ * bounds it is compared with. */
+void orc_hash_bwd_f64(uint32_t n, const float* x, const float* dy, const uint32_t* offsets, uint32_t n_levels,
+                      uint32_t base_res, float log2_pls, double* grid_grad, double* grid_abs, uint32_t* grid_cnt) {
+    const size_t np = (size_t)offsets[n_levels] * 2;
+    memset(grid_grad, 0, np * sizeof(double));
+    memset(grid_abs, 0, np * sizeof(double));
+    memset(grid_cnt, 0, np * sizeof(uint32_t));
+#pragma omp parallel for schedule(static)
+    for (int64_t lv = 0; lv < (int64_t)n_levels; ++lv) {
+        uint32_t level = (uint32_t)lv;
+        double* g = grid_grad + (size_t)offsets[level] * 2;
+        double* a = grid_abs + (size_t)offsets[level] * 2;
+        uint32_t* c = grid_cnt + (size_t)offsets[level] * 2;
+        uint32_t size = offsets[level + 1] - offsets[level], res; float scale;
+        level_setup(level, base_res, log2_pls, &scale, &res);
+        for (uint32_t i = 0; i < n; ++i) {
+            float pos[3]; uint32_t pg[3];
+            for (int d = 0; d < 3; ++d) pos_fract(x[i * 3 + d], scale, &pos[d], &pg[d]);
+            const double g01[2] = {dy[(size_t)i * n_levels * 2 + level * 2], dy[(size_t)i * n_levels * 2 + level * 2 + 1]};
+            if (g01[0] == 0.0 && g01[1] == 0.0) continue;
+            for (uint32_t idx = 0; idx < 8; ++idx) {
+                float w = 1; uint32_t pl[3];
+                for (uint32_t d = 0; d < 3; ++d) {
+                    if ((idx & (1u << d)) == 0) { w *= 1 - pos[d]; pl[d] = pg[d]; }
+                    else { w *= pos[d]; pl[d] = pg[d] + 1; }
+                }
+                uint32_t index = grid_index(size, res, pl);
+                for (uint32_t f = 0; f < 2; ++f) {
+                    const double v = g01[f] * (double)w;
+                    if (v == 0.0) continue;
+                    g[index + f] += v;
+                    a[index + f] += fabs(v);
+                    c[index + f] += 1;
+                }
+            }
+        }
+    }
+}
 
 /* ------------------------------------------------------------------------------------------------
  * R4: spherical harmonics, degree 4  (SH/op_header/SphericalEncode.h:65-95; SH/sh_encoder.py:16)

@@ -119,6 +119,21 @@ def hash_bwd(cfg, x, dy, acc32=False):
     return g
 
 
+def hash_bwd_f64(cfg, x, dy):
+    """The exact scatter of an fp32 dL/dy (n, 2L): per feature of every entry (g, a, cnt) = (sum dy*w in float64, sum |dy*w|, number of
+    nonzero contributions), with the fp32 corner weights w the kernels form."""
+    n = x.shape[0]
+    x = np.ascontiguousarray(x, np.float32)
+    dy = np.ascontiguousarray(dy, np.float32)
+    assert dy.shape == (n, cfg.n_levels * 2)
+    g = np.empty(cfg.n_params, np.float64)
+    a = np.empty(cfg.n_params, np.float64)
+    cnt = np.empty(cfg.n_params, np.uint32)
+    oracle().orc_hash_bwd_f64(_u32(n), _ptr(x), _ptr(dy), _ptr(cfg.offsets), _u32(cfg.n_levels), _u32(cfg.base), _f32(cfg.log2_pls),
+                              _ptr(g), _ptr(a), _ptr(cnt))
+    return g, a, cnt
+
+
 def ref_hash_fwd(cfg, x, grid):
     r = ref("ref_hash_cpu")
     n = x.shape[0]
