@@ -172,6 +172,46 @@ int ngp_mip_composite_loss_bwd(void* stream, uint32_t n_rays, uint32_t n_samples
                                const float* target, const float* mask, float rgb_padding, float density_bias, int white_bkgd, float coarse_loss_mult,
                                float grad_scale, float* rgb_out, float* loss_out, void* draw_out);
 
+/* ---- X1-X9  Plenoxels (contrib/plenoxel of the reference: models/networks/svox2_network.py, ops/svox_ops/op/op_header/*.h),
+ * csrc/svox.cu, DESIGN.md section 12 ----------------------------------------------------------------------------------------------
+ * A grid is links (X, Y, Z) int32 row-major (< 0: empty), density (capacity) and sh (capacity, 27) fp32, SH degree 2 channel-major.
+ * xform (host, 6 floats): offset[3], scaling[3] from world to grid coordinates (_offset * reso - 0.5, _scaling * reso).  opts (host, 4
+ * floats): step_size, sigma_thresh, stop_thresh, background_brightness.  Cameras: c2w row-major 3x4 OpenCV camera-to-world, pixel
+ * (img * H + y) * W + x, ray through the pixel centre.  Gradients are signed 64-bit fixed point, 2^48 units per 1.0, added with integer
+ * atomics (order-independent); a term or sum out of range ORs 1 into *flag (device), which stays set until the caller clears it.
+ * X1: one training step of n_rays pixels: forward, dL/drgb = 2 (rgb - gt) / (3 n_rays) with gt the RGBA image composited on white,
+ * the backward into grad_density / grad_sh (added to), and the per-ray squared error sqerr_out (n_rays). */
+int ngp_svox_train_step(void* stream, uint32_t n_rays, const int32_t* pix, uint32_t W, uint32_t H, const float* c2w, float fx, float fy, float cx,
+                        float cy, const uint8_t* images_rgba, const int32_t* links, int X, int Y, int Z, const float* density, const float* sh,
+                        const float* xform, const float* opts, long long* grad_density, long long* grad_sh, float* sqerr_out, unsigned* flag);
+/* X2: rgb_out (n, 3) of pixels [first, first + n) (row-major y * W + x) of one camera c2w (12 floats). */
+int ngp_svox_render(void* stream, uint32_t n, uint32_t first, uint32_t W, const float* c2w, float fx, float fy, float cx, float cy, const int32_t* links,
+                    int X, int Y, int Z, const float* density, const float* sh, const float* xform, const float* opts, float* rgb_out);
+/* X3: sparse TV of columns [0, dim) of data (capacity, dim) over the cells (start + i) mod (X Y Z), i < n_cells, added into grad
+ * (loss_kernel.h:51-118; scale is lambda / n_cells). */
+int ngp_svox_tv_grad(void* stream, const int32_t* links, int X, int Y, int Z, const float* data, uint32_t dim, uint32_t start, uint32_t n_cells,
+                     float scale, int ignore_edge, long long* grad, unsigned* flag);
+/* X4: RMSprop over density (n_density) and sh (n_sh entries): v = a v + (1 - a) g^2, p -= lr g / (sqrt(v) + eps) with g the
+ * fixed-point gradient, which is set to 0. */
+int ngp_svox_rmsprop(void* stream, uint64_t n_density, uint64_t n_sh, float* density, float* sh, long long* grad_density, long long* grad_sh,
+                     float* rms_density, float* rms_sh, float lr_density, float lr_sh, float alpha_density, float alpha_sh, float eps);
+/* X5: trilerp of density (and, want_sh, of the 27 SH columns) at n points (n, 3) given in grid coordinates. */
+int ngp_svox_sample(void* stream, uint32_t n, const float* points, const int32_t* links, int X, int Y, int Z, const float* density, const float* sh,
+                    int want_sh, float* density_out, float* sh_out);
+/* X6: max over the rays of one camera (W x H) of each sample's weight, onto the 8 corners of its cell of the dense grid data (X, Y, Z):
+ * weight_out (X, Y, Z) is max-ed into. */
+int ngp_svox_weight_render(void* stream, uint32_t W, uint32_t H, const float* c2w, float fx, float fy, float cx, float cy, const float* data, int X, int Y,
+                           int Z, const float* xform, float step_size, float stop_thresh, float* weight_out);
+/* X7: out = the 26-neighbourhood dilation of mask (X, Y, Z) uint8. */
+int ngp_svox_dilate(void* stream, int X, int Y, int Z, const uint8_t* mask, uint8_t* out);
+/* X8: bytes of the workspace of X9. */
+int ngp_svox_compact_workspace_bytes(int X, int Y, int Z, uint64_t* bytes_out);
+/* X9: links_out (X, Y, Z) = the exclusive count of kept cells before each kept cell, -1 elsewhere; kept cell c gets density_out[c] =
+ * dense_density of the cell and points_out[c] = lattice[0:3] + (x, y, z) * lattice[3:6] (host lattice).  capacity = number of kept
+ * cells. */
+int ngp_svox_compact(void* stream, int X, int Y, int Z, const uint8_t* mask, const float* dense_density, const float* lattice, uint32_t capacity,
+                     void* workspace, int32_t* links_out, float* density_out, float* points_out);
+
 /* ---- M1-M4  mesh extraction (tools/extract_mesh.py of the reference: a trained model -> mesh-origin.ply / mesh-color.ply) --------
  * Resolution n must be in [2, 1024]; vertices are (V,3) f32, triangles (T,3) int32 (V, T < 2^31); counts are 64-bit.
  * workspace: *bytes_out of ngp_mesh_workspace_bytes(n, 0, 0, .) for ngp_marching_cubes, of (0, V, T, .) for the other two.

@@ -19,6 +19,7 @@ SOURCES = {
     "nerf_mlp.cu": [],
     "mip_mlp.cu": [],
     "mip_sampler.cu": ["-fmad=false"],
+    "svox.cu": [],
     "sampler.cu": ["-fmad=false"],
     "grid_update.cu": ["-fmad=false"],
     "mesh.cu": ["-fmad=false"],

@@ -55,6 +55,24 @@ SRC = {
     "grid_update_bitfield": "NGP_OK(ngp_grid_update_bitfield(0, in0_p, out1_p, (uint8_t*)out0_p, NERF_CASCADES()));",
     # optims/adam.py + optims/ema.py in one sweep per parameter tensor
     "adam_ema": "NGP_OK(ngp_adam_ema(0, in0_shape0, in0_p, NGP_F16, in1_p, NGP_F16, 1.0f, in2_p, in3_p, in4_p, (float){lr}, 0.9f, 0.99f, 1e-15f, {step}, 0.95f, 1));",
+    # contrib/plenoxel: volume_render_cuvol.py (forward, and forward + MSE + backward fused), tv_grad_sparse.py, optims/svox2_optim.py,
+    # sample_grid.py, grid_weight_render.py, dilate.py and the link rebuild of svox2_network.py:470-482 (xform_p: offset[3] + scaling[3],
+    # opts_p: step, sigma_thresh, stop_thresh, background, host float arrays declared before the call)
+    "svox_train_step": ("NGP_OK(ngp_svox_train_step(0, in0_shape0, in0_p, {W}, {H}, in1_p, {fx}, {fy}, {cx}, {cy}, (const uint8_t*)in2_p, in3_p, "
+                        "in3_shape0, in3_shape1, in3_shape2, in4_p, in5_p, xform_p, opts_p, out0_p, out1_p, out2_p, out3_p));"),
+    "svox_render": ("NGP_OK(ngp_svox_render(0, out0_shape0, {first}, {W}, in0_p, {fx}, {fy}, {cx}, {cy}, in1_p, in1_shape0, in1_shape1, in1_shape2, "
+                    "in2_p, in3_p, xform_p, opts_p, out0_p));"),
+    "svox_tv_grad": ("NGP_OK(ngp_svox_tv_grad(0, in0_p, in0_shape0, in0_shape1, in0_shape2, in1_p, in1_shape1, {start}, {n_cells}, (float){scale}, "
+                     "{ignore_edge}, out0_p, out1_p));"),
+    "svox_rmsprop": ("NGP_OK(ngp_svox_rmsprop(0, in0_shape0, in1_shape0 * in1_shape1, in0_p, in1_p, in2_p, in3_p, in4_p, in5_p, (float){lr_sigma}, "
+                     "(float){lr_sh}, 0.95f, 0.95f, 1e-8f));"),
+    "svox_sample": ("NGP_OK(ngp_svox_sample(0, in0_shape0, in0_p, in1_p, in1_shape0, in1_shape1, in1_shape2, in2_p, in3_p, {want_sh}, out0_p, "
+                    "out1_p));"),
+    "svox_weight_render": ("NGP_OK(ngp_svox_weight_render(0, {W}, {H}, in1_p, {fx}, {fy}, {cx}, {cy}, in0_p, in0_shape0, in0_shape1, in0_shape2, "
+                           "xform_p, 0.5f, 0.2f, out0_p));"),
+    "svox_dilate": "NGP_OK(ngp_svox_dilate(0, in0_shape0, in0_shape1, in0_shape2, (const uint8_t*)in0_p, (uint8_t*)out0_p));",
+    "svox_compact": ("NGP_OK(ngp_svox_compact(0, in0_shape0, in0_shape1, in0_shape2, (const uint8_t*)in0_p, in1_p, lattice_p, out1_shape0, out3_p, "
+                     "out0_p, out1_p, out2_p));"),
 }
 
 

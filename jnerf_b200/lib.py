@@ -41,6 +41,16 @@ SIGNATURES = {
     "ngp_mip_fwd": (_i32, [_vp, _u32, _u32, _vp, _vp, _i32, _i32, _i32, _vp, _vp, _vp]),
     "ngp_mip_composite_fwd": (_i32, [_vp, _u32, _u32, _vp, _i32, _vp, _vp, _f32, _f32, _i32, _vp, _vp, _vp, _vp]),
     "ngp_mip_composite_loss_bwd": (_i32, [_vp, _u32, _u32, _vp, _i32, _vp, _vp, _vp, _vp, _f32, _f32, _i32, _f32, _f32, _vp, _vp, _vp]),
+    "ngp_svox_train_step": (_i32, [_vp, _u32, _vp, _u32, _u32, _vp, _f32, _f32, _f32, _f32, _vp, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp,
+                                   _vp, _vp, _vp]),
+    "ngp_svox_render": (_i32, [_vp, _u32, _u32, _u32, _vp, _f32, _f32, _f32, _f32, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp]),
+    "ngp_svox_tv_grad": (_i32, [_vp, _vp, _i32, _i32, _i32, _vp, _u32, _u32, _u32, _f32, _i32, _vp, _vp]),
+    "ngp_svox_rmsprop": (_i32, [_vp, _u64, _u64, _vp, _vp, _vp, _vp, _vp, _vp, _f32, _f32, _f32, _f32, _f32]),
+    "ngp_svox_sample": (_i32, [_vp, _u32, _vp, _vp, _i32, _i32, _i32, _vp, _vp, _i32, _vp, _vp]),
+    "ngp_svox_weight_render": (_i32, [_vp, _u32, _u32, _vp, _f32, _f32, _f32, _f32, _vp, _i32, _i32, _i32, _vp, _f32, _f32, _vp]),
+    "ngp_svox_dilate": (_i32, [_vp, _i32, _i32, _i32, _vp, _vp]),
+    "ngp_svox_compact_workspace_bytes": (_i32, [_i32, _i32, _i32, _vp]),
+    "ngp_svox_compact": (_i32, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _u32, _vp, _vp, _vp, _vp]),
     "ngp_mesh_workspace_bytes": (_i32, [_u32, _u64, _u64, _vp]),
     "ngp_density_lattice": (_i32, [_vp, _u32, _vp, _vp, _vp, _vp]),
     "ngp_marching_cubes": (_i32, [_vp, _u32, _vp, _f32, _vp, _vp, _u64, _vp, _u64, _vp]),
@@ -92,6 +102,8 @@ KERNELS_PER_CALL = {
     "ngp_nerf_fwd": 1, "ngp_nerf_density": 1, "ngp_nerf_bwd": 3,
     "ngp_mip_rays": 1, "ngp_mip_sample": 1, "ngp_mip_resample": 1, "ngp_mip_encode": 1, "ngp_mip_fwd": 1, "ngp_mip_composite_fwd": 1,
     "ngp_mip_composite_loss_bwd": 1,
+    "ngp_svox_train_step": 1, "ngp_svox_render": 1, "ngp_svox_tv_grad": 1, "ngp_svox_rmsprop": 1, "ngp_svox_sample": 1, "ngp_svox_weight_render": 1,
+    "ngp_svox_dilate": 1, "ngp_svox_compact": 5,
 }
 launch_count = 0
 _lib = None

@@ -556,3 +556,96 @@ def dp_exchange_step(world, rank, slice_len, n_w, peer_table, peer_table_grad, p
 
 def dp_exchange_wait(world, my_flags, epoch):
     lib.call("ngp_dp_exchange_wait", _stream(), int(world), _p(my_flags), int(epoch))
+
+
+# ---- Plenoxels (include/ngp_b200.h X1-X9; grid = links (X, Y, Z) int32, density (cap,), sh (cap, 27); gradients int64 fixed point) ----
+SVOX_FX_UNIT = 2.0 ** -48          # one unit of the fixed-point gradients
+
+
+def _host_f32(vals):
+    a = np.ascontiguousarray(np.asarray(vals, np.float32).reshape(-1))
+    return a, a.ctypes.data
+
+
+def svox_train_step(pix, W, H, c2w, intrin, images, links, density, sh, xform, opts, grad_density, grad_sh, flag):
+    """One training step of the rays of pixel ids pix (int32, (img * H + y) * W + x): adds the gradient of the MSE into the int64
+    fixed-point grad_density / grad_sh and returns the per-ray squared error (R,).  intrin = (fx, fy, cx, cy); xform = offset[3] +
+    scaling[3] (world -> grid); opts = (step_size, sigma_thresh, stop_thresh, background)."""
+    R = pix.numel()
+    sqerr = torch.empty(R, dtype=torch.float32, device=pix.device)
+    xf, xf_p = _host_f32(xform)
+    op, op_p = _host_f32(opts)
+    X, Y, Z = links.shape
+    lib.call("ngp_svox_train_step", _stream(), R, _p(pix), int(W), int(H), _p(c2w), *(float(v) for v in intrin), _p(images), _p(links), X, Y, Z,
+             _p(density), _p(sh), xf_p, op_p, _p(grad_density), _p(grad_sh), _p(sqerr), _p(flag))
+    return sqerr
+
+
+def svox_render(n, first, W, c2w, intrin, links, density, sh, xform, opts, out=None):
+    """(n, 3) colours of pixels [first, first + n) (row-major) of the camera c2w (12 floats, device)."""
+    if out is None:
+        out = torch.empty((n, 3), dtype=torch.float32, device=links.device)
+    xf, xf_p = _host_f32(xform)
+    op, op_p = _host_f32(opts)
+    X, Y, Z = links.shape
+    lib.call("ngp_svox_render", _stream(), int(n), int(first), int(W), _p(c2w), *(float(v) for v in intrin), _p(links), X, Y, Z, _p(density), _p(sh),
+             xf_p, op_p, _p(out))
+    return out
+
+
+def svox_tv_grad(links, data, start, n_cells, scale, ignore_edge, grad, flag):
+    """Sparse TV of data (cap, dim) over the cells (start + i) mod (X Y Z), i < n_cells, added into grad (int64 fixed point)."""
+    X, Y, Z = links.shape
+    dim = data.shape[1] if data.dim() == 2 else 1
+    lib.call("ngp_svox_tv_grad", _stream(), _p(links), X, Y, Z, _p(data), dim, int(start), int(n_cells), float(scale), int(bool(ignore_edge)), _p(grad),
+             _p(flag))
+
+
+def svox_rmsprop(density, sh, grad_density, grad_sh, rms_density, rms_sh, lr_density, lr_sh, alpha_density, alpha_sh, eps):
+    """RMSprop of both tensors from their fixed-point gradients, which are cleared."""
+    lib.call("ngp_svox_rmsprop", _stream(), density.numel(), sh.numel(), _p(density), _p(sh), _p(grad_density), _p(grad_sh), _p(rms_density), _p(rms_sh),
+             float(lr_density), float(lr_sh), float(alpha_density), float(alpha_sh), float(eps))
+
+
+def svox_sample(points, links, density, sh, want_sh):
+    """Trilerp at points (n, 3) in grid coordinates -> (density (n,), sh (n, 27) or None)."""
+    n = points.shape[0]
+    d = torch.empty(n, dtype=torch.float32, device=points.device)
+    s = torch.empty((n, 27), dtype=torch.float32, device=points.device) if want_sh else None
+    X, Y, Z = links.shape
+    lib.call("ngp_svox_sample", _stream(), n, _p(points), _p(links), X, Y, Z, _p(density), _p(sh), int(bool(want_sh)), _p(d), _p(s))
+    return d, s
+
+
+def svox_weight_render(data, W, H, c2w, intrin, xform, step_size, stop_thresh, out):
+    """Max-accumulates into out (X, Y, Z) the weights of one camera's rays through the dense density grid data (X, Y, Z)."""
+    xf, xf_p = _host_f32(xform)
+    X, Y, Z = data.shape
+    lib.call("ngp_svox_weight_render", _stream(), int(W), int(H), _p(c2w), *(float(v) for v in intrin), _p(data), X, Y, Z, xf_p, float(step_size),
+             float(stop_thresh), _p(out))
+    return out
+
+
+def svox_dilate(mask):
+    out = torch.empty_like(mask)
+    X, Y, Z = mask.shape
+    lib.call("ngp_svox_dilate", _stream(), X, Y, Z, _p(mask), _p(out))
+    return out
+
+
+def svox_compact(mask, dense_density, lattice, capacity):
+    """mask (X, Y, Z) uint8 with `capacity` kept cells -> (links (X, Y, Z) int32, density (capacity,), centres (capacity, 3) of the kept
+    cells, lattice[0:3] + index * lattice[3:6])."""
+    import ctypes as C
+    X, Y, Z = mask.shape
+    nb = C.c_uint64()
+    lib.call("ngp_svox_compact_workspace_bytes", X, Y, Z, C.addressof(nb))
+    dev = mask.device
+    ws = torch.empty(nb.value, dtype=torch.uint8, device=dev)
+    links = torch.empty((X, Y, Z), dtype=torch.int32, device=dev)
+    dens = torch.empty(capacity, dtype=torch.float32, device=dev)
+    pts = torch.empty((capacity, 3), dtype=torch.float32, device=dev)
+    lt, lt_p = _host_f32(lattice)
+    lib.call("ngp_svox_compact", _stream(), X, Y, Z, _p(mask), _p(dense_density), lt_p, int(capacity), _p(ws), _p(links), _p(dens) if capacity else None,
+             _p(pts) if capacity else None)
+    return links, dens, pts

@@ -174,3 +174,36 @@ class LinearLog:
 
     def load_state_dict(self, sd):
         self.steps = sd["steps"]
+
+
+@OPTIMS.register_module()
+class PlenOptimRMSprop:
+    """contrib/plenoxel optims/svox2_optim.py:59-81: Jittor's nn.RMSprop with one group for the density and one for the SH, dense over
+    every entry: v = alpha v + (1 - alpha) g^2, p -= lr g / (sqrt(v) + eps) (Jittor's documented RMSprop; DESIGN.md section 12).  It owns
+    the gradients, as Jittor's optimizer does: int64 fixed-point sums (ops.SVOX_FX_UNIT a unit) that the training kernels add into and
+    step() reads and clears, and the device flag those kernels set when a term or sum leaves the fixed-point range."""
+
+    def __init__(self, p_density, p_sh, lr_sigma, lr_sh, alpha_sigma, alpha_sh, eps=1e-8):
+        self.p_density, self.p_sh = p_density, p_sh
+        self.lr_sigma, self.lr_sh, self.alpha_sigma, self.alpha_sh, self.eps = lr_sigma, lr_sh, alpha_sigma, alpha_sh, eps
+        dev = p_density.device
+        self.rms_density, self.rms_sh = torch.zeros_like(p_density), torch.zeros_like(p_sh)
+        self.grad_density = torch.zeros(p_density.shape, dtype=torch.int64, device=dev)
+        self.grad_sh = torch.zeros(p_sh.shape, dtype=torch.int64, device=dev)
+        self.flag = torch.zeros(1, dtype=torch.int32, device=dev)
+
+    def update_lr(self, lr_sigma, lr_sh, alpha_sigma, alpha_sh):
+        self.lr_sigma, self.lr_sh, self.alpha_sigma, self.alpha_sh = lr_sigma, lr_sh, alpha_sigma, alpha_sh
+
+    def zero_grad(self):
+        self.grad_density.zero_()
+        self.grad_sh.zero_()
+
+    def step(self):
+        ops.svox_rmsprop(self.p_density, self.p_sh, self.grad_density, self.grad_sh, self.rms_density, self.rms_sh, self.lr_sigma, self.lr_sh,
+                         self.alpha_sigma, self.alpha_sh, self.eps)
+
+    def check_overflow(self):
+        """Raises if a gradient left the fixed-point range since the optimizer was built (reads the device flag: a synchronisation)."""
+        if int(self.flag.item()):
+            raise FloatingPointError("PlenOptimRMSprop: a gradient term or sum left the 64-bit fixed-point range (or was not finite)")
