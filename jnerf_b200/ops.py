@@ -176,10 +176,15 @@ def nerf_density(pos, params):
     return out
 
 
-def nerf_bwd(params, saved, dout, n_dev=None):
-    """dout (N,4) fp16 + nerf_fwd's saved activations -> fp32 gradient of the flat parameter vector."""
+def nerf_bwd(params, saved, dout, n_dev=None, scratch=None):
+    """dout (N,4) fp16 + nerf_fwd's saved activations -> fp32 gradient of the flat parameter vector.  scratch: None, or a caller-owned
+    uint8 buffer of at least nerf_workspace_bytes(N)[1] bytes; it then holds every layer's pre-activation gradient and the per-chunk
+    weight-gradient partial sums afterwards."""
     n = dout.shape[0]
-    scratch = torch.empty(nerf_workspace_bytes(n)[1], dtype=torch.uint8, device=dout.device)
+    need = nerf_workspace_bytes(n)[1]
+    if scratch is None:
+        scratch = torch.empty(need, dtype=torch.uint8, device=dout.device)
+    assert scratch.dtype == torch.uint8 and scratch.numel() >= need, "nerf_bwd: scratch is smaller than nerf_workspace_bytes(N)[1]"
     grad = torch.empty(params.numel(), dtype=torch.float32, device=dout.device)
     lib.call("ngp_nerf_bwd", _stream(), n, _p(n_dev), _p(params), _p(saved), _p(dout), _p(scratch), _p(grad))
     return grad
