@@ -1,7 +1,8 @@
-"""NerfDataset (mirror of dataset/dataset.py:16-270) and SyntheticNerfDataset, the stand-in used when the
-NeRF-synthetic `lego` scene is unavailable (the reference downloads it at run time, dataset_util.py:101-109).
+"""NerfDataset (mirror of dataset/dataset.py:16-270), LLFFDataset (mirror of dataset/llff_dataset.py: forward-facing captures in the
+`poses_bounds.npy` layout) and SyntheticNerfDataset, the stand-in used when the NeRF-synthetic `lego` scene is unavailable (the
+reference downloads it at run time, dataset_util.py:101-109); write_synthetic_llff writes a forward-facing stand-in to disk.
 
-Both expose what the sampler / runner read: n_images, resolution [W,H], aabb_scale, aabb_range, metadata (n,11),
+All expose what the sampler / runner read: n_images, resolution [W,H], aabb_scale, aabb_range, metadata (n,11),
 focal_lengths (n,2), transforms_gpu (n, 3x4 stored column-major = 12 floats, dataset.py:164-165), image_data
 (n, H*W, 4), batch_size and __next__() -> (img_ids, rays_o, rays_d, rgba)."""
 import json
@@ -142,6 +143,153 @@ class NerfDataset(_RayBatcher):
         self._finish_init()
 
 
+def _normalize(x):
+    return x / np.linalg.norm(x)
+
+
+def _viewmatrix(z, up, pos):
+    """dataset_util.py:92-98: camera-to-world [x, y, z | pos] looking along z with `up` roughly upwards."""
+    z = _normalize(z)
+    x = _normalize(np.cross(up, z))
+    return np.stack([x, _normalize(np.cross(z, x)), z, pos], 1)
+
+
+def _poses_avg(poses):
+    """llff_dataset.py:181-190: the mean camera (3x5) of (n,3,5) poses -- mean position, summed viewing and up axes."""
+    c2w = _viewmatrix(poses[:, :3, 2].sum(0), poses[:, :3, 1].sum(0), poses[:, :3, 3].mean(0))
+    return np.concatenate([c2w, poses[0, :3, -1:]], 1)
+
+
+def _recenter_poses(poses):
+    """llff_dataset.py:167-179: all cameras expressed in the frame of the mean camera."""
+    out = poses + 0
+    bottom = np.reshape([0, 0, 0, 1.0], [1, 4])
+    c2w = np.concatenate([_poses_avg(poses)[:3, :4], bottom], -2)
+    full = np.concatenate([poses[:, :3, :4], np.tile(bottom[None], [poses.shape[0], 1, 1])], -2)
+    out[:, :3, :4] = (np.linalg.inv(c2w) @ full)[:, :3, :4]
+    return out
+
+
+def _image_files(d):
+    return [os.path.join(d, f) for f in sorted(os.listdir(d)) if f.endswith(("JPG", "jpg", "png"))]                 # llff_dataset.py:213-214
+
+
+@DATASETS.register_module()
+class LLFFDataset(_RayBatcher):
+    """Forward-facing captures as LLFF / COLMAP `imgs2poses` writes them: root_dir/poses_bounds.npy (n,17) and root_dir/images_{factor}
+    (or root_dir/images, reduced in memory when the former is missing).  Nothing is written into root_dir (DESIGN.md section 7)."""
+
+    def __init__(self, root_dir, batch_size, mode="train", factor=4, llffhold=0, recenter=True, bd_factor=.75, spherify=False,
+                 correct_pose=(1, -1, -1), aabb_scale=None, scale=None, offset=None, img_alpha=True, to_jt=True, have_img=True,
+                 preload_shuffle=True, seed=0):
+        from PIL import Image
+        assert mode in ("train", "val", "test")
+        if not isinstance(factor, int) or isinstance(factor, bool) or factor < 1:
+            raise ValueError(f"LLFFDataset: factor must be a positive integer, got {factor!r}")                      # llff_dataset.py:48,204-206
+        self.root_dir, self.batch_size, self.mode, self.seed = root_dir, batch_size, mode, seed
+        self.scale, self.offset = NERF_SCALE, [0.5, 0.5, 0.5]          # the `scale` / `offset` arguments are discarded (llff_dataset.py:24-25)
+        self.correct_pose = tuple(correct_pose)
+        self.have_img = have_img                                        # images are read whatever this says (llff_dataset.py:91-94)
+        # `spherify` is accepted and ignored, as in the reference (its load_data never reads it)
+        if aabb_scale is None:
+            print("llff dataset need set aabbscale in config file ,automatically set to 32")                          # llff_dataset.py:32-34
+            aabb_scale = 32
+        self.aabb_scale = aabb_scale
+        arr = np.load(os.path.join(root_dir, "poses_bounds.npy"))
+        poses = arr[:, :-2].reshape([-1, 3, 5]).transpose([1, 2, 0])                                                  # (3,5,n), :195
+        bds = arr[:, -2:].transpose([1, 0])                                                                           # (2,n), :196
+        imgdir = os.path.join(root_dir, f"images_{factor}")
+        reduce_here = not os.path.isdir(imgdir)                         # the reference runs ImageMagick inside root_dir then (:229-275)
+        files = _image_files(os.path.join(root_dir, "images") if reduce_here else imgdir)
+        if poses.shape[-1] != len(files):
+            raise ValueError(f"LLFFDataset: {len(files)} images in {os.path.dirname(files[0]) if files else root_dir} but "
+                             f"{poses.shape[-1]} poses in poses_bounds.npy")
+
+        def read(path):
+            im = Image.open(path)
+            if reduce_here and factor > 1:
+                im = im.resize((int(round(im.width / factor)), int(round(im.height / factor))), Image.BOX)
+            im = np.asarray(im)
+            if im.ndim == 2:
+                im = im[..., None].repeat(3, -1)
+            if img_alpha and im.shape[-1] == 3:                                                                       # :130-132
+                im = np.concatenate([im, np.full(im.shape[:2] + (1,), 255, np.uint8)], -1)
+            return im
+        first = read(files[0])
+        poses[:2, 4, :] = np.array(first.shape[:2]).reshape([2, 1])                                                   # :221-223
+        poses[2, 4, :] = poses[2, 4, :] * 1. / factor
+        poses = np.concatenate([poses[:, 1:2, :], -poses[:, 0:1, :], poses[:, 2:, :]], 1)                             # [down,right,back] -> [right,up,back], :139-140
+        poses = np.moveaxis(poses, -1, 0).astype(np.float32)
+        bds = np.moveaxis(bds, -1, 0).astype(np.float32)
+        sc = 1. if bd_factor is None else 1. / (bds.min() * bd_factor)                                                # :147-149
+        poses[:, :3, 3] *= sc
+        bds *= sc
+        if recenter:
+            poses = _recenter_poses(poses)
+        n = poses.shape[0]
+        if llffhold > 0:                                                                                              # :57-59
+            i_test = np.arange(n)[::llffhold]
+        else:                                                           # the view closest to the mean camera, :155-160
+            i_test = np.array([np.argmin(np.sum(np.square(_poses_avg(poses)[:3, 3] - poses[:, :3, 3]), -1))])
+        # val is the test set, train is the rest (:60-62); the reference also writes this split to root_dir/split.json
+        self.i_select = np.array([i for i in range(n) if i not in i_test]) if mode == "train" else np.asarray(i_test)
+        hwf = poses[0, :3, -1]
+        self.H, self.W = int(hwf[0]), int(hwf[1])                                                                     # :88-90,121-122
+        self._focal = (float(hwf[2]), float(hwf[2]))
+        self._cx, self._cy = self.W / 2, self.H / 2                                                                   # :106-107
+        poses = poses[:, :3, :4].astype(np.float32)
+        self.poses = [poses[i].copy() for i in self.i_select]                                  # NeRF camera-to-world, recentred and rescaled
+        self._xforms = [matrix_nerf2ngp(p, self.scale, self.offset, self.correct_pose) for p in self.poses]
+        imgs = [first if i == 0 else read(files[i]) for i in self.i_select]
+        self.image_data = torch.from_numpy(np.stack(imgs)).to(DEVICE).reshape(len(imgs), self.H * self.W, -1)
+        self._finish_init()
+
+
+def write_synthetic_llff(dst, n_images=20, H=378, W=504, factor=None, seed=0, radius=4.0, extent=0.6, obj_scale=2.2, backdrop_radius=8.0):
+    """A forward-facing stand-in on disk, in the layout LLFFDataset reads: dst/poses_bounds.npy and dst/images/*.png of H x W pixels (with
+    `factor` also dst/images_{factor}, box-reduced).  Cameras sit on a jittered planar grid of half-width `extent` (NeRF world units) at
+    `radius` from the scene and all look at it, as in a hand-held forward-facing capture; the images are ray-traced from
+    SyntheticNerfDataset.shade with the opaque backdrop of the "fox" style (every pixel has alpha 1), the two bounds of a view are its
+    nearest and farthest analytic hit.  Returns the NeRF camera-to-world matrices [right, up, back | t] it wrote (n,3,4)."""
+    from PIL import Image
+    rng = np.random.default_rng(seed)
+    scene = object.__new__(SyntheticNerfDataset)
+    scene.scale, scene.obj_scale, scene.backdrop_radius = NERF_SCALE, obj_scale, backdrop_radius
+    focal = 0.81 * W                                                    # the field of view of a phone camera (the fern capture: 3260 / 4032)
+    p0 = radius * np.array([math.cos(math.radians(20.0)), 0.0, math.sin(math.radians(20.0))])
+    fwd0 = -p0 / np.linalg.norm(p0)
+    right0 = _normalize(np.cross(fwd0, [0, 0, 1.0]))
+    up0 = np.cross(right0, fwd0)
+    side = math.ceil(math.sqrt(n_images))
+    os.makedirs(os.path.join(dst, "images"), exist_ok=True)
+    if factor:
+        os.makedirs(os.path.join(dst, f"images_{factor}"), exist_ok=True)
+    v, u = torch.meshgrid(torch.arange(H, device=DEVICE), torch.arange(W, device=DEVICE), indexing="ij")
+    d_cam = torch.stack([(u.reshape(-1) + 0.5 - W / 2) / focal, (v.reshape(-1) + 0.5 - H / 2) / focal, torch.ones(H * W, device=DEVICE)], -1)
+    rows, mats = [], []
+    for k in range(n_images):
+        g = (np.array([k % side, k // side]) + rng.uniform(-0.3, 0.3, 2)) / max(side - 1, 1) * 2 - 1
+        pos = p0 + extent * (g[0] * right0 + g[1] * up0)
+        back = _normalize(pos)                                          # the camera looks along -z at the scene centre
+        right = _normalize(np.cross(-back, [0, 0, 1.0]))
+        up = np.cross(right, -back)
+        c2w = np.stack([right, up, back, pos], 1)
+        xf = torch.from_numpy(matrix_nerf2ngp(c2w, NERF_SCALE, [0.5, 0.5, 0.5])).to(DEVICE)
+        d = torch.nn.functional.normalize(d_cam @ xf[:, :3].T, dim=-1)
+        rgba, t = scene.shade(xf[:, 3].expand(H * W, 3).contiguous(), d.contiguous(), return_t=True)
+        t = t / NERF_SCALE                                              # NGP units -> NeRF world units
+        img = (rgba[:, :3] * 255.0 + 0.5).clamp(0, 255).to(torch.uint8).reshape(H, W, 3).cpu().numpy()
+        im = Image.fromarray(img, "RGB")
+        im.save(os.path.join(dst, "images", f"image{k:03d}.png"))
+        if factor:
+            im.resize((int(round(W / factor)), int(round(H / factor))), Image.BOX).save(os.path.join(dst, f"images_{factor}", f"image{k:03d}.png"))
+        m = np.concatenate([np.stack([-up, right, back, pos], 1), np.array([[H], [W], [focal]])], 1)      # inverse of llff_dataset.py:139-140
+        rows.append(np.concatenate([m.reshape(-1), [float(t.min()), float(t.max())]]))
+        mats.append(c2w)
+    np.save(os.path.join(dst, "poses_bounds.npy"), np.stack(rows))
+    return np.stack(mats)
+
+
 def synthetic_cameras(n_images, radius=4.0, seed=0, azimuth=(0.0, 360.0), elevation=(5.0, 85.0)):
     """Camera-to-world matrices (NeRF/blender convention, looking at the origin) on a sphere of `radius`,
     upper hemisphere like NeRF-synthetic (cf. dataset/camera_path.py:27-28 which also uses radius 4); `azimuth` / `elevation`
@@ -228,8 +376,9 @@ class SyntheticNerfDataset(_RayBatcher):
             out[i] = (self.shade(o, d) * 255.0 + 0.5).clamp(0, 255).to(torch.uint8)
         return out
 
-    def shade(self, o, d):
-        """RGBA in [0,1] of the analytic scene along rays (o,d) given in NGP coordinates."""
+    def shade(self, o, d, return_t=False):
+        """RGBA in [0,1] of the analytic scene along rays (o,d) given in NGP coordinates; with `return_t` also the distance to the
+        hit (inf where the ray leaves the scene)."""
         n = o.shape[0]
         t_best = torch.full((n,), float("inf"), device=o.device)
         col = torch.zeros((n, 3), device=o.device)
@@ -289,4 +438,5 @@ class SyntheticNerfDataset(_RayBatcher):
         alpha = torch.isfinite(t_best).float()
         lam = 0.35 + 0.65 * (nrm * light).sum(-1).clamp_min(0)
         rgb = (col * lam[:, None]).clamp(0, 1) * alpha[:, None]
-        return torch.cat([rgb, alpha[:, None]], -1)
+        rgba = torch.cat([rgb, alpha[:, None]], -1)
+        return (rgba, t_best) if return_t else rgba

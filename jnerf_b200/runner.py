@@ -907,6 +907,18 @@ def fox_cfg(fp16=True, synthetic=True, **over):
     return c
 
 
+def llff_cfg(root_dir, fp16=True, **over):
+    """projects/ngp/configs/ngp_llff.py key for key (a forward-facing LLFF capture: images reduced 8x, every 8th view held out,
+    aabb_scale 64 -> 7 occupancy cascades, cone stepping, fp16) with the capture's directory taken from `root_dir`."""
+    c = lego_cfg(fp16=fp16, synthetic=False)
+    split = lambda mode, **kw: dict(type="LLFFDataset", root_dir=root_dir, batch_size=4096, mode=mode, **kw, factor=8, llffhold=8, aabb_scale=64)
+    c.update(dataset_type="LLFFDataset", dataset_dir=root_dir,
+             dataset=dict(train=split("train"), val=split("val", preload_shuffle=False), test=split("test", preload_shuffle=False)),
+             exp_name="fern", const_dt=False)
+    c.update(over)
+    return c
+
+
 def nerf_cfg(fp16=True, synthetic=True, **over):
     """projects/nerf/configs/nerf_base.py key for key (vanilla NeRF: FrequencyEncoder(10) / FrequencyEncoder(4), OriginNeRFNetworks, Adam
     lr 1e-2, 512 rays a batch, 200 000 steps); `synthetic` swaps data/lego for the procedural stand-in."""

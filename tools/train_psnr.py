@@ -2,6 +2,7 @@
 """Train the lego configuration on the synthetic stand-in scene and report held-out PSNR against steps and device time.
 
     python tools/train_psnr.py [--steps 5000] [--images 100] [--res 400] [--evals 500,1000,2000,5000] [--out gpurun_out/psnr.json]
+    python tools/train_psnr.py --workload llff [--data-dir CAPTURE] [--images 40]
 
 This is the quality check that goes with bench.py's throughput number: same Runner.train_step path, same configuration
 (projects/ngp/configs/ngp_base.py + fp16), validation views drawn from cameras the model never trains on
@@ -27,18 +28,31 @@ def main():
                     help="BASELINE metric 'PSNR@5min': keep training after --steps until this much device time has been spent on training "
                          "steps or the configuration's tot_train_steps (40 000, ngp_base.py) is reached, then evaluate once more")
     ap.add_argument("--data-dir", default=None, help="a real capture in the reference's dataset layout (train/val splits) instead of the stand-in")
-    ap.add_argument("--workload", default="lego", choices=["lego", "fox"],
-                    help="fox = projects/ngp/configs/ngp_fox.py (aabb_scale from the capture, cone stepping); PSNR on training views (the capture has no val split)")
+    ap.add_argument("--workload", default="lego", choices=["lego", "fox", "llff"],
+                    help="fox = projects/ngp/configs/ngp_fox.py (aabb_scale from the capture, cone stepping); PSNR on training views (the capture has no val split). "
+                         "llff = projects/ngp/configs/ngp_llff.py (aabb_scale 64: 7 occupancy cascades, every 8th view held out) on --data-dir, an LLFF "
+                         "capture (poses_bounds.npy + images/), or on the forward-facing stand-in written to a temporary directory")
     args = ap.parse_args()
 
     import torch
     from jnerf_b200 import lib, plugin  # noqa: F401
-    from jnerf_b200.runner import Runner, fox_cfg, lego_cfg
+    from jnerf_b200.runner import Runner, fox_cfg, lego_cfg, llff_cfg
     from jnerf_b200.utils.config import get_cfg, update_cfg
 
     lib.load()
     get_cfg().clear()
-    if args.workload == "fox":
+    tmp = None
+    if args.workload == "llff":
+        root = args.data_dir
+        if root is None:
+            import tempfile
+            from jnerf_b200.plugin.dataset import write_synthetic_llff
+            tmp = tempfile.TemporaryDirectory()
+            root = tmp.name
+            write_synthetic_llff(root, n_images=args.images, H=8 * 192, W=8 * 256)    # read at 192 x 256 (factor 8); the fern capture is read at 378 x 504
+        update_cfg(**llff_cfg(root, fp16=True, seed=1))
+        cfg = get_cfg()
+    elif args.workload == "fox":
         update_cfg(**fox_cfg(fp16=True, synthetic=args.data_dir is None, seed=1))
         cfg = get_cfg()
         if args.data_dir:
@@ -83,6 +97,9 @@ def main():
     if args.workload == "fox":
         res["config"] = (f"ngp_fox.py (fp16, cone stepping) on {args.data_dir or 'the synthetic fox stand-in'}, PSNR on {args.val_images} training views "
                          f"(the capture has no validation split)")
+    if args.workload == "llff":
+        res["config"] = (f"ngp_llff.py (fp16, cone stepping, aabb_scale 64) on {args.data_dir or 'the forward-facing stand-in'}: "
+                         f"{runner.dataset['train'].n_images} training views of {runner.W}x{runner.H}, PSNR on {args.val_images} held-out views")
     if args.budget_seconds > 0:
         tot = int(cfg.tot_train_steps or 40000)
         while train_ms * 1e-3 < args.budget_seconds and done < tot:
@@ -102,6 +119,8 @@ def main():
     if args.out:
         os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
         json.dump(res, open(args.out, "w"), indent=1)
+    if tmp is not None:
+        tmp.cleanup()
 
 
 if __name__ == "__main__":
