@@ -775,6 +775,102 @@ void orc_composite_bwd(uint32_t n_rays, uint32_t n_elements, const void* net, in
         }
     }
 }
+/* The composite in float64 with a per-entry error bound for an fp32 evaluation of it (the bound is derived in
+ * tests/test_gpu_composite_reference.py).  Every value below is an (exact value, absolute error bound) pair; the rules:
+ *   ev_mul / ev_add: a rounded fp32 operation on inputs with errors ea, eb: |a| eb + |b| ea + ea eb, plus u (|v| + e) for the
+ *     rounding and 2^-150 for a result in the subnormal range (u = 2^-24);
+ *   __expf(x): relative (2 + floor(1.173 |x|)) 2^-23, plus 2^-126 for a flushed subnormal result;
+ *   logistic_sfu: __expf, one rounded add, __fdividef (2 ulp = 4u, and 0 for a denominator beyond 2^126, so 2^-126 absolute);
+ *   products of m transmittance factors and sums of m non-negative fmaf terms: gamma_m = m u / (1 - m u) of the magnitude, any
+ *     association (a sum of m terms in any binary tree rounds at most m times on the way from a term to the result).
+ * dt is the kernel's own fp32 value (nerf_unwarp_dt is one fmaf); net rows, bg, lg, rr, loss_scale and l1 are exact inputs.
+ * numsteps_in == NULL: inference (no background).  lg == NULL: forward only. */
+typedef struct { double v, e; } ev;
+#define EV_U 0x1p-24
+#define EV_TINY 0x1p-150
+static inline ev ev_exact(double v) { ev r = {v, 0.0}; return r; }
+static inline ev ev_round(double v, double e) { ev r = {v, e + EV_U * (fabs(v) + e) + EV_TINY}; return r; }
+static inline ev ev_mul(ev a, ev b) { return ev_round(a.v * b.v, fabs(a.v) * b.e + fabs(b.v) * a.e + a.e * b.e); }
+static inline ev ev_add(ev a, ev b) { return ev_round(a.v + b.v, a.e + b.e); }
+static inline double expf_rel(double x) { return (2.0 + floor(1.173 * fabs(x))) * 0x1p-23; }
+static inline double gamma_m(double m) { return m * EV_U / (1.0 - m * EV_U); }
+
+void orc_composite_f64(uint32_t n_rays, const void* net, int is_half, const float* coords, const uint32_t* numsteps_in,
+                       const uint32_t* numsteps_c, const float* bg, uint32_t cascades, float loss_scale, float l1,
+                       const float* lg, const float* rr, double* rgb, double* rgb_err, double* T_final, double* T_err,
+                       double* alpha, double* alpha_err, double* dnet, double* dnet_err) {
+    march_cfg c = make_cfg(cascades, 1);
+    const float max_step = c.min_cone * (float)(1u << (cascades - 1)), span = max_step - c.min_cone;
+    for (uint32_t i = 0; i < n_rays; ++i) {
+        const uint32_t n = numsteps_c[2 * i], base = numsteps_c[2 * i + 1];
+        const int full = numsteps_in != NULL && n == numsteps_in[2 * i];
+        double T = 1, Tu = 1, Tl = 1;                    /* exact transmittance, and with every factor at its upper / lower bound */
+        double P[3] = {0, 0, 0}, D[3] = {0, 0, 0}, M[3] = {0, 0, 0};   /* sum w c, its propagated error, sum of magnitudes */
+        for (uint32_t j = 0; j < n; ++j) {
+            const size_t k = (size_t)(base + j) * 4;
+            const double o[4] = {NET(k), NET(k + 1), NET(k + 2), NET(k + 3)};
+            const double dt = fmaf(coords[(size_t)(base + j) * 7 + 3], span, c.min_cone);
+            ev col[3];
+            for (int q = 0; q < 3; ++q) {
+                const double E = exp(-o[q]), cq = 1.0 / (1.0 + E), om = isinf(E) ? 1.0 : E / (1.0 + E);   /* om = 1 - c */
+                const double rel = (1 + 4 * EV_U) / ((1 - om * expf_rel(o[q])) * (1 - EV_U)) - 1;
+                col[q].v = cq; col[q].e = cq * rel + 0x1p-126;
+            }
+            /* alpha = 1 - exp(-sigma dt): bracket the kernel's exp(fl(-fl(__expf(o_w)) dt)) */
+            const double sig = exp(o[3]), es = expf_rel(o[3]);
+            const double z = -sig * dt, E2 = exp(z), a = -expm1(z), f = E2;
+            const double zlo = -(sig * (1 + es) + 0x1p-126) * dt * (1 + EV_U), zhi = -fmax(sig * (1 - es) - 0x1p-126, 0.0) * dt * (1 - EV_U);
+            const double ez = isinf(zlo) ? 0.0 : expf_rel(zlo);
+            const double E2hi = exp(zhi) * (1 + ez) + 0x1p-126, E2lo = fmax(exp(zlo) * (1 - ez) - 0x1p-126, 0.0);
+            double A = fmax(E2hi - E2, E2 - E2lo);
+            A += EV_U * (a + A);                                             /* alpha = fl(1 - E2) */
+            const double Phi = A + EV_U * (f + A);                            /* the factor fl(1 - alpha) */
+            const double g_b = gamma_m(j), g_a = gamma_m(j + 1);
+            const ev Tb = {T, fmax(Tu - T, T - Tl) + g_b * Tu + j * EV_TINY};
+            const ev w = ev_mul((ev){a, A}, Tb);
+            T *= f; Tu *= f + Phi; Tl *= fmax(f - Phi, 0.0);
+            const ev Ta = {T, fmax(Tu - T, T - Tl) + g_a * Tu + (j + 1) * EV_TINY};
+            for (int q = 0; q < 3; ++q) {                                    /* fmaf: the product w c is not rounded on its own */
+                const double t = w.v * col[q].v, et = fabs(w.v) * col[q].e + fabs(col[q].v) * w.e + w.e * col[q].e;
+                P[q] += t; D[q] += et; M[q] += fabs(t) + et;
+            }
+            if (lg == NULL) continue;
+            ev dl[4], tq[3];
+            for (int q = 0; q < 3; ++q) {
+                const ev run = {P[q], D[q] + gamma_m(j + 1) * M[q] + (j + 1) * EV_TINY};
+                const ev suffix = ev_add(ev_exact(rr[3 * i + q]), (ev){-run.v, run.e});
+                const ev tc = ev_mul(Ta, col[q]);
+                tq[q] = ev_add(tc, (ev){-suffix.v, suffix.e});
+                const ev om = ev_add(ev_exact(1.0), (ev){-col[q].v, col[q].e});
+                const ev g = ev_mul(col[q], om);
+                dl[q] = ev_mul(ev_exact(loss_scale), ev_mul(ev_mul(w, ev_exact(lg[3 * i + q])), g));
+            }
+            /* Eigen's fixed-size redux: x0 + (x1 + x2) */
+            const ev dot = ev_add(ev_mul(ev_exact(lg[3 * i]), tq[0]),
+                         ev_add(ev_mul(ev_exact(lg[3 * i + 1]), tq[1]), ev_mul(ev_exact(lg[3 * i + 2]), tq[2])));
+            const float cl = o[3] < -15.0 ? -15.0f : (o[3] > 15.0 ? 15.0f : (float)o[3]);
+            const double dd = exp((double)cl);
+            dl[3] = ev_mul(ev_exact(loss_scale), ev_mul((ev){dd, dd * expf_rel(cl)}, ev_mul(ev_exact(dt), dot)));
+            if (o[3] < 0) dl[3] = ev_add(dl[3], ev_exact(-(double)l1));
+            for (int q = 0; q < 4; ++q) { dnet[k + q] = dl[q].v; dnet_err[k + q] = dl[q].e; }
+        }
+        const double gn = gamma_m(n);
+        const ev Tn = {T, n ? fmax(Tu - T, T - Tl) + gn * Tu + n * EV_TINY : 0.0};
+        T_final[i] = Tn.v; T_err[i] = Tn.e;
+        alpha[i] = n ? 1 - T : 0; alpha_err[i] = n ? Tn.e + EV_U * (1 - T + Tn.e) : 0;
+        for (int q = 0; q < 3; ++q) {
+            double v = P[q], e = D[q] + gn * M[q] + n * EV_TINY;
+            if (numsteps_in != NULL && n == 0) { v = bg[3 * i + q]; e = 0; }
+            else if (full) {                                                 /* fmaf(T, bg, r): one more rounding */
+                const double b = bg[3 * i + q];
+                v = P[q] + T * b;
+                e = D[q] + Tn.e * b + gamma_m(n + 1) * (M[q] + (T + Tn.e) * b) + (n + 1) * EV_TINY;
+            }
+            rgb[3 * i + q] = v; rgb_err[3 * i + q] = e;
+        }
+    }
+}
+
 /* Huber loss gradient (models/losses/huber_loss.py:11-14), unreduced loss summed by Jittor's backward */
 void orc_huber_grad(uint32_t n, const float* x, const float* target, float delta, float* grad, float* loss) {
     for (uint32_t i = 0; i < n; ++i) {

@@ -310,6 +310,30 @@ def composite_bwd(net, coords, numsteps_c, loss_grad, rgb_ray, mean, cascades=5)
     return dnet
 
 
+def composite_f64(net, coords, numsteps_in, numsteps_c, bg, cascades=5, loss_scale=None, l1=0.0, loss_grad=None, rgb_ray=None):
+    """The composite in float64 with per-entry error bounds for an fp32 evaluation (orc_composite_f64).  numsteps_in None: inference
+    (no background).  loss_grad / rgb_ray None: forward only.  loss_scale defaults to the kernels' fp32 128 / R.  Returns a dict of
+    rgb, rgb_err (R,3), T, T_err, alpha, alpha_err (R,) and, for the backward, dnet, dnet_err (N,4), NaN where no ray covers a row."""
+    R = numsteps_c.shape[0]
+    net = np.ascontiguousarray(net)
+    N = net.shape[0]
+    if loss_scale is None:
+        loss_scale = np.float32(128) / np.float32(R)
+    out = {k: np.zeros((R, 3)) for k in ("rgb", "rgb_err")}
+    out.update({k: np.zeros(R) for k in ("T", "T_err", "alpha", "alpha_err")})
+    bwd = loss_grad is not None
+    out["dnet"] = np.full((N, 4), np.nan) if bwd else None
+    out["dnet_err"] = np.full((N, 4), np.nan) if bwd else None
+    f32 = lambda a: None if a is None else np.ascontiguousarray(a, np.float32)
+    u32 = lambda a: None if a is None else np.ascontiguousarray(a).view(np.uint32)
+    args = [f32(coords), u32(numsteps_in), u32(numsteps_c), f32(bg), f32(loss_grad), f32(rgb_ray)]      # alive until the call returns
+    co, ns_in, ns_c, bg_, lg, rr = (_ptr(a) for a in args)
+    oracle().orc_composite_f64(_u32(R), _ptr(net), _i32(int(net.dtype == np.float16)), co, ns_in, ns_c, bg_, _u32(cascades), _f32(loss_scale),
+                               _f32(l1), lg, rr, _ptr(out["rgb"]), _ptr(out["rgb_err"]), _ptr(out["T"]), _ptr(out["T_err"]),
+                               _ptr(out["alpha"]), _ptr(out["alpha_err"]), _ptr(out["dnet"]), _ptr(out["dnet_err"]))
+    return out
+
+
 def ref_composite(net, coords, numsteps_in, numsteps_c, bg, loss_grad=None, mean=0.0):
     r = ref("ref_sampler_cpu_constdt")
     R = numsteps_c.shape[0]
