@@ -90,7 +90,9 @@ int ngp_mlp_param_count(uint32_t n_hidden_matmuls);
 /* ---- R7+R2+R4 fused: NGPNetworks.execute (models/networks/ngp_network.py:77-84) -----------------------
  * coords (n_max,7) f32 = NerfCoordinate {pos[3], dt, dir[3]} (DGS/op_header/ray_sampler_header.h:548-574).
  * n_dev: optional device uint32 with the live row count (rows beyond it are skipped, no host sync); NULL = n_max.
- * out (n_max,4) fp16 = {rgb, sigma_raw}; enc_save (n_max,32) fp16 (kept for backward) may be NULL. */
+ * out (n_max,4) fp16 = {rgb, sigma_raw}; enc_save (n_max,32) fp16 (kept for backward) may be NULL.
+ * Rows at or past the live count are not written, except that a 16-byte-aligned enc_save may also have the rows of the last live
+ * 128-row tile written up to the tile's end or n_max (they are stored by TMA, one whole tile at a time). */
 int ngp_network_fwd(void* stream, uint32_t n_max, const uint32_t* n_dev, const float* coords, const void* grid,
                     const void* levels_dev, const void* w_density, const void* w_rgb, void* out, void* enc_save);
 /* Backward of the above: dout (n_max,4) fp16 -> grid_grad (fp16, ACCUMULATED: caller zeroes),

@@ -48,6 +48,7 @@ import pytest
 import torch
 
 import oracle_lib as ol
+from ngp_fwd_ref import WD_N, WR_N, mirror
 from test_gpu_ops import device_scales
 
 sys.path.insert(0, os.path.join(os.path.dirname(__file__), "golden"))
@@ -56,7 +57,6 @@ from make_bwd_digests import inputs as ray_inputs  # noqa: E402
 pytestmark = pytest.mark.gpu
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-WD_N, WR_N = 64 * 32 + 16 * 64, 64 * 32 + 64 * 64 + 16 * 64
 
 
 def _b3_run():
@@ -83,51 +83,6 @@ def _levels(aabb, log2T):
     if (aabb, log2T) not in _TABLES:
         _TABLES[(aabb, log2T)] = (ops.HashLevels(aabb, log2_hashmap_size=log2T), ol.HashCfg(aabb, log2_hashmap_size=log2T))
     return _TABLES[(aabb, log2T)]
-
-
-# ------------------------------------------------------------------------------------------------ float64 mirror of the chain
-def _h(x):
-    """One fp16 rounding, where the kernel stores a value to a slab."""
-    return x.to(torch.float16).to(torch.float64)
-
-
-def mirror(enc, sh, dout, wd, wr):
-    """The fused network's forward and backward in float64 from fp16 tensors enc (n,32), sh (n,16), dout (n,4), wd, wr (flat), on their
-    device.  Returns out (n,4), the slab values, d_enc, and per weight vector (dwd, dwr) the gradient and the sum of |term|."""
-    f = lambda t: t.to(torch.float64)
-    wd, wr = f(wd), f(wr)
-    W0d, Woutd = wd[:2048].view(64, 32), wd[2048:].view(16, 64)
-    W0r, W1r, Woutr = wr[:2048].view(64, 32), wr[2048:6144].view(64, 64), wr[6144:].view(16, 64)
-    enc, dout = f(enc), f(dout)
-    hd = _h(torch.relu(enc @ W0d.T))
-    h = _h(hd @ Woutd.T)
-    rin = torch.cat([h, f(sh)], 1)
-    h1 = _h(torch.relu(rin @ W0r.T))
-    h2 = _h(torch.relu(h1 @ W1r.T))
-    out = torch.cat([_h(h2 @ Woutr[:3].T), h[:, :1]], 1)
-    dYr = dout[:, :3]
-    g_h2 = _h((dYr @ Woutr[:3]) * (h2 > 0))
-    g_h1 = _h((g_h2 @ W1r) * (h1 > 0))
-    dYd = g_h1 @ W0r[:, :16]
-    dYd[:, 0] += dout[:, 3]                                  # dL/dsigma joins before the one rounding, as the kernel adds it in fp32
-    dYd = _h(dYd)
-    g_hd = _h((dYd @ Woutd) * (hd > 0))
-    d_enc = _h(g_hd @ W0d)
-    pairs_d = [(g_hd, enc), (dYd, hd)]                       # W0d [out][in] = g_hd^T enc, Woutd [out][in] = dYd^T hd
-    pairs_r = [(g_h1, rin), (g_h2, h1), (dYr, h2)]           # W0r, W1r, Woutr (rows >= 3 zero)
-
-    def grads(pairs, n_w):
-        g, a = torch.zeros(n_w, dtype=torch.float64, device=enc.device), torch.zeros(n_w, dtype=torch.float64, device=enc.device)
-        o = 0
-        for x, y in pairs:
-            gx, ax = (x.T @ y).reshape(-1), (x.abs().T @ y.abs()).reshape(-1)
-            g[o:o + gx.numel()], a[o:o + gx.numel()] = gx, ax
-            o += gx.numel() if x.shape[1] != 3 else 16 * 64
-        assert o == n_w
-        return g, a
-
-    slabs = dict(hd=hd, h=h, rin=rin, h1=h1, h2=h2, g_h2=g_h2, g_h1=g_h1, dYd=dYd, g_hd=g_hd, d_enc_abs=g_hd.abs() @ W0d.abs())
-    return out, slabs, d_enc, grads(pairs_d, WD_N), grads(pairs_r, WR_N)
 
 
 def test_mirror_matches_oracle_mlp():
