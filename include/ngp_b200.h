@@ -134,8 +134,9 @@ int ngp_nerf_density(void* stream, uint32_t n, const float* pos, const void* par
 int ngp_nerf_bwd(void* stream, uint32_t n_max, const uint32_t* n_dev, const void* params, const void* saved, const void* dout, void* scratch,
                  float* grad);
 
-/* ---- P1-P7  Mip-NeRF (contrib/mipnerf of the reference: models/samplers/mip_sampler/mip_sampler.py, utils/miputils.py,
- * models/networks/mip_network.py, dataset/nerf_datasets.py:22-235), csrc/mip_sampler.cu + csrc/mip_mlp.cu, DESIGN.md section 11 --------
+/* ---- P1-P13  Mip-NeRF (contrib/mipnerf of the reference: models/samplers/mip_sampler/mip_sampler.py, utils/miputils.py,
+ * models/networks/mip_network.py, dataset/nerf_datasets.py:22-235, dataset/nerf.py), csrc/mip_sampler.cu + csrc/mip_mlp.cu +
+ * csrc/mip_multiscale.cu + csrc/mip_mlp_wide.cu, DESIGN.md section 11 --------------------------------------------------------------------------------------------
  * A ray row is 12 floats: origin[3], direction[3] (unnormalised), viewdir[3], base radius, near, far.  t holds S + 1 fenceposts a ray
  * (S = n_samples <= 128 for the per-ray kernels).  Network rows are (ray, interval) pairs, row r = interval r % S of ray r / S.  The
  * kernels that draw uniforms give ray g the pcg32 draws [g (S + 1), (g + 1)(S + 1)) of the stream at (rng_state, rng_inc), in fencepost
@@ -173,6 +174,28 @@ int ngp_mip_composite_fwd(void* stream, uint32_t n_rays, uint32_t n_samples, con
 int ngp_mip_composite_loss_bwd(void* stream, uint32_t n_rays, uint32_t n_samples, const void* raw, int dtype, const float* t, const float* rays,
                                const float* target, const float* mask, float rgb_padding, float density_bias, int white_bkgd, float coarse_loss_mult,
                                float grad_scale, float* rgb_out, float* loss_out, void* draw_out);
+/* P8: rays, targets and loss weights of the multiscale datasets (dataset/nerf.py: Blenders :207-314, Multicam :108-204), csrc/mip_multiscale.cu.
+ * n_images images of different sizes: global pixel p of image i is offsets[i] + y W_i + x (offsets (n_images + 1) ascending, wh (n_images, 2)
+ * = {W_i, H_i} with H_i >= 3); cams (n_images, 24) = {pix2cam 3x3, cam2world 3x4 (both row-major), lossmult, near, far}; images_rgba
+ * (offsets[n_images], 4), uint8 (read as v / 255) or, with float_images, fp32.  focal != 0: the directions of P1's camera model with that
+ * focal length (Blenders); focal = 0: (x + .5, y + .5, 1) @ pix2cam^T @ cam2world[:3, :3]^T (Multicam).  rays_out (n, 12), target_out
+ * (n, 3) = rgb a + (1 - a) with white_bkgd, else rgb; lossmult_out (n). */
+int ngp_mip_rays_multi(void* stream, uint32_t n, const uint32_t* pix, uint32_t n_images, const uint32_t* offsets, const uint32_t* wh,
+                       const float* cams, float focal, int white_bkgd, const void* images_rgba, int float_images, float* rays_out, float* target_out,
+                       float* lossmult_out);
+/* P10-P13: MipNerfMLP's fused network at degs = 8 or 16 IPE degrees (max_deg_point - min_deg_point), csrc/mip_mlp_wide.cu.  degs = 8 is
+ * P5 + F4 (ngp_nerf_*) unchanged.  degs = 16: kernel layer 0 reads 96 columns, the skip layer 352 (the 96 encoding columns, then h4),
+ * ngp_mip_param_count gives 618 912 fp16 parameters; saved (ngp_mip_workspace_bytes' first size) holds 320 groups of 8 halfs a row.  As
+ * with P5, two forwards whose rows are multiples of 128 may save into consecutive parts of one buffer and share one ngp_mip_bwd_deg,
+ * which writes the fp32 gradient of the flat parameters into grad, deterministically. */
+int ngp_mip_param_count(int degs, uint64_t* count_out);
+int ngp_mip_workspace_bytes(int degs, uint32_t n_max, uint64_t* saved_bytes, uint64_t* scratch_bytes);
+int ngp_mip_fwd_deg(void* stream, uint32_t n_rays, uint32_t n_samples, const float* rays, const float* t, int ray_shape, int integrate,
+                    int min_deg, int degs, const void* params, void* out, void* saved);
+int ngp_mip_bwd_deg(void* stream, uint32_t n_max, int degs, const void* params, const void* saved, const void* dout, void* scratch, float* grad);
+/* P9: P4 at degs = 8 or 16 IPE degrees: enc_out (N, 6 degs), view_out (N, 27).  Equal to P4 bit for bit at degs = 8. */
+int ngp_mip_encode_deg(void* stream, uint32_t n_rays, uint32_t n_samples, const float* rays, const float* t, int ray_shape, int integrate,
+                       int min_deg, int degs, float* enc_out, float* view_out);
 
 /* ---- X1-X9  Plenoxels (contrib/plenoxel of the reference: models/networks/svox2_network.py, ops/svox_ops/op/op_header/*.h),
  * csrc/svox.cu, DESIGN.md section 12 ----------------------------------------------------------------------------------------------

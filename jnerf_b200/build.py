@@ -18,7 +18,9 @@ SOURCES = {
     "fused_net.cu": [],
     "nerf_mlp.cu": [],
     "mip_mlp.cu": [],
+    "mip_mlp_wide.cu": ["-fmad=false"],
     "mip_sampler.cu": ["-fmad=false"],
+    "mip_multiscale.cu": ["-fmad=false"],
     "svox.cu": [],
     "sampler.cu": ["-fmad=false"],
     "grid_update.cu": ["-fmad=false"],

@@ -33,19 +33,27 @@ __device__ __forceinline__ void gaussian(const float* ray, float t0, float t1, u
     var = integrate ? t_var * (d * d) + r_var * (1.f - d * d / d_mag_sq) : 0.f;
 }
 
-// integrated_pos_enc (:242-275) of one coordinate: put(3k + dim, sin(y) e^(-var'/2)) and put(24 + 3k + dim, cos(y) e^(-var'/2)) with
-// y = mean 2^(min_deg+k), var' = var 4^(min_deg+k), k < 8 -- sin(y + pi/2) of the reference as cos(y), full-range sincosf (arguments reach
-// several hundred radians).
-template <class Put>
+// integrated_pos_enc (:242-275) of one coordinate: put(3k + dim, sin(y) e^(-var'/2)) and put(3 DEGS + 3k + dim, cos(y) e^(-var'/2)) with
+// y = mean 2^(min_deg+k), var' = var 4^(min_deg+k), k < DEGS -- sin(y + pi/2) of the reference as cos(y), full-range sincosf (arguments
+// reach several hundred radians at 8 degrees, ~1e5 at 16).
+template <uint32_t DEGS = IPE_DEGS, class Put>
 __device__ __forceinline__ void ipe(float mean, float var, uint32_t dim, int min_deg, Put put) {
 #pragma unroll
-    for (uint32_t k = 0; k < IPE_DEGS; ++k) {
+    for (uint32_t k = 0; k < DEGS; ++k) {
         const float s = ldexpf(1.f, min_deg + (int)k);
         const float e = expf(-0.5f * (var * (s * s)));
         float sn, cs;
         sincosf(mean * s, &sn, &cs);
         put(3 * k + dim, sn * e);
-        put(3 * IPE_DEGS + 3 * k + dim, cs * e);
+        put(3 * DEGS + 3 * k + dim, cs * e);
     }
+}
+
+// Blender camera direction (dataset/nerf_datasets.py:193-235, dataset/nerf.py:265-276): camera_dirs = [(x - W/2 + 0.5) / f,
+// -(y - H/2 + 0.5) / f, -1], direction = camera_dirs @ R^T, in fp32 in numpy's order (callers are built with -fmad=false).
+__device__ __forceinline__ void cam_dir(const float* c2w, float x, float y, uint32_t W, uint32_t H, float focal, float d[3]) {
+    const float cx = (x - W * 0.5f + 0.5f) / focal, cy = -((y - H * 0.5f + 0.5f) / focal), cz = -1.f;
+#pragma unroll
+    for (int j = 0; j < 3; ++j) d[j] = cx * c2w[4 * j] + cy * c2w[4 * j + 1] + cz * c2w[4 * j + 2];
 }
 }  // namespace mip

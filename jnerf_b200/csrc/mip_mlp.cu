@@ -11,6 +11,7 @@ namespace nerf {
 // encode mean 0, variance 0.  dir(): FrequencyEncoder(4) of the ray's viewdir in the kernel's own order; plugin/mip.py permutes the
 // view layer's columns to the reference's pos_enc order.
 struct MipEnc {
+    static constexpr uint32_t EG = 8;
     const float* t;
     uint32_t cylinder, integrate;
     int min_deg;

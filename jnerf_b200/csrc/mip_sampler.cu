@@ -34,13 +34,8 @@ __device__ __forceinline__ float warp_scan(float v, uint32_t lane) {
 // ---- Blender rays (dataset/nerf_datasets.py:193-235) ---------------------------------------------------------------------------------
 // Pixel p = (img * H + y) * W + x.  camera_dirs = [(x - W/2 + 0.5) / f, -(y - H/2 + 0.5) / f, -1], direction = camera_dirs @ R^T, radius
 // = |direction(y) - direction(y + 1)| * 2 / sqrt(12) (the last row takes that of row H - 3, as dx[-2:-1] does), all in fp32 in the order
-// numpy evaluates them (this file is built with -fmad=false); the division by sqrt(12) in fp64, as numpy promotes it.
-__device__ __forceinline__ void cam_dir(const float* c2w, float x, float y, uint32_t W, uint32_t H, float focal, float d[3]) {
-    const float cx = (x - W * 0.5f + 0.5f) / focal, cy = -((y - H * 0.5f + 0.5f) / focal), cz = -1.f;
-#pragma unroll
-    for (int j = 0; j < 3; ++j) d[j] = cx * c2w[4 * j] + cy * c2w[4 * j + 1] + cz * c2w[4 * j + 2];
-}
-
+// numpy evaluates them (this file is built with -fmad=false); the division by sqrt(12) in fp64, as numpy promotes it.  cam_dir is in
+// mip_common.cuh.
 __global__ void mip_rays_kernel(uint32_t n, const uint32_t* __restrict__ pix, uint32_t W, uint32_t H, const float* __restrict__ c2w, float focal,
                                 float near, float far, const uint8_t* __restrict__ images, float* __restrict__ rays, float* __restrict__ target) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;

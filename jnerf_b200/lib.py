@@ -38,6 +38,12 @@ SIGNATURES = {
     "ngp_mip_sample": (_i32, [_vp, _u32, _u32, _vp, _i32, _i32, _u64, _u64, _vp]),
     "ngp_mip_resample": (_i32, [_vp, _u32, _u32, _vp, _vp, _f32, _i32, _u64, _u64, _vp]),
     "ngp_mip_encode": (_i32, [_vp, _u32, _u32, _vp, _vp, _i32, _i32, _i32, _vp, _vp]),
+    "ngp_mip_rays_multi": (_i32, [_vp, _u32, _vp, _u32, _vp, _vp, _vp, _f32, _i32, _vp, _i32, _vp, _vp, _vp]),
+    "ngp_mip_encode_deg": (_i32, [_vp, _u32, _u32, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp]),
+    "ngp_mip_param_count": (_i32, [_i32, _vp]),
+    "ngp_mip_workspace_bytes": (_i32, [_i32, _u32, _vp, _vp]),
+    "ngp_mip_fwd_deg": (_i32, [_vp, _u32, _u32, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp]),
+    "ngp_mip_bwd_deg": (_i32, [_vp, _u32, _i32, _vp, _vp, _vp, _vp, _vp]),
     "ngp_mip_fwd": (_i32, [_vp, _u32, _u32, _vp, _vp, _i32, _i32, _i32, _vp, _vp, _vp]),
     "ngp_mip_composite_fwd": (_i32, [_vp, _u32, _u32, _vp, _i32, _vp, _vp, _f32, _f32, _i32, _vp, _vp, _vp, _vp]),
     "ngp_mip_composite_loss_bwd": (_i32, [_vp, _u32, _u32, _vp, _i32, _vp, _vp, _vp, _vp, _f32, _f32, _i32, _f32, _f32, _vp, _vp, _vp]),
@@ -101,7 +107,8 @@ KERNELS_PER_CALL = {
     "ngp_render_init": 3, "ngp_render_march_round": 3, "ngp_render_composite_round": 3,
     "ngp_nerf_fwd": 1, "ngp_nerf_density": 1, "ngp_nerf_bwd": 3,
     "ngp_mip_rays": 1, "ngp_mip_sample": 1, "ngp_mip_resample": 1, "ngp_mip_encode": 1, "ngp_mip_fwd": 1, "ngp_mip_composite_fwd": 1,
-    "ngp_mip_composite_loss_bwd": 1,
+    "ngp_mip_composite_loss_bwd": 1, "ngp_mip_rays_multi": 1, "ngp_mip_encode_deg": 1, "ngp_mip_fwd_deg": 1,
+    "ngp_mip_bwd_deg": 3,
     "ngp_svox_train_step": 1, "ngp_svox_render": 1, "ngp_svox_tv_grad": 1, "ngp_svox_rmsprop": 1, "ngp_svox_sample": 1, "ngp_svox_weight_render": 1,
     "ngp_svox_dilate": 1, "ngp_svox_compact": 5,
 }

@@ -219,24 +219,76 @@ def mip_resample(t, weights, resample_padding, randomized, rng):
     return out
 
 
-def mip_encode(rays, t, ray_shape="cone", integrate=True, min_deg=0):
-    """fp32 (IPE (N, 48), view encoding (N, 27)) of the N = R * S intervals, in the reference's column orders."""
+def mip_rays_multi(pix, table, focal, white_bkgd):
+    """Rays of the multiscale datasets (include/ngp_b200.h P8) for global pixel ids pix -> (rays (n, 12), target rgb (n, 3), lossmult (n,)).
+    table: offsets (n_img + 1) int32, wh (n_img, 2) int32, cams (n_img, 24) fp32 and images (offsets[-1], 4), uint8 or fp32."""
+    n = pix.numel()
+    rays = torch.empty((n, 12), dtype=torch.float32, device=pix.device)
+    target = torch.empty((n, 3), dtype=torch.float32, device=pix.device)
+    lossmult = torch.empty(n, dtype=torch.float32, device=pix.device)
+    images = table["images"]
+    assert images.dtype in (torch.uint8, torch.float32)
+    lib.call("ngp_mip_rays_multi", _stream(), n, _p(pix), table["wh"].shape[0], _p(table["offsets"]), _p(table["wh"]), _p(table["cams"]), float(focal),
+             int(bool(white_bkgd)), _p(images), int(images.dtype == torch.float32), _p(rays), _p(target), _p(lossmult))
+    return rays, target, lossmult
+
+
+def mip_encode(rays, t, ray_shape="cone", integrate=True, min_deg=0, degs=8):
+    """fp32 (IPE (N, 6 degs), view encoding (N, 27)) of the N = R * S intervals, in the reference's column orders; degs 8 or 16."""
     R, S = t.shape[0], t.shape[1] - 1
-    enc = torch.empty((R * S, 48), dtype=torch.float32, device=t.device)
+    enc = torch.empty((R * S, 6 * degs), dtype=torch.float32, device=t.device)
     view = torch.empty((R * S, 27), dtype=torch.float32, device=t.device)
-    lib.call("ngp_mip_encode", _stream(), R, S, _p(rays), _p(t), RAY_SHAPES.index(ray_shape), int(bool(integrate)), int(min_deg), _p(enc), _p(view))
+    if degs == 8:
+        lib.call("ngp_mip_encode", _stream(), R, S, _p(rays), _p(t), RAY_SHAPES.index(ray_shape), int(bool(integrate)), int(min_deg), _p(enc), _p(view))
+    else:
+        lib.call("ngp_mip_encode_deg", _stream(), R, S, _p(rays), _p(t), RAY_SHAPES.index(ray_shape), int(bool(integrate)), int(min_deg), int(degs),
+                 _p(enc), _p(view))
     return enc, view
 
 
-def mip_fwd(rays, t, params, ray_shape="cone", integrate=True, min_deg=0, out=None, saved=None):
-    """The fused MipNerfMLP forward: (R * S, 4) fp16 {raw rgb, raw density}.  saved: None, or a uint8 buffer of at least
-    nerf_workspace_bytes(R * S)[0] bytes for nerf_bwd."""
+def mip_fwd(rays, t, params, ray_shape="cone", integrate=True, min_deg=0, out=None, saved=None, degs=8):
+    """The fused MipNerfMLP forward at degs (8 or 16) IPE degrees: (R * S, 4) fp16 {raw rgb, raw density}.  saved: None, or a uint8 buffer
+    of at least mip_workspace_bytes(R * S, degs)[0] bytes for mip_bwd (nerf_bwd at 8 degrees)."""
     R, S = t.shape[0], t.shape[1] - 1
     if out is None:
         out = torch.empty((R * S, 4), dtype=torch.float16, device=t.device)
-    lib.call("ngp_mip_fwd", _stream(), R, S, _p(rays), _p(t), RAY_SHAPES.index(ray_shape), int(bool(integrate)), int(min_deg), _p(params), _p(out),
-             _p(saved))
+    if degs == 8:
+        lib.call("ngp_mip_fwd", _stream(), R, S, _p(rays), _p(t), RAY_SHAPES.index(ray_shape), int(bool(integrate)), int(min_deg), _p(params),
+                 _p(out), _p(saved))
+    else:
+        lib.call("ngp_mip_fwd_deg", _stream(), R, S, _p(rays), _p(t), RAY_SHAPES.index(ray_shape), int(bool(integrate)), int(min_deg), int(degs),
+                 _p(params), _p(out), _p(saved))
     return out
+
+
+def mip_param_count(degs=8):
+    b = np.zeros(1, np.uint64)
+    lib.call("ngp_mip_param_count", int(degs), b.ctypes.data)
+    return int(b[0])
+
+
+def mip_workspace_bytes(n, degs=8):
+    """(saved bytes of mip_fwd, scratch bytes of mip_bwd) for n rows at degs IPE degrees; nerf_workspace_bytes at 8."""
+    if degs == 8:
+        return nerf_workspace_bytes(n)
+    b = np.zeros(2, np.uint64)
+    lib.call("ngp_mip_workspace_bytes", int(degs), int(n), b.ctypes.data, b[1:].ctypes.data)
+    return int(b[0]), int(b[1])
+
+
+def mip_bwd(params, saved, dout, degs=8, scratch=None):
+    """The fused MipNerfMLP backward at degs IPE degrees (nerf_bwd at 8): dout (N, 4) fp16 + mip_fwd's saved activations -> the fp32
+    gradient of the flat parameters, deterministic."""
+    if degs == 8:
+        return nerf_bwd(params, saved, dout, scratch=scratch)
+    n = dout.shape[0]
+    need = mip_workspace_bytes(n, degs)[1]
+    if scratch is None:
+        scratch = torch.empty(need, dtype=torch.uint8, device=dout.device)
+    assert scratch.dtype == torch.uint8 and scratch.numel() >= need, "mip_bwd: scratch is smaller than mip_workspace_bytes(N, degs)[1]"
+    grad = torch.empty(params.numel(), dtype=torch.float32, device=dout.device)
+    lib.call("ngp_mip_bwd_deg", _stream(), n, int(degs), _p(params), _p(saved), _p(dout), _p(scratch), _p(grad))
+    return grad
 
 
 def mip_composite_fwd(raw, t, rays, rgb_padding, density_bias, white_bkgd, weights=True):

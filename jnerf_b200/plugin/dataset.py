@@ -440,3 +440,57 @@ class SyntheticNerfDataset(_RayBatcher):
         rgb = (col * lam[:, None]).clamp(0, 1) * alpha[:, None]
         rgba = torch.cat([rgb, alpha[:, None]], -1)
         return (rgba, t_best) if return_t else rgba
+
+
+MULTISCALE_LEVELS = 4                  # full, 1/2, 1/4 and 1/8 resolution, as mip-NeRF's multiscale NeRF-synthetic
+
+
+def synthetic_multicam(split, n_images=100, H=800, W=800, seed=0, camera_angle_x=0.6911112070083618):
+    """The lego stand-in (SyntheticNerfDataset's cameras and images; val and test share the held-out cameras) as a multiscale capture in
+    mip-NeRF's layout: every view at full, 1/2, 1/4 and 1/8 resolution (box filter of the full-resolution RGBA, rounded to uint8), view by
+    view.  Returns (metadata of the split: {file_path, cam2world (3x4), width, height, pix2cam, lossmult, near, far} lists, [RGBA uint8
+    images]).  pix2cam = diag(1, -1, -1) K^-1 (the y and z flips of a NeRF camera), lossmult = the area ratio 4^level."""
+    if H % 8 or W % 8:
+        raise ValueError(f"synthetic_multicam: H and W must be multiples of 8, got {H} x {W}")
+    ds = SyntheticNerfDataset(batch_size=1, mode="train" if split == "train" else "test", n_images=n_images, H=H, W=W, seed=seed,
+                              camera_angle_x=camera_angle_x)
+    f = float(ds._focal[0])
+    meta = {k: [] for k in ("file_path", "cam2world", "width", "height", "pix2cam", "lossmult", "near", "far")}
+    images = []
+    full = ds.image_data.reshape(ds.n_images, H, W, 4).cpu().numpy()
+    for k in range(ds.n_images):
+        for lvl in range(MULTISCALE_LEVELS):
+            s = 2 ** lvl
+            h, w = H // s, W // s
+            im = np.floor(full[k].reshape(h, s, w, s, 4).astype(np.float64).mean((1, 3)) + 0.5).astype(np.uint8)
+            K = np.array([[f / s, 0, 0.5 * w], [0, f / s, 0.5 * h], [0, 0, 1.0]])
+            meta["file_path"].append(f"{split}/r_{k}" + (f"_d{lvl}" if lvl else "") + ".png")
+            meta["cam2world"].append(np.asarray(ds.poses[k], np.float64)[:3, :4].tolist())
+            meta["width"].append(w)
+            meta["height"].append(h)
+            meta["pix2cam"].append((np.diag([1.0, -1.0, -1.0]) @ np.linalg.inv(K)).tolist())
+            meta["lossmult"].append(float(s * s))
+            meta["near"].append(2.0)
+            meta["far"].append(6.0)
+            images.append(im)
+    return meta, images
+
+
+def write_synthetic_multicam(dst, n_images=100, H=800, W=800, seed=0, camera_angle_x=0.6911112070083618):
+    """Writes the multiscale stand-in of synthetic_multicam to dst in mip-NeRF's layout: {split}/r_{k}.png (full resolution) and
+    r_{k}_d{1,2,3}.png, and metadata.json, for train / val / test.  transforms_{split}.json lists the full-resolution views, so Blenders
+    reads the same directory as the single-scale capture."""
+    from PIL import Image
+    all_meta = {}
+    for split in ("train", "val", "test"):
+        meta, images = synthetic_multicam(split, n_images, H, W, seed, camera_angle_x)
+        os.makedirs(os.path.join(dst, split), exist_ok=True)
+        for p, im in zip(meta["file_path"], images):
+            Image.fromarray(im, "RGBA").save(os.path.join(dst, p))
+        all_meta[split] = meta
+        frames = [dict(file_path="./" + p[:-len(".png")], transform_matrix=c + [[0.0, 0.0, 0.0, 1.0]])
+                  for p, c, lm in zip(meta["file_path"], meta["cam2world"], meta["lossmult"]) if lm == 1.0]
+        with open(os.path.join(dst, f"transforms_{split}.json"), "w") as fh:
+            json.dump(dict(camera_angle_x=camera_angle_x, frames=frames), fh)
+    with open(os.path.join(dst, "metadata.json"), "w") as fh:
+        json.dump(all_meta, fh)

@@ -3,7 +3,7 @@ models/samplers/mip_sampler/mip_sampler.py, dataset/nerf_datasets.py:22-235) on 
 section 11.
 
 With using_fp16=True MipNerfMLP is ONE flat fp16 vector in the layout of the vanilla NeRF kernels (plugin/nerf.py), whose forward computes
-the integrated positional encoding on chip (ops.mip_fwd) and whose backward is ops.nerf_bwd.  With using_fp16=False (mip_base.py) it is an
+the integrated positional encoding on chip (ops.mip_fwd) and whose backward is ops.mip_bwd (ops.nerf_bwd at 8 IPE degrees).  With using_fp16=False (mip_base.py) it is an
 fp32 torch.nn.Linear chain under the reference's module names, fed by the fp32 encoder kernel (ops.mip_encode).
 
 Flat layout: the kernel layers of plugin/nerf.py, with the reference's names and column orders mapped as
@@ -32,55 +32,88 @@ N_SAMPLES_MAX = 128
 _VIEW_COLS = [(0, 0, 256), (256, 256, 3)]
 for _k in range(4):
     _VIEW_COLS += [(259 + 3 * _k, 259 + 6 * _k, 3), (271 + 3 * _k, 262 + 6 * _k, 3)]
-REF_LAYERS = {f"layers.{i}.0": ((256, 256), i, 0, [(0, 0, 256)]) for i in (1, 2, 3, 4, 6, 7)}
-REF_LAYERS.update({
-    "layers.0.0": ((256, 48), 0, 0, [(0, 0, 48)]),
-    "layers.5.0": ((256, 304), 5, 0, [(0, 64, 256), (256, 0, 48)]),
-    "density_layer": ((1, 256), 8, 0, [(0, 0, 256)]),
-    "extra_layer": ((256, 256), 8, 16, [(0, 0, 256)]),
-    "view_layers.0.0": ((128, 283), 9, 0, _VIEW_COLS),
-    "color_layer": ((3, 128), 10, 0, [(0, 0, 128)]),
-})
+IPE_DEGS = (8, 16)                     # max_deg_point - min_deg_point of mip_base.py and multicam.py
+
+
+def enc_pad(degs=8):
+    """Kernel columns of the encoding: 6 degs rounded up to whole 8-column groups, at least 64 (csrc/nerf_mlp.cuh: in_pad(0, EG) = 8 EG)."""
+    return max(64, (6 * degs + 7) // 8 * 8)
+
+
+def kernel_in(degs=8):
+    """The padded input widths of the kernel layers at `degs` IPE degrees: layer 0 reads the encoding, layer 5 [encoding, h4]."""
+    e = enc_pad(degs)
+    return (e,) + nerf.IN[1:5] + (256 + e,) + nerf.IN[6:]
+
+
+def ref_layers(degs=8):
+    """The reference-name table at `degs` IPE degrees: layers.0.0 is (256, 6 degs), layers.5.0 (256, 256 + 6 degs) reading [h4, enc],
+    whose h4 columns are kernel columns enc_pad(degs).. and whose enc columns are kernel columns 0.."""
+    w, e = 6 * degs, enc_pad(degs)
+    layers = {f"layers.{i}.0": ((256, 256), i, 0, [(0, 0, 256)]) for i in (1, 2, 3, 4, 6, 7)}
+    layers.update({
+        "layers.0.0": ((256, w), 0, 0, [(0, 0, w)]),
+        "layers.5.0": ((256, 256 + w), 5, 0, [(0, e, 256), (256, 0, w)]),
+        "density_layer": ((1, 256), 8, 0, [(0, 0, 256)]),
+        "extra_layer": ((256, 256), 8, 16, [(0, 0, 256)]),
+        "view_layers.0.0": ((128, 283), 9, 0, _VIEW_COLS),
+        "color_layer": ((3, 128), 10, 0, [(0, 0, 128)]),
+    })
+    return layers
+
+
+REF_LAYERS = ref_layers(8)
 # construction order of the reference's modules (mip_network.py:140-173)
 REF_ORDER = [f"layers.{i}.0" for i in range(8)] + ["density_layer", "extra_layer", "view_layers.0.0", "color_layer"]
 
 
-def pack(ref):
-    return nerf.pack(ref, REF_LAYERS)
+def pack(ref, degs=8):
+    return nerf.pack(ref, ref_layers(degs), kernel_in(degs))
 
 
-def unpack(flat):
-    return nerf.unpack(flat, REF_LAYERS)
+def unpack(flat, degs=None):
+    """The flat vector -> {reference name: (weight, bias)}; degs None: from its length (8 or 16 IPE degrees)."""
+    if degs is None:
+        degs = next(d for d in IPE_DEGS if nerf.w_offsets(kernel_in(d))[-1] == flat.numel())
+    return nerf.unpack(flat, ref_layers(degs), kernel_in(degs))
 
 
 def _encoder_args(cfg):
-    return dict(ray_shape=cfg.ray_shape, integrate=not cfg.disable_integration, min_deg=int(cfg.min_deg_point))
+    args = dict(ray_shape=cfg.ray_shape, integrate=not cfg.disable_integration, min_deg=int(cfg.min_deg_point))
+    degs = int(cfg.max_deg_point) - int(cfg.min_deg_point)
+    if degs != 8:
+        args["degs"] = degs
+    return args
 
 
 @NETWORKS.register_module()
 class MipNerfMLP(Module):
-    """mip_network.py:124-216 for its only configuration (mip_base.py): depth 8, width 256, skip 4, one 128-wide view layer, degrees
-    [min_deg_point, min_deg_point + 8) and deg_view 4.  execute(enc (N, 48), view (N, 27)) -> (N, 4) {raw rgb, raw density}."""
+    """mip_network.py:124-216 for the configurations of mip_base.py and multicam.py: depth 8, width 256, skip 4, one 128-wide view layer,
+    degrees [min_deg_point, min_deg_point + D) with D = 8 or 16, and deg_view 4.  execute(enc (N, 6 D), view (N, 27)) ->
+    (N, 4) {raw rgb, raw density}."""
 
     def __init__(self):
         super().__init__()
         cfg = get_cfg()
         shape = (cfg.net_depth, cfg.net_width, cfg.skip_layer, cfg.net_depth_condition, cfg.net_width_condition, cfg.num_density_channels,
                  cfg.num_rgb_channels, cfg.max_deg_point - cfg.min_deg_point, cfg.deg_view, bool(cfg.use_viewdirs))
-        if shape != (8, 256, 4, 1, 128, 1, 3, 8, 4, True):
-            raise NotImplementedError("MipNerfMLP: the kernels are built for mip_base.py's network: net_depth 8, net_width 256, skip_layer 4, "
-                                      "net_depth_condition 1, net_width_condition 128, 1 density and 3 rgb channels, max_deg_point - "
-                                      "min_deg_point = 8, deg_view 4, use_viewdirs")
+        degs = shape[7]
+        if shape[:7] + shape[8:] != (8, 256, 4, 1, 128, 1, 3, 4, True) or degs not in IPE_DEGS:
+            raise NotImplementedError("MipNerfMLP: the kernels are built for mip_base.py's / multicam.py's network: net_depth 8, net_width 256, "
+                                      "skip_layer 4, net_depth_condition 1, net_width_condition 128, 1 density and 3 rgb channels, "
+                                      "max_deg_point - min_deg_point = 8 or 16, deg_view 4, use_viewdirs")
         self.using_fp16 = bool(cfg.using_fp16)
+        self.degs = degs
         self.enc_args = _encoder_args(cfg)
+        layers = ref_layers(degs)
         gen = torch.Generator(device="cuda").manual_seed(int(cfg.seed or 1) + 1)
-        ref = nerf.init_reference_params(gen, REF_LAYERS, REF_ORDER)
+        ref = nerf.init_reference_params(gen, layers, REF_ORDER)
         if self.using_fp16:
-            self.params = torch.nn.Parameter(pack(ref))
+            self.params = torch.nn.Parameter(pack(ref, degs))
             return
 
         def linear(name):
-            (o, i) = REF_LAYERS[name][0]
+            (o, i) = layers[name][0]
             lin = torch.nn.Linear(i, o).cuda()
             with torch.no_grad():
                 lin.weight.copy_(ref[name][0])
@@ -111,9 +144,9 @@ class MipNerfMLP(Module):
         return self.execute(enc, view)
 
     def reference_params(self):
-        """{reference name: (weight, bias)} in fp32, e.g. layers.5.0 -> ((256, 304), (256,))."""
+        """{reference name: (weight, bias)} in fp32, e.g. layers.5.0 -> ((256, 304), (256,)) at 8 degrees."""
         if self.using_fp16:
-            return unpack(self.params.detach())
+            return unpack(self.params.detach(), self.degs)
         return {name[:-len(".weight")]: (p.detach().float(), self.get_parameter(name[:-len("weight")] + "bias").detach().float())
                 for name, p in self.named_parameters() if name.endswith(".weight")}
 
@@ -188,6 +221,9 @@ class _BlenderRays:
         pix = torch.arange(self.H * self.W, device="cuda", dtype=torch.int32) + int(img_id) * self.H * self.W
         return self.rays_for(pix)
 
+    def image_hw(self, img_id):
+        return self.H, self.W
+
 
 @DATASETS.register_module()
 class Blender(_BlenderRays):
@@ -256,9 +292,171 @@ class SyntheticBlender(_BlenderRays):
         self._finish_init(seed)
 
 
-@DATASETS.register_module()
-class Blenders:
-    """nerf_datasets.py's multi-camera (multiscale) dataset of multicam.py: not supported."""
+# ---- the multiscale datasets of multicam.py (dataset/nerf.py of the reference's contrib/mipnerf) ----------------------------------------
+CAM_FLOATS = 24                       # a table row of ops.mip_rays_multi: pix2cam (3x3), cam2world (3x4), lossmult, near, far
 
-    def __init__(self, *a, **k):
-        raise NotImplementedError("Blenders (the multiscale multicam dataset) is not supported; use Blender")
+
+def cam_row(pix2cam=None, cam2world=None, lossmult=1.0, near=2.0, far=6.0):
+    row = np.zeros(CAM_FLOATS, np.float32)
+    if pix2cam is not None:
+        row[0:9] = np.asarray(pix2cam, np.float32)[:3, :3].reshape(-1)
+    row[9:21] = np.asarray(cam2world, np.float32)[:3, :4].reshape(-1)
+    row[21:24] = (lossmult, near, far)
+    return row
+
+
+class _MultiscaleRays:
+    """The device half of Blenders / Multicam: images of different sizes in one ragged RGBA table (ops.mip_rays_multi), batches of global
+    pixel ids.  Subclasses call _finish_init(images [(H, W, 4) uint8 or fp32], cams (n, 24), focal (0: the table's pix2cam), seed)."""
+    BATCH_TYPES = ("all_images", "single_image")
+
+    def _check_keys(self, name, split, batch_type, legacy):
+        if legacy:
+            raise NotImplementedError(f"{name} takes the keys of the reference's dataset/nerf.py (data_dir, split, batch_size, batch_type, "
+                                      f"white_bkgd{', factor' if name == 'Blenders' else ''}), not Blender's {', '.join(sorted(legacy))}")
+        if split not in ("train", "val", "test"):
+            raise ValueError(f"{name}: split must be train, val or test, got {split!r}")
+        if batch_type not in self.BATCH_TYPES:
+            raise ValueError(f"{name}: batch_type must be one of {self.BATCH_TYPES}, got {batch_type!r}")
+        if split != "train" and batch_type != "single_image":
+            raise ValueError(f"{name}: the {split} split keeps the image shapes: batch_type must be single_image (dataset/nerf.py:68)")
+
+    def _finish_init(self, images, cams, focal, seed):
+        self.n_images = self.n_examples = len(images)
+        self.Hs = [int(im.shape[0]) for im in images]
+        self.Ws = [int(im.shape[1]) for im in images]
+        if min(self.Hs) < 3:
+            raise ValueError(f"{type(self).__name__}: images must be at least 3 rows high (the last row's radius takes row H - 3)")
+        sizes = [h * w for h, w in zip(self.Hs, self.Ws)]
+        self.offsets = [0] + np.cumsum(sizes).tolist()
+        if self.offsets[-1] >= 2 ** 31:
+            raise ValueError(f"{type(self).__name__}: {self.offsets[-1]} pixels; global pixel ids must stay below 2^31")
+        self.focal = float(focal)
+        self.table = dict(offsets=torch.tensor(self.offsets, dtype=torch.int32).to("cuda"),
+                          wh=torch.tensor([[w, h] for h, w in zip(self.Hs, self.Ws)], dtype=torch.int32).reshape(-1, 2).to("cuda"),
+                          cams=torch.from_numpy(np.stack(cams).astype(np.float32)).to("cuda"),
+                          images=torch.from_numpy(np.concatenate([im.reshape(-1, 4) for im in images])).to("cuda"))
+        self.H, self.W = self.Hs[0], self.Ws[0]
+        self.resolution = [self.W, self.H]
+        self.idx_now = 0
+        self._gen = torch.Generator(device="cuda").manual_seed(int(seed))
+        self._host_rng = np.random.default_rng(int(seed))
+        self.shuffle_index = None
+        if self.batch_type == "all_images":
+            self.shuffle_index = torch.randperm(self.offsets[-1], device="cuda", generator=self._gen).int()
+
+    def rays_for(self, pix):
+        """(rays (n, 12), target (n, 3), lossmult (n,)) of global pixel ids."""
+        return ops.mip_rays_multi(pix.contiguous(), self.table, self.focal, self.white_bkgd)
+
+    def __next__(self):
+        """nerf.py:82-105: all_images takes the next batch_size pixels of the shuffled list of every pixel (reshuffled when it runs out);
+        single_image one random image and batch_size of its pixels, drawn with replacement."""
+        if self.batch_type == "all_images":
+            n = self.offsets[-1]
+            if self.idx_now + self.batch_size >= n:
+                self.shuffle_index = torch.randperm(n, device="cuda", generator=self._gen).int()
+                self.idx_now = 0
+            pix = self.shuffle_index[self.idx_now:self.idx_now + self.batch_size]
+            self.idx_now += self.batch_size
+        else:
+            i = int(self._host_rng.integers(self.n_images))
+            pix = torch.randint(0, self.Hs[i] * self.Ws[i], (self.batch_size,), device="cuda", generator=self._gen, dtype=torch.int32)
+            pix = pix + self.offsets[i]
+        return self.rays_for(pix)
+
+    def image_rays(self, img_id):
+        """(rays (H * W, 12), target (H * W, 3)) of image img_id in row-major pixel order."""
+        i = int(img_id)
+        pix = torch.arange(self.Hs[i] * self.Ws[i], device="cuda", dtype=torch.int32) + self.offsets[i]
+        return self.rays_for(pix)[:2]
+
+    def image_hw(self, img_id):
+        return self.Hs[int(img_id)], self.Ws[int(img_id)]
+
+
+def _read_rgba(path):
+    from PIL import Image
+    im = np.asarray(Image.open(path))
+    if im.ndim == 2:
+        im = im[..., None].repeat(3, -1)
+    if im.shape[-1] == 3:
+        im = np.concatenate([im, np.full(im.shape[:2] + (1,), 255, np.uint8)], -1)
+    return np.ascontiguousarray(im)
+
+
+def area_half(im):
+    """The 2x2 area mean of an fp32 (H, W, C) image -> (H // 2, W // 2, C): cv2.resize(..., INTER_AREA) at exactly half size, as
+    ((a + b) + (c + d)) * 0.25 in fp32 (an odd last row or column is dropped)."""
+    h, w = im.shape[0] // 2 * 2, im.shape[1] // 2 * 2
+    a, b, c, d = im[0:h:2, 0:w:2], im[0:h:2, 1:w:2], im[1:h:2, 0:w:2], im[1:h:2, 1:w:2]
+    return ((a + b) + (c + d)) * np.float32(0.25)
+
+
+@DATASETS.register_module()
+class Blenders(_MultiscaleRays):
+    """dataset/nerf.py:25-105 + 207-314: NeRF-synthetic transforms_{split}.json (train: its own frames only; val and test: the first 20),
+    images {file_path}.png as uint8 / 255 composited on white in fp32 when white_bkgd, factor 2 their 2x2 area mean, near 2, far 6,
+    lossmult 1, the camera directions of Blender with focal .5 W / tan(.5 camera_angle_x)."""
+
+    def __init__(self, data_dir=None, split=None, batch_size=4096, batch_type="all_images", white_bkgd=True, factor=0, seed=0, **legacy):
+        self._check_keys("Blenders", split, batch_type, legacy)
+        if factor not in (0, 2):
+            raise ValueError(f"Blender dataset only supports factor=0 or 2, {factor} set.")
+        self.data_dir, self.split, self.batch_size, self.batch_type = data_dir, split, int(batch_size), batch_type
+        self.white_bkgd, self.factor, self.near, self.far = bool(white_bkgd), factor, 2.0, 6.0
+        with open(os.path.join(data_dir, f"transforms_{split}.json")) as fh:
+            meta = json.load(fh)
+        frames = meta["frames"] if split == "train" else meta["frames"][:20]
+        images, cams = [], []
+        for fr in frames:
+            im = _read_rgba(os.path.join(data_dir, fr["file_path"] + ".png"))
+            if factor == 2:
+                im = area_half(im.astype(np.float32) / np.float32(255.0))
+            images.append(im)
+            cams.append(cam_row(cam2world=np.array(fr["transform_matrix"], np.float32)))
+        if len({im.shape for im in images}) > 1:
+            raise ValueError("Blenders: every image of a split must have the same size")
+        w = images[0].shape[1]
+        self._finish_init(images, cams, .5 * w / np.tan(.5 * float(meta["camera_angle_x"])), seed)
+
+
+@DATASETS.register_module()
+class Multicam(_MultiscaleRays):
+    """dataset/nerf.py:108-204: the multiscale NeRF-synthetic layout of metadata.json (per split: file_path, cam2world, width, height,
+    pix2cam, lossmult, near, far; val and test take the first 20 entries).  Rays from the pixel centre through pix2cam and cam2world,
+    lossmult per image (the area ratio to full resolution), images of different sizes."""
+
+    def __init__(self, data_dir=None, split=None, batch_size=4096, batch_type="all_images", white_bkgd=True, seed=0, **legacy):
+        self._check_keys("Multicam", split, batch_type, legacy)
+        self.data_dir, self.split, self.batch_size, self.batch_type = data_dir, split, int(batch_size), batch_type
+        self.white_bkgd = bool(white_bkgd)
+        with open(os.path.join(data_dir, "metadata.json")) as fh:
+            meta = json.load(fh)[split]
+        if split != "train":
+            meta = {k: v[:20] for k, v in meta.items()}
+        images = [_read_rgba(os.path.join(data_dir, p)) for p in meta["file_path"]]
+        for k, im in enumerate(images):
+            if (im.shape[1], im.shape[0]) != (int(meta["width"][k]), int(meta["height"][k])):
+                raise ValueError(f"Multicam: {meta['file_path'][k]} is {im.shape[1]}x{im.shape[0]}, metadata.json says "
+                                 f"{meta['width'][k]}x{meta['height'][k]}")
+        cams = [cam_row(meta["pix2cam"][k], meta["cam2world"][k], meta["lossmult"][k], meta["near"][k], meta["far"][k]) for k in range(len(images))]
+        self._finish_init(images, cams, 0.0, seed)
+
+
+@DATASETS.register_module()
+class SyntheticMulticam(_MultiscaleRays):
+    """Multicam on the procedural stand-in of the lego scene, made in memory (plugin/dataset.py: synthetic_multicam, the images that
+    write_synthetic_multicam puts on disk).  data_dir is not read."""
+
+    def __init__(self, data_dir=None, split=None, batch_size=4096, batch_type="all_images", white_bkgd=True, n_images=100, H=800, W=800,
+                 seed=0, **legacy):
+        from .dataset import synthetic_multicam
+        self._check_keys("SyntheticMulticam", split, batch_type, legacy)
+        self.data_dir, self.split, self.batch_size, self.batch_type = data_dir, split, int(batch_size), batch_type
+        self.white_bkgd = bool(white_bkgd)
+        meta, images = synthetic_multicam(split, n_images=n_images, H=H, W=W, seed=seed)
+        if split != "train":
+            meta, images = {k: v[:20] for k, v in meta.items()}, images[:20]
+        cams = [cam_row(meta["pix2cam"][k], meta["cam2world"][k], meta["lossmult"][k], meta["near"][k], meta["far"][k]) for k in range(len(images))]
+        self._finish_init(images, cams, 0.0, seed)

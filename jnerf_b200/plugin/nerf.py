@@ -44,30 +44,40 @@ REF_LAYERS.update({
 REF_ORDER = [f"pts_linears.{i}" for i in range(8)] + ["views_linears.0", "feature_linear", "alpha_linear", "rgb_linear"]
 
 
-def _kernel_views(flat, name, layers=REF_LAYERS):
+def w_offsets(ins=IN):
+    """Offsets of every kernel layer's weight in the flat vector (and its length last) for the padded input widths `ins`."""
+    off = [0]
+    for o, i in zip(OUT, ins):
+        off.append(off[-1] + o * (i + 1))
+    return off
+
+
+def _kernel_views(flat, name, layers=REF_LAYERS, ins=IN):
     (o, _), l, r0, cols = layers[name]
-    W = flat[W_OFF[l]:W_OFF[l] + OUT[l] * IN[l]].view(OUT[l], IN[l])
-    b = flat[W_OFF[l] + OUT[l] * IN[l]:W_OFF[l + 1]]
+    w_off = W_OFF if ins == IN else w_offsets(ins)
+    W = flat[w_off[l]:w_off[l] + OUT[l] * ins[l]].view(OUT[l], ins[l])
+    b = flat[w_off[l] + OUT[l] * ins[l]:w_off[l + 1]]
     return W[r0:r0 + o], b[r0:r0 + o], cols
 
 
-def pack(ref, layers=REF_LAYERS):
-    """{reference name: (weight (out, in), bias (out,))} -> the flat fp16 vector of the kernels (layers: the name table, e.g. plugin/mip.py's)."""
+def pack(ref, layers=REF_LAYERS, ins=IN):
+    """{reference name: (weight (out, in), bias (out,))} -> the flat fp16 vector of the kernels (layers: the name table, e.g. plugin/mip.py's;
+    ins: the kernel layers' padded input widths, e.g. Mip-NeRF's at 16 IPE degrees)."""
     dev = next(iter(ref.values()))[0].device
-    flat = torch.zeros(N_PARAMS, dtype=torch.float16, device=dev)
+    flat = torch.zeros(w_offsets(ins)[-1], dtype=torch.float16, device=dev)
     for name, (W, b) in ref.items():
-        Wk, bk, cols = _kernel_views(flat, name, layers)
+        Wk, bk, cols = _kernel_views(flat, name, layers, ins)
         for rc, kc, n in cols:
             Wk[:, kc:kc + n] = W[:, rc:rc + n].to(torch.float16)
         bk.copy_(b.to(torch.float16))
     return flat
 
 
-def unpack(flat, layers=REF_LAYERS):
+def unpack(flat, layers=REF_LAYERS, ins=IN):
     """The flat vector (parameters or gradients) -> {reference name: (weight (out, in), bias (out,))} in fp32."""
     out = {}
     for name, ((o, i), _, _, _) in layers.items():
-        Wk, bk, cols = _kernel_views(flat, name, layers)
+        Wk, bk, cols = _kernel_views(flat, name, layers, ins)
         W = torch.empty((o, i), dtype=torch.float32, device=flat.device)
         for rc, kc, n in cols:
             W[:, rc:rc + n] = Wk[:, kc:kc + n].float()

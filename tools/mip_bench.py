@@ -2,9 +2,10 @@
 """Mip-NeRF training step on the H100: the fused MipNerfMLP kernels (ops.mip_fwd + one ops.nerf_bwd over both levels) against the same
 network as fp16 torch.nn.Linear + autograd (cuBLAS), both around the same sampler kernels (mip_sample, mip_resample, mip_composite_fwd,
 mip_composite_loss_bwd) and Adam.  Per step: the time of every stage from CUDA events, and the whole step.  Rays per step: 288 (mip_base.py's
-batch) and 4096; 128 samples a level.  Prints one JSON line with the GPU's name, power limit and SM clock.
+batch) and 4096; 128 samples a level.  --degs 16 times the network at multicam.py's 16 IPE degrees (96 encoding columns; multicam.py's
+batch is --rays 3072).  Prints one JSON line with the GPU's name, power limit and SM clock.
 
-    python tools/mip_bench.py [--steps 50] [--warmup 5] [--rays 288 4096]"""
+    python tools/mip_bench.py [--steps 50] [--warmup 5] [--rays 288 4096] [--degs 8]"""
 import argparse
 import json
 import os
@@ -22,14 +23,14 @@ from jnerf_b200.utils.config import get_cfg, update_cfg  # noqa: E402
 STAGES = ("sample", "fwd_coarse", "composite", "resample", "fwd_fine", "loss_bwd", "net_bwd", "adam")
 
 
-def make(fused, seed=1):
+def make(fused, degs, seed=1):
     get_cfg().clear()
-    update_cfg(**mip_cfg(using_fp16=fused, seed=seed))
+    update_cfg(**mip_cfg(using_fp16=fused, seed=seed, max_deg_point=degs))
     m = mip.MipNerfMLP()
     return m if fused else m.half()
 
 
-def step(m, fused, rays, target, rng, saved, ev):
+def step(m, fused, rays, target, rng, saved, ev, degs):
     S, R = 128, rays.shape[0]
     n = R * S
     cfg = get_cfg()
@@ -40,10 +41,10 @@ def step(m, fused, rays, target, rng, saved, ev):
     if fused:
         raw = torch.empty((2 * n, 4), dtype=torch.float16, device="cuda")
         half = saved.numel() // 2
-        ops.mip_fwd(rays, t_c, m.params, out=raw[:n], saved=saved[:half])
+        ops.mip_fwd(rays, t_c, m.params, out=raw[:n], saved=saved[:half], degs=degs)
         raw_c = raw[:n]
     else:
-        enc, view = ops.mip_encode(rays, t_c)
+        enc, view = ops.mip_encode(rays, t_c, degs=degs)
         raw_c = m.execute(enc.half(), view.half())
     ev[2].record()
     w = ops.mip_composite_fwd(raw_c.detach(), t_c, rays, p, bias, False)[3]
@@ -51,16 +52,16 @@ def step(m, fused, rays, target, rng, saved, ev):
     t_f = ops.mip_resample(t_c, w, 0.01, True, rng)
     ev[4].record()
     if fused:
-        ops.mip_fwd(rays, t_f, m.params, out=raw[n:], saved=saved[half:])
+        ops.mip_fwd(rays, t_f, m.params, out=raw[n:], saved=saved[half:], degs=degs)
     else:
-        enc, view = ops.mip_encode(rays, t_f)
+        enc, view = ops.mip_encode(rays, t_f, degs=degs)
         raw_f = m.execute(enc.half(), view.half())
         raw = torch.cat([raw_c.detach(), raw_f.detach()])
     ev[5].record()
     _, _, draw = ops.mip_composite_loss_bwd(raw, torch.cat([t_c, t_f]), rays, target, None, p, bias, False, 0.1, grad_scale=float(R))
     ev[6].record()
     if fused:
-        grads = [ops.nerf_bwd(m.params, saved, draw)]
+        grads = [ops.mip_bwd(m.params, saved, draw, degs)]
     else:
         torch.autograd.backward([raw_c, raw_f], [draw[:n], draw[n:]])
         grads = [q.grad for q in m.parameters()]
@@ -71,8 +72,8 @@ def step(m, fused, rays, target, rng, saved, ev):
     ev[8].record()
 
 
-def run(fused, R, steps, warmup):
-    m = make(fused)
+def run(fused, R, steps, warmup, degs=8):
+    m = make(fused, degs)
     m._adam = [tuple(torch.zeros(q.numel(), dtype=torch.float32, device="cuda") for _ in range(2)) + (q.detach().float().reshape(-1).clone(),)
                for q in m.parameters()]
     g = torch.Generator(device="cuda").manual_seed(0)
@@ -81,12 +82,12 @@ def run(fused, R, steps, warmup):
     rays = torch.cat([o, d, d, torch.full((R, 1), 1.2e-3, device="cuda"), torch.full((R, 1), 2.0, device="cuda"),
                       torch.full((R, 1), 6.0, device="cuda")], -1).contiguous()
     target = torch.rand((R, 3), device="cuda", generator=g)
-    saved = torch.empty(2 * ops.nerf_workspace_bytes(R * 128)[0], dtype=torch.uint8, device="cuda") if fused else None
+    saved = torch.empty(2 * ops.mip_workspace_bytes(R * 128, degs)[0], dtype=torch.uint8, device="cuda") if fused else None
     rng = ops.pcg32_seed(1)
     ev = [torch.cuda.Event(enable_timing=True) for _ in range(len(STAGES) + 1)]
     acc = dict.fromkeys(STAGES, 0.0)
     for i in range(warmup + steps):
-        step(m, fused, rays, target, rng, saved, ev)
+        step(m, fused, rays, target, rng, saved, ev, degs)
         ops.pcg32_advance(rng, 2 * R * 129)
         torch.cuda.synchronize()
         if i >= warmup:
@@ -101,13 +102,14 @@ def main():
     ap.add_argument("--steps", type=int, default=50)
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--rays", type=int, nargs="+", default=[288, 4096])
+    ap.add_argument("--degs", type=int, default=8, choices=(8, 16))
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("mip_bench.py measures on the GPU: no CUDA device")
     q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm,clocks.sm", "--format=csv,noheader"], capture_output=True, text=True)
-    res = {"gpu": q.stdout.strip().splitlines()[0] if q.returncode == 0 else torch.cuda.get_device_name(), "samples_per_level": 128, "ms": {}}
+    res = {"gpu": q.stdout.strip().splitlines()[0] if q.returncode == 0 else torch.cuda.get_device_name(), "samples_per_level": 128, "ipe_degs": a.degs, "ms": {}}
     for R in a.rays:
-        fused, chain = run(True, R, a.steps, a.warmup), run(False, R, a.steps, a.warmup)
+        fused, chain = run(True, R, a.steps, a.warmup, a.degs), run(False, R, a.steps, a.warmup, a.degs)
         res["ms"][str(R)] = {"fused": fused, "cublas_fp16": chain, "step_speedup": round(chain["step"] / fused["step"], 3),
                              "network_speedup": round((chain["fwd_coarse"] + chain["fwd_fine"] + chain["net_bwd"])
                                                       / (fused["fwd_coarse"] + fused["fwd_fine"] + fused["net_bwd"]), 3)}
