@@ -2,7 +2,8 @@
 
 The kernels keep two per-tile slab buffers: `saved`, every layer's input as the forward stored it, and, in the backward's scratch, `dys`,
 every layer's pre-activation gradient.  Both are blocks of [groups][128 rows][8 halfs] per 128-row tile.  decode() turns them into
-row-major (rows, 8 * groups) matrices whose columns are:
+row-major (rows, 8 * groups) matrices whose columns are, at the 8 encoder groups of NeRF and of Mip-NeRF at 8 IPE degrees (Layout
+gives the saved columns at the 12 groups of Mip-NeRF at 16 degrees, csrc/mip_mlp_wide.cu):
 
     saved (S_GROUPS = 316)       dys (D_GROUPS = 320)
     enc_pos    0 ..   63         dY_l       256 l .. 256 l + 255, l < 8
@@ -29,77 +30,113 @@ import math
 import numpy as np
 import torch
 
-from jnerf_b200.plugin.nerf import IN, N_PARAMS, OUT, W_OFF
+from jnerf_b200.plugin import mip, nerf
+from jnerf_b200.plugin.nerf import OUT
 
 ROWS = 128
 GB = ROWS * 16                     # bytes of one slab group
-S_GROUPS, D_GROUPS = 316, 320
+D_GROUPS = 320
 U = 2.0 ** -23                     # per-step error of an fp32 accumulator that truncates
 FLOOR = 2.0 ** -12                 # the tensor core's alignment floor, relative to the largest operand (module docstring)
-
-ENC, F, DIR, V = 0, 2112, 2368, 2400
-SAVED_COLS, DYS_COLS = 8 * S_GROUPS, 8 * D_GROUPS
-
-
-def H(l):
-    """saved column of h_l, the ReLU output of trunk layer l"""
-    return 64 + 256 * l
+DYS_COLS = 8 * D_GROUPS
 
 
 def DY(l):
-    """dys column of kernel layer l's pre-activation gradient"""
+    """dys column of kernel layer l's pre-activation gradient (the same at every encoder width)"""
     return 256 * l if l < 8 else {8: 2048, 9: 2368, 10: 2496}[l]
 
 
-def in_cols(l):
-    """[(saved column, width)] of kernel layer l's input, concatenated in the weight's column order"""
-    if l == 0:
-        return [(ENC, 64)]
-    if l == 5:
-        return [(ENC, 64), (H(4), 256)]
-    if l == 9:
-        return [(F, 256), (DIR, 32)]
-    if l == 10:
-        return [(V, 128)]
-    return [(H(l - 1), 256)]
+class Layout:
+    """The column map and parameter layout of the kernels at eg 8-column encoder groups (Layout<EG> of nerf_mlp.cuh).  eg 8: vanilla
+    NeRF's 63-column encoding (Mip-NeRF's 48 at 8 IPE degrees uses the same layout); eg 12: Mip-NeRF's 96 columns at 16 IPE degrees,
+    which fill the groups.  The saved block puts the encoding first, so every later saved column moves by 8 (eg - 8):
+
+        saved          eg = 8 (316 groups)    eg = 12 (320 groups)
+        enc_pos        0 .. 63                0 .. 95
+        h_l            64 + 256 l             96 + 256 l
+        f              2112 .. 2367           2144 .. 2399
+        enc_dir        2368 .. 2399           2400 .. 2431
+        v              2400 .. 2527           2432 .. 2559
+
+    The dys block does not depend on eg (module docstring)."""
+
+    def __init__(self, eg):
+        E = 8 * eg
+        self.eg, self.enc_width = eg, {8: 63, 12: 96}[eg]
+        self.ENC, self.F = 0, E + 256 * 8
+        self.DIR = self.F + 256
+        self.V = self.DIR + 32
+        self.S_GROUPS = self.V // 8 + 16
+        self.SAVED_COLS = 8 * self.S_GROUPS
+        self.IN = mip.kernel_in({8: 8, 12: 16}[eg])
+        assert self.IN[0] == E
+        self.W_OFF = nerf.w_offsets(self.IN)
+        self.N_PARAMS = self.W_OFF[-1]
+        # Forward: kernel layer -> [(first weight row, rows, ("saved" | "out", first column), ReLU)]
+        self.FWD = {l: [(0, 256, ("saved", self.H(l)), True)] for l in range(8)}
+        self.FWD[8] = [(0, 1, ("out", 3), False), (16, 256, ("saved", self.F), False)]          # alpha_linear, feature_linear
+        self.FWD[9] = [(0, 128, ("saved", self.V), True)]
+        self.FWD[10] = [(0, 3, ("out", 0), False)]
+        # Dgrad: (kernel layer l, first weight column, columns, saved column of the ReLU mask or None, dys column written), in the
+        # kernel's order.  dY_l (OUT[l] columns at DY(l)) times W_l; layer 9 yields df only (no encoder gradient), layer 5 only its h4
+        # columns, which start at 8 eg.
+        self.DGRAD = [(10, 0, 128, self.V, DY(9)), (9, 0, 256, None, DY(8) + 16), (8, 0, 256, self.H(7), DY(7))] + \
+                     [(l, E if l == 5 else 0, 256, self.H(l - 1), DY(l - 1)) for l in range(7, 0, -1)]
+
+    def H(self, l):
+        """saved column of h_l, the ReLU output of trunk layer l"""
+        return 8 * self.eg + 256 * l
+
+    def in_cols(self, l):
+        """[(saved column, width)] of kernel layer l's input, concatenated in the weight's column order"""
+        E = 8 * self.eg
+        if l == 0:
+            return [(self.ENC, E)]
+        if l == 5:
+            return [(self.ENC, E), (self.H(4), 256)]
+        if l == 9:
+            return [(self.F, 256), (self.DIR, 32)]
+        if l == 10:
+            return [(self.V, 128)]
+        return [(self.H(l - 1), 256)]
 
 
-# Forward: kernel layer -> [(first weight row, rows, ("saved" | "out", first column), ReLU)]
-FWD = {l: [(0, 256, ("saved", H(l)), True)] for l in range(8)}
-FWD[8] = [(0, 1, ("out", 3), False), (16, 256, ("saved", F), False)]          # alpha_linear, feature_linear
-FWD[9] = [(0, 128, ("saved", V), True)]
-FWD[10] = [(0, 3, ("out", 0), False)]
+L8, L12 = Layout(8), Layout(12)
 
-# Dgrad: (kernel layer l, first weight column, columns, saved column of the ReLU mask or None, dys column written), in the kernel's order.
-# dY_l (OUT[l] columns at DY(l)) times W_l; layer 9 yields df only (no encoder gradient), layer 5 only its h4 columns.
-DGRAD = [(10, 0, 128, V, DY(9)), (9, 0, 256, None, DY(8) + 16), (8, 0, 256, H(7), DY(7))] + \
-        [(l, 64 if l == 5 else 0, 256, H(l - 1), DY(l - 1)) for l in range(7, 0, -1)]
+# the 8-group map under its own names (vanilla NeRF, Mip-NeRF at 8 IPE degrees)
+S_GROUPS, SAVED_COLS, N_PARAMS, IN, W_OFF = L8.S_GROUPS, L8.SAVED_COLS, L8.N_PARAMS, L8.IN, L8.W_OFF
+ENC, F, DIR, V = L8.ENC, L8.F, L8.DIR, L8.V
+H, in_cols, FWD, DGRAD = L8.H, L8.in_cols, L8.FWD, L8.DGRAD
+assert (IN, W_OFF, N_PARAMS) == (nerf.IN, nerf.W_OFF, nerf.N_PARAMS)
 
 
-def decode(buf, groups, tiles):
-    """The first `tiles` blocks of a slab buffer (any dtype; uint8 is read as fp16) -> (tiles * 128, 8 * groups) rows."""
+def decode(buf, groups, tiles, t0=0):
+    """Blocks t0 .. tiles - 1 of a slab buffer (any dtype; uint8 is read as fp16) -> ((tiles - t0) * 128, 8 * groups) rows."""
     h = buf.view(torch.float16) if buf.dtype == torch.uint8 else buf
-    return h[:tiles * groups * ROWS * 8].view(tiles, groups, ROWS, 8).permute(0, 2, 1, 3).reshape(tiles * ROWS, groups * 8)
+    nt = tiles - t0
+    return h[t0 * groups * ROWS * 8:tiles * groups * ROWS * 8].view(nt, groups, ROWS, 8).permute(0, 2, 1, 3).reshape(nt * ROWS, groups * 8)
 
 
-def layer_params(P, l):
+def layer_params(P, l, lay=L8):
     """(W (OUT[l], IN[l]), b (OUT[l])) of kernel layer l of the flat vector, float64"""
-    W = P[W_OFF[l]:W_OFF[l] + OUT[l] * IN[l]].view(OUT[l], IN[l]).double()
-    return W, P[W_OFF[l] + OUT[l] * IN[l]:W_OFF[l + 1]].double()
+    o, i = lay.W_OFF[l], lay.IN[l]
+    W = P[o:o + OUT[l] * i].view(OUT[l], i).double()
+    return W, P[o + OUT[l] * i:lay.W_OFF[l + 1]].double()
 
 
-def layer_input(sv, l):
-    return torch.cat([sv[:, c:c + w] for c, w in in_cols(l)], 1)
+def layer_input(sv, l, lay=L8):
+    return torch.cat([sv[:, c:c + w] for c, w in lay.in_cols(l)], 1)
 
 
-def pad_mask(device="cpu"):
+def pad_mask(device="cpu", lay=L8):
     """True at the entries of the flat vector that no reference parameter maps to: they must receive exactly zero gradient"""
-    m = torch.ones(N_PARAMS, dtype=torch.bool, device=device)
+    m = torch.ones(lay.N_PARAMS, dtype=torch.bool, device=device)
+    E, w = 8 * lay.eg, lay.enc_width
     for l in range(11):
-        W = m[W_OFF[l]:W_OFF[l] + OUT[l] * IN[l]].view(OUT[l], IN[l])
-        b = m[W_OFF[l] + OUT[l] * IN[l]:W_OFF[l + 1]]
+        W = m[lay.W_OFF[l]:lay.W_OFF[l] + OUT[l] * lay.IN[l]].view(OUT[l], lay.IN[l])
+        b = m[lay.W_OFF[l] + OUT[l] * lay.IN[l]:lay.W_OFF[l + 1]]
         rows = {8: [0] + list(range(16, 272)), 10: [0, 1, 2]}.get(l, range(OUT[l]))
-        cols = {0: range(63), 5: [c for c in range(320) if c != 63], 9: range(283)}.get(l, range(IN[l]))
+        cols = {0: range(w), 5: [c for c in range(E + 256) if c < w or c >= E], 9: range(283)}.get(l, range(lay.IN[l]))
         W[torch.tensor(list(rows))[:, None], torch.tensor(list(cols))[None, :]] = False
         b[list(rows)] = False
     return m
@@ -124,44 +161,44 @@ def dgrad_layer(dy, W):
     return dy @ W, (W.shape[0] + 2) * U * (dy.abs() @ W.abs() + _floor(dy.abs().amax(1), W.abs().amax(0)))
 
 
-def wgrad_flat(dys, sv):
+def wgrad_flat(dys, sv, lay=L8):
     """The flat gradient sum_rows dY_l^T X_l (weights) and sum_rows dY_l (biases) of decoded rows, the same sums of magnitudes, and the
     floor F of every weight entry (0 for the biases, which are plain fp32 sums).  Over several row blocks g and a add up, F is the
     largest."""
-    g = torch.zeros(N_PARAMS, dtype=torch.float64, device=dys.device)
+    g = torch.zeros(lay.N_PARAMS, dtype=torch.float64, device=dys.device)
     a, f = torch.zeros_like(g), torch.zeros_like(g)
     for l in range(11):
-        dy, x = dys[:, DY(l):DY(l) + OUT[l]].double(), layer_input(sv, l).double()
-        w0, b0 = W_OFF[l], W_OFF[l] + OUT[l] * IN[l]
+        dy, x = dys[:, DY(l):DY(l) + OUT[l]].double(), layer_input(sv, l, lay).double()
+        w0, b0 = lay.W_OFF[l], lay.W_OFF[l] + OUT[l] * lay.IN[l]
         g[w0:b0], a[w0:b0] = (dy.T @ x).reshape(-1), (dy.abs().T @ x.abs()).reshape(-1)
         if dy.shape[0]:
             f[w0:b0] = _floor(dy.abs().amax(0), x.abs().amax(0)).reshape(-1)
-        g[b0:W_OFF[l + 1]], a[b0:W_OFF[l + 1]] = dy.sum(0), dy.abs().sum(0)
+        g[b0:lay.W_OFF[l + 1]], a[b0:lay.W_OFF[l + 1]] = dy.sum(0), dy.abs().sum(0)
     return g, a, f
 
 
-def forward_chain(P, enc_pos, enc_dir, rnd=lambda t: t):
-    """The whole network from encodings (rows, 64) and (rows, 32) through FWD: (saved (rows, 2528), out (rows, 4)), float64.  rnd is
-    applied wherever the kernel stores a value (identity: the exact network)."""
-    n = enc_pos.shape[0]
-    sv = torch.zeros((n, SAVED_COLS), dtype=torch.float64, device=enc_pos.device)
+def forward_chain(P, enc_pos, enc_dir, rnd=lambda t: t, lay=L8):
+    """The whole network from encodings (rows, 8 eg) and (rows, 32) through FWD: (saved (rows, SAVED_COLS), out (rows, 4)), float64.
+    rnd is applied wherever the kernel stores a value (identity: the exact network)."""
+    n, E = enc_pos.shape[0], 8 * lay.eg
+    sv = torch.zeros((n, lay.SAVED_COLS), dtype=torch.float64, device=enc_pos.device)
     out = torch.zeros((n, 4), dtype=torch.float64, device=enc_pos.device)
-    sv[:, ENC:ENC + 64], sv[:, DIR:DIR + 32] = enc_pos.double(), enc_dir.double()
+    sv[:, lay.ENC:lay.ENC + E], sv[:, lay.DIR:lay.DIR + 32] = enc_pos.double(), enc_dir.double()
     for l in range(11):
-        W, b = layer_params(P, l)
-        x = layer_input(sv, l)
-        for r0, nr, (dst, c), relu in FWD[l]:
+        W, b = layer_params(P, l, lay)
+        x = layer_input(sv, l, lay)
+        for r0, nr, (dst, c), relu in lay.FWD[l]:
             y = fwd_layer(x, W[r0:r0 + nr], b[r0:r0 + nr])[0]
             (sv if dst == "saved" else out)[:, c:c + nr] = rnd(y.clamp_min(0) if relu else y)
     return sv, out
 
 
-def backward_chain(P, sv, dout, rnd=lambda t: t):
+def backward_chain(P, sv, dout, rnd=lambda t: t, lay=L8):
     """dys (rows, 2560) of the dgrad chain through DGRAD from dout (rows, 4), float64, masks read from sv"""
     dys = torch.zeros((sv.shape[0], DYS_COLS), dtype=torch.float64, device=sv.device)
     dys[:, DY(10):DY(10) + 3], dys[:, DY(8)] = dout[:, :3].double(), dout[:, 3].double()
-    for l, c0, nc, mask, dst in DGRAD:
-        W = layer_params(P, l)[0]
+    for l, c0, nc, mask, dst in lay.DGRAD:
+        W = layer_params(P, l, lay)[0]
         y = dgrad_layer(dys[:, DY(l):DY(l) + OUT[l]], W[:, c0:c0 + nc])[0]
         if mask is not None:
             y = y * (sv[:, mask:mask + nc] > 0)
@@ -221,6 +258,42 @@ def freq_encoding(x, L):
     w = 3 + 6 * L
     pad = torch.zeros((x.shape[0], (w + 7) // 8 * 8 - w), dtype=torch.float64, device=x.device)
     return torch.cat(ys + [pad], 1), torch.cat(es + [pad], 1)
+
+
+def gaussian64(rays, t, ray_shape, integrate):
+    """Mip-NeRF's conical (or cylindrical) frustum Gaussians of rays (R, 12) and fenceposts t (R, S + 1) in float64: mean, variance and
+    the magnitude |d t_mean| + |o| the fp32 mean is rounded against, (R S, 3) each."""
+    rays, t = rays.double(), t.double()
+    d, o, r = rays[:, None, 3:6], rays[:, None, 0:3], rays[:, 9:10]
+    t0, t1 = t[:, :-1], t[:, 1:]
+    if ray_shape == "cone":
+        mu, hw = (t0 + t1) / 2, (t1 - t0) / 2
+        t_mean = mu + (2 * mu * hw ** 2) / (3 * mu ** 2 + hw ** 2)
+        t_var = hw ** 2 / 3 - (4 / 15) * ((hw ** 4 * (12 * mu ** 2 - hw ** 2)) / (3 * mu ** 2 + hw ** 2) ** 2)
+        r_var = r ** 2 * (mu ** 2 / 4 + (5 / 12) * hw ** 2 - 4 / 15 * hw ** 4 / (3 * mu ** 2 + hw ** 2))
+    else:
+        t_mean, r_var, t_var = (t0 + t1) / 2, (r ** 2 / 4).expand_as(t0), (t1 - t0) ** 2 / 12
+    mean = d * t_mean[..., None] + o
+    d2 = d ** 2
+    var = t_var[..., None] * d2 + r_var[..., None] * (1 - d2 / d2.sum(-1, keepdim=True).clamp_min(1e-10))
+    if not integrate:
+        var = torch.zeros_like(var)
+    return mean.reshape(-1, 3), var.reshape(-1, 3), (d.abs() * t_mean[..., None].abs() + o.abs()).reshape(-1, 3)
+
+
+def ipe64(rays, t, ray_shape="cone", integrate=True, degs=16):
+    """The integrated positional encoding in float64, (R S, 6 degs) [sin | cos], degree-major, xyz inner, and the bound of an fp32
+    evaluation (mip::ipe).  Column (k, dim): sin / cos(mean 2^k) e^(-var 4^k / 2).  The fp32 mean carries the rounding of mip::gaussian,
+    a few ulps of |d t_mean| + |o|, amplified by 2^k; bound: 16 such ulps times 2^k times the attenuation, + 16 ulps of the variance
+    term's relative error on the attenuation, + 4 ulps for sincosf / expf and the products."""
+    mean, var, mag = gaussian64(rays, t, ray_shape, integrate)
+    k = torch.arange(degs, device=mean.device, dtype=torch.float64)
+    y = (mean[:, None, :] * 2 ** k[None, :, None]).reshape(-1, 3 * degs)
+    vv = (var[:, None, :] * 4 ** k[None, :, None]).reshape(-1, 3 * degs)
+    att = torch.exp(-0.5 * vv)
+    amp = (mag[:, None, :] * 2 ** k[None, :, None]).reshape(-1, 3 * degs)
+    bound = 16 * U * (amp + vv) * att + 4 * U
+    return torch.cat([torch.sin(y) * att, torch.cos(y) * att], -1), torch.cat([bound, bound], -1)
 
 
 def numpy_rn16(y):

@@ -10,6 +10,7 @@ import torch
 
 import mip_cpu_backend as ref
 import multicam_cpu_backend as mref
+import nerf_mlp_ref
 from test_mip_gpu import FWD_TOL
 
 pytestmark = pytest.mark.gpu
@@ -60,46 +61,16 @@ def _rays(R, seed=0):
                       torch.full((R, 1), 6.0, device="cuda")], -1).contiguous()
 
 
-def _gaussian64(rays, t, ray_shape, integrate):
-    """fp64 mean, variance and the magnitude |d t_mean| + |o| the fp32 mean is rounded against, (N, 3) each."""
-    rays, t = rays.double(), t.double()
-    d, o, r = rays[:, None, 3:6], rays[:, None, 0:3], rays[:, 9:10]
-    t0, t1 = t[:, :-1], t[:, 1:]
-    if ray_shape == "cone":
-        mu, hw = (t0 + t1) / 2, (t1 - t0) / 2
-        t_mean = mu + (2 * mu * hw ** 2) / (3 * mu ** 2 + hw ** 2)
-        t_var = hw ** 2 / 3 - (4 / 15) * ((hw ** 4 * (12 * mu ** 2 - hw ** 2)) / (3 * mu ** 2 + hw ** 2) ** 2)
-        r_var = r ** 2 * (mu ** 2 / 4 + (5 / 12) * hw ** 2 - 4 / 15 * hw ** 4 / (3 * mu ** 2 + hw ** 2))
-    else:
-        t_mean, r_var, t_var = (t0 + t1) / 2, (r ** 2 / 4).expand_as(t0), (t1 - t0) ** 2 / 12
-    mean = d * t_mean[..., None] + o
-    d2 = d ** 2
-    var = t_var[..., None] * d2 + r_var[..., None] * (1 - d2 / d2.sum(-1, keepdim=True).clamp_min(1e-10))
-    if not integrate:
-        var = torch.zeros_like(var)
-    return mean.reshape(-1, 3), var.reshape(-1, 3), (d.abs() * t_mean[..., None].abs() + o.abs()).reshape(-1, 3)
-
-
 @pytest.mark.parametrize("ray_shape,integrate", [("cone", True), ("cylinder", True), ("cone", False)])
 def test_16_degree_encoder_against_fp64_per_degree(ray_shape, integrate):
-    """Column (k, dim) of degree k: sin / cos(mean 2^k) e^(-var 4^k / 2).  The fp32 mean carries the rounding of mip::gaussian, a few ulps
-    of |d t_mean| + |o|, amplified by 2^k; bound: 16 such ulps times 2^k times the attenuation, + 16 ulps of the variance term's relative
-    error on the attenuation, + 4 ulps for sincosf / expf and the products."""
+    """Column (k, dim) of degree k against float64, within the per-degree bound of tests/nerf_mlp_ref.py: ipe64."""
     from jnerf_b200 import ops
     R, S = 61, 128
     rays = _rays(R, seed=3)
     t = ops.mip_sample(rays, S, False, True, ops.pcg32_seed(7))
     enc, view = ops.mip_encode(rays, t, ray_shape, integrate, 0, degs=16)
     assert enc.shape == (R * S, 96)
-    mean, var, mag = _gaussian64(rays, t, ray_shape, integrate)
-    k = torch.arange(16, device="cuda", dtype=torch.float64)
-    y = (mean[:, None, :] * 2 ** k[None, :, None]).reshape(-1, 48)
-    vv = (var[:, None, :] * 4 ** k[None, :, None]).reshape(-1, 48)
-    att = torch.exp(-0.5 * vv)
-    want = torch.cat([torch.sin(y) * att, torch.cos(y) * att], -1)
-    amp = (mag[:, None, :] * 2 ** k[None, :, None]).reshape(-1, 48)
-    bound = 16 * EPS * (amp + vv) * att + 4 * EPS
-    bound = torch.cat([bound, bound], -1)
+    want, bound = nerf_mlp_ref.ipe64(rays, t, ray_shape, integrate, 16)
     ratio = ((enc.double() - want).abs() / bound).reshape(-1, 2, 16, 3).amax((0, 1, 3))
     print(f"{ray_shape} integrate={integrate}: worst error / bound per degree", [round(float(x), 3) for x in ratio])
     assert float(ratio.max()) <= 1.0

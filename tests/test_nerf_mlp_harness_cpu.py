@@ -150,3 +150,90 @@ def test_freq_encoding_matches_plugin_encoder():
     assert y.shape == (50, 64) and not y[:, 63].any() and not e[:, 63].any() and not e[:, :3].any()
     assert torch.allclose(y[:, :63].float(), nerf.freq_encode(x, 10), atol=2e-6)
     assert bool((e[:, 3:63] > 0).all()) and float((e / y.abs().clamp_min(1e-30))[:, 3:63].max()) <= 2 * 2.0 ** -23
+
+
+# ---------------------------------------------------------------------------------------------------------------- 12 encoder groups
+def _layout_decl(eg):
+    """The saved-group bases of Layout<EG> (nerf_mlp.cuh) evaluated at eg, and the values its static_assert states at 12 groups"""
+    src = open(os.path.join(ROOT, "jnerf_b200", "csrc", "nerf_mlp.cuh")).read()
+    body = re.search(r"struct Layout \{(.*?)\n\};", src, re.S).group(1)
+    env = {"EG": eg}
+    for item in re.search(r"static constexpr uint32_t (S_H = EG,[^;]*);", body).group(1).split(","):
+        k, v = item.split("=")
+        env[k.strip()] = eval(v, {}, dict(env))
+    return env, {k: int(v) for k, v in re.findall(r"Layout<12>::(\w+) == (\d+)", src)}
+
+
+def test_12_group_column_map_is_layout_12():
+    c8, _ = _layout_decl(8)
+    assert (8 * c8["S_H"], 8 * c8["S_F"], 8 * c8["S_DIR"], 8 * c8["S_V"], c8["S_GROUPS"]) == (R.H(0), R.F, R.DIR, R.V, R.S_GROUPS)
+    c, asserted = _layout_decl(12)
+    L = R.L12
+    assert (8 * c["S_F"], 8 * c["S_DIR"], 8 * c["S_V"], c["S_GROUPS"]) == (L.F, L.DIR, L.V, L.S_GROUPS)
+    assert all(8 * (c["S_H"] + 32 * l) == L.H(l) for l in range(8))
+    assert asserted["S_GROUPS"] == L.S_GROUPS == 320 and 8 * asserted["S_V"] == L.V == 2432
+    assert asserted["N_PARAMS"] == L.N_PARAMS == 618912
+    from jnerf_b200.plugin import mip
+    assert L.IN == mip.kernel_in(16) and L.IN[0] == 96 and L.IN[5] == 352
+    assert L.in_cols(0) == [(0, 96)] and L.in_cols(5) == [(0, 96), (96 + 256 * 4, 256)]
+    assert [d for d in L.DGRAD if d[0] == 5] == [(5, 96, 256, L.H(4), R.DY(4))]
+    assert R.L8.S_GROUPS == 316 and R.L8.N_PARAMS == R.N_PARAMS
+
+
+def test_decoder_takes_a_tile_range():
+    groups, tiles = R.L12.S_GROUPS, 5
+    h = torch.arange(tiles * groups * R.ROWS * 8, dtype=torch.float64)
+    whole = R.decode(h, groups, tiles)
+    assert torch.equal(R.decode(h, groups, 4, 2), whole[2 * R.ROWS:4 * R.ROWS])
+    assert R.decode(h, groups, 3, 3).shape == (0, 8 * groups)
+
+
+def test_pad_mask_at_12_groups_is_what_pack_leaves_zero():
+    from jnerf_b200.plugin import mip
+    ones = {name: (torch.ones(shape), torch.ones(shape[0])) for name, (shape, _, _, _) in mip.ref_layers(16).items()}
+    pad = R.pad_mask(lay=R.L12)
+    assert torch.equal(pad, mip.pack(ones, 16) == 0)
+    # at 16 degrees the encoding fills layer 0 and layer 5: only the padded rows of layers 8 and 10 and columns 283.. of layer 9 remain
+    assert int(pad.sum()) == 15 * 257 + 13 * 129 + 5 * 128
+
+
+def test_layer_tables_at_12_groups_compose_to_the_16_degree_reference_network():
+    """FWD / DGRAD / wgrad_flat at 12 groups composed over the flat vector against plugin/mip.py's named chain at 16 IPE degrees (the
+    reference's column orders: layers.5.0 reads [h4, enc], view_layers.0.0 reads [bottleneck, x, sin, cos]), float64 on both sides."""
+    from jnerf_b200.plugin import mip
+    g = torch.Generator().manual_seed(3)
+    ref = {name: ((torch.rand((o, i), generator=g) * 2 - 1) * math.sqrt(3 / i) * 1.5, (torch.rand(o, generator=g) * 2 - 1) * 0.3)
+           for name, ((o, i), _, _, _) in mip.ref_layers(16).items()}
+    P = mip.pack(ref, 16)
+    leaves = {k: (W.double().requires_grad_(), b.double().requires_grad_()) for k, (W, b) in mip.unpack(P, 16).items()}
+    n = 300
+    enc = torch.rand((n, 96), generator=g, dtype=torch.float64) * 2 - 1
+    encd = torch.zeros((n, 32), dtype=torch.float64)
+    encd[:, :27] = torch.rand((n, 27), generator=g, dtype=torch.float64) * 2 - 1
+    view = torch.zeros((n, 27), dtype=torch.float64)                     # the kernel's FrequencyEncoder(4) order -> the reference's
+    for rc, kc, w in mip._VIEW_COLS[1:]:
+        view[:, rc - 256:rc - 256 + w] = encd[:, kc - 256:kc - 256 + w]
+    dout = torch.randn((n, 4), generator=g, dtype=torch.float64)
+    lin = lambda name, x: x @ leaves[name][0].t() + leaves[name][1]
+    h = enc
+    for i in range(8):
+        h = torch.relu(lin(f"layers.{i}.0", h))
+        if i == 4:
+            h = torch.cat([h, enc], -1)
+    v = torch.relu(lin("view_layers.0.0", torch.cat([lin("extra_layer", h), view], -1)))
+    want = torch.cat([lin("color_layer", v), lin("density_layer", h)], -1)
+    (want * dout).sum().backward()
+
+    L = R.L12
+    sv, out = R.forward_chain(P, enc, encd, lay=L)
+    assert torch.allclose(out, want.detach(), rtol=1e-12, atol=1e-12)
+    assert torch.allclose(sv[:, L.V:L.V + 128], v.detach(), rtol=1e-12, atol=1e-12)
+    dys = R.backward_chain(P, sv, dout, lay=L)
+    grad, mag, _ = R.wgrad_flat(dys, sv, lay=L)
+    pad = R.pad_mask(lay=L)
+    assert torch.equal(grad[pad], torch.zeros_like(grad[pad])) and bool((mag[~pad] > 0).any())
+    got = mip.unpack(grad, 16)
+    for name, (W, b) in leaves.items():
+        assert torch.allclose(got[name][0].double(), W.grad, rtol=1e-6, atol=1e-9), name
+        assert torch.allclose(got[name][1].double(), b.grad, rtol=1e-6, atol=1e-9), name
+    assert not dys[:, R.DY(8) + 1:R.DY(8) + 16].any() and not dys[:, R.DY(8) + 272:R.DY(9)].any() and not dys[:, R.DY(10) + 3:].any()
