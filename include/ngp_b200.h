@@ -197,6 +197,32 @@ int ngp_mip_bwd_deg(void* stream, uint32_t n_max, int degs, const void* params, 
 int ngp_mip_encode_deg(void* stream, uint32_t n_rays, uint32_t n_samples, const float* rays, const float* t, int ray_shape, int integrate,
                        int min_deg, int degs, float* enc_out, float* view_out);
 
+/* ---- N1-N5  pixelNeRF (contrib/pixelnerf of the reference), csrc/pixelnerf.cu, DESIGN.md section 13 -----------------------------------------
+ * rays (n_rays, 6) fp32 origin then direction (not normalised); z (n_samples) the sample depths shared by every ray (Render.py:22-26).
+ * params: ngp_pixelnerf_param_count fp16 values in the layout of plugin/pixelnerf.py (mlp.0 padded to 64 input columns).
+ * feats (n_ref, feat_h, feat_w, 512) fp16 channel-last; cams (n_ref, 12) fp32: R_t = c2w[:3,:3]^T row-major, then the camera position;
+ * scale = (H / 2) / focal.  raw (n_rays n_samples, 4) fp16: relu(o0), sigmoid(o1:4). */
+int ngp_pixelnerf_param_count(uint64_t* count_out);
+/* N1: buffer sizes for n_rows = n_rays n_samples sample rows: saved (training forward), infer (forward with saved NULL), bwd (backward scratch). */
+int ngp_pixelnerf_workspace_bytes(uint32_t n_ref, uint32_t n_rows, uint64_t* saved_bytes, uint64_t* infer_bytes, uint64_t* bwd_bytes);
+/* N2: Render.py:10-15 + Dataset.py:86-94 + Network.py:66-94: projection, feature gather, network.  saved non-NULL: the training forward,
+ * keeping what ngp_pixelnerf_bwd reads; saved NULL: inference, temporaries in scratch.  raw is the same bit for bit either way.
+ * pixel_aligned = 0 is the reference's projection (uv = p.xy / p.z / scale, v negated), 1 the pinhole one (both negated, then v). */
+int ngp_pixelnerf_fwd(void* stream, uint32_t n_rays, uint32_t n_samples, const float* rays, const float* z, const void* params, const void* feats,
+                      uint32_t n_ref, uint32_t feat_h, uint32_t feat_w, const float* cams, float scale, int pixel_aligned, void* raw_out, void* saved,
+                      void* scratch);
+/* N3: the backward of N2 from draw (like raw) into grad (param_count fp32, overwritten), deterministic.  Replaces main.py:46's
+ * optimizer.step(loss) gradient. */
+int ngp_pixelnerf_bwd(void* stream, uint32_t n_rays, uint32_t n_samples, uint32_t n_ref, const void* params, const void* feats, const void* saved,
+                      const void* raw, const void* draw, void* scratch, float* grad);
+/* N4: Render.py:16-18 + :34-46: rgb (n_rays, 3), depth, acc (n_rays, may be NULL); n_samples <= 64. */
+int ngp_pixelnerf_composite_fwd(void* stream, uint32_t n_rays, uint32_t n_samples, const void* raw, const float* z, const float* rays, float* rgb_out,
+                                float* depth_out, float* acc_out);
+/* N5: N4, main.py:45's MSE over the 3 n_rays colour entries (loss_out: per-ray terms that sum to it) and draw_out = grad_scale dloss / draw
+ * in fp16, saturated to +-65504. */
+int ngp_pixelnerf_composite_loss_bwd(void* stream, uint32_t n_rays, uint32_t n_samples, const void* raw, const float* z, const float* rays,
+                                     const float* target, float grad_scale, float* rgb_out, float* loss_out, void* draw_out);
+
 /* ---- X1-X9  Plenoxels (contrib/plenoxel of the reference: models/networks/svox2_network.py, ops/svox_ops/op/op_header/*.h),
  * csrc/svox.cu, DESIGN.md section 12 ----------------------------------------------------------------------------------------------
  * A grid is links (X, Y, Z) int32 row-major (< 0: empty), density (capacity) and sh (capacity, 27) fp32, SH degree 2 channel-major.

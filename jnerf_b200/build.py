@@ -22,6 +22,7 @@ SOURCES = {
     "mip_sampler.cu": ["-fmad=false"],
     "mip_multiscale.cu": ["-fmad=false"],
     "svox.cu": [],
+    "pixelnerf.cu": [],
     "sampler.cu": ["-fmad=false"],
     "grid_update.cu": ["-fmad=false"],
     "mesh.cu": ["-fmad=false"],

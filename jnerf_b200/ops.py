@@ -317,6 +317,73 @@ def mip_composite_loss_bwd(raw, t, rays, target, mask, rgb_padding, density_bias
     return rgb, loss, draw
 
 
+# ---- pixelNeRF (include/ngp_b200.h N1-N5; contrib/pixelnerf of the reference) ----
+def pixelnerf_param_count():
+    b = np.zeros(1, np.uint64)
+    lib.call("ngp_pixelnerf_param_count", b.ctypes.data)
+    return int(b[0])
+
+
+def pixelnerf_workspace_bytes(n_rows, n_ref):
+    """(saved bytes of the training forward, scratch bytes of the inference forward, scratch bytes of the backward) for n_rows sample rows."""
+    b = np.zeros(3, np.uint64)
+    lib.call("ngp_pixelnerf_workspace_bytes", int(n_ref), int(n_rows), b.ctypes.data, b[1:].ctypes.data, b[2:].ctypes.data)
+    return int(b[0]), int(b[1]), int(b[2])
+
+
+def pixelnerf_fwd(rays, z, params, feats, cams, scale, pixel_aligned=False, saved=None, scratch=None, out=None):
+    """The pixelNeRF network on rays (R, 6) x z (S,) -> raw (R S, 4) fp16.  feats (n_ref, fh, fw, 512) fp16, cams (n_ref, 12).  saved: a uint8
+    buffer of pixelnerf_workspace_bytes(R S, n_ref)[0] for the training forward; None: inference (scratch of [1] bytes, allocated if None)."""
+    R, S = rays.shape[0], z.shape[0]
+    n_ref, fh, fw = feats.shape[:3]
+    need = pixelnerf_workspace_bytes(R * S, n_ref)
+    if saved is not None:
+        assert saved.dtype == torch.uint8 and saved.numel() >= need[0], "pixelnerf_fwd: saved is smaller than pixelnerf_workspace_bytes(...)[0]"
+    elif scratch is None:
+        scratch = torch.empty(need[1], dtype=torch.uint8, device=rays.device)
+    else:
+        assert scratch.dtype == torch.uint8 and scratch.numel() >= need[1], "pixelnerf_fwd: scratch is smaller than pixelnerf_workspace_bytes(...)[1]"
+    out = torch.empty((R * S, 4), dtype=torch.float16, device=rays.device) if out is None else out
+    lib.call("ngp_pixelnerf_fwd", _stream(), R, S, _p(rays), _p(z), _p(params), _p(feats), n_ref, fh, fw, _p(cams), float(scale),
+             int(bool(pixel_aligned)), _p(out), _p(saved), None if saved is not None else _p(scratch))
+    return out
+
+
+def pixelnerf_bwd(rays_count, n_samples, params, feats, saved, raw, draw, scratch=None):
+    """The backward of pixelnerf_fwd's training forward: draw (R S, 4) fp16 -> the fp32 gradient of the flat parameters, deterministic."""
+    n_ref = feats.shape[0]
+    need = pixelnerf_workspace_bytes(rays_count * n_samples, n_ref)[2]
+    if scratch is None:
+        scratch = torch.empty(need, dtype=torch.uint8, device=draw.device)
+    assert scratch.dtype == torch.uint8 and scratch.numel() >= need, "pixelnerf_bwd: scratch is smaller than pixelnerf_workspace_bytes(...)[2]"
+    grad = torch.empty(params.numel(), dtype=torch.float32, device=draw.device)
+    lib.call("ngp_pixelnerf_bwd", _stream(), int(rays_count), int(n_samples), n_ref, _p(params), _p(feats), _p(saved), _p(raw), _p(draw), _p(scratch),
+             _p(grad))
+    return grad
+
+
+def pixelnerf_composite_fwd(raw, z, rays):
+    """(rgb (R, 3), depth (R,), acc (R,))."""
+    R, S = rays.shape[0], z.shape[0]
+    dev = rays.device
+    rgb = torch.empty((R, 3), dtype=torch.float32, device=dev)
+    depth = torch.empty(R, dtype=torch.float32, device=dev)
+    acc = torch.empty(R, dtype=torch.float32, device=dev)
+    lib.call("ngp_pixelnerf_composite_fwd", _stream(), R, S, _p(raw), _p(z), _p(rays), _p(rgb), _p(depth), _p(acc))
+    return rgb, depth, acc
+
+
+def pixelnerf_composite_loss_bwd(raw, z, rays, target, grad_scale=1.0):
+    """(rgb (R, 3), per-ray loss terms (R,) summing to the MSE, grad_scale * dloss/draw (R S, 4) fp16)."""
+    R, S = rays.shape[0], z.shape[0]
+    dev = rays.device
+    rgb = torch.empty((R, 3), dtype=torch.float32, device=dev)
+    loss = torch.empty(R, dtype=torch.float32, device=dev)
+    draw = torch.empty_like(raw)
+    lib.call("ngp_pixelnerf_composite_loss_bwd", _stream(), R, S, _p(raw), _p(z), _p(rays), _p(target), float(grad_scale), _p(rgb), _p(loss), _p(draw))
+    return rgb, loss, draw
+
+
 # ---- mesh extraction (include/ngp_b200.h M1-M6; tools/extract_mesh.py of the reference) ----
 def _mesh_workspace(device, n=0, n_verts=0, n_tris=0):
     b = np.zeros(1, np.uint64)
