@@ -268,7 +268,7 @@ network_fwd_kernel(uint32_t n_max, const uint32_t* __restrict__ n_dev, const flo
 // Gradients rotate through buffers that died one stage earlier:
 //     g_h2 -> GX (the one extra slab), g_h1 -> the h2 slab, dYd -> the dYr slab, g_hd -> the h1 slab,
 // whose last reader (a weight-gradient wgmma) completed before the stage barrier the writing warpgroup passed.
-// Warps: 0-7 MLP chain, 8-15 hash-grid scatter of the previous pair of tiles.
+// Warps: 0-7 MLP chain, 8-19 hash-grid scatter of the previous pair of tiles.
 //
 // Both gradient sums are independent of scheduling, so that a training run is reproducible: each CTA stores its weight-gradient sums
 // in its own slot (layout [dwd | dwr]) and wgrad_reduce_kernel adds the slots in CTA order; the scatter adds into a 64-bit fixed-point
@@ -277,11 +277,18 @@ network_fwd_kernel(uint32_t n_max, const uint32_t* __restrict__ n_dev, const flo
 // and the scratch.  Without that scratch (see ngp_network_bwd) the kernel reduces straight into the outputs instead, with
 // fp32 / f16x2 reductions whose rounding depends on their order.
 constexpr uint32_t B3_G_GX = 32, B3_G_DY = 40, B3_G_DENC = 42, B3_GROUPS = 46;   // slab groups of one tile after the 32 activation groups
-constexpr uint32_t B3_EPI_THREADS = 256, B3_SCATTER_WARPS = 8, B3_THREADS = B3_EPI_THREADS + 32 * B3_SCATTER_WARPS;
+constexpr uint32_t B3_EPI_THREADS = 256, B3_SCATTER_WARPS = 12, B3_THREADS = B3_EPI_THREADS + 32 * B3_SCATTER_WARPS;
 // scatter items: (level, run of B3_RUN consecutive rows of the pair), 16 levels x 12 runs, each walked by a group of 4 lanes
 constexpr uint32_t B3_RUNS = 12, B3_ITEMS = 16 * B3_RUNS, B3_RUN = (2 * 128 + B3_RUNS - 1) / B3_RUNS;   // 22 rows
-constexpr uint32_t B3_SCATTER_GROUPS = 32 * B3_SCATTER_WARPS / 4, B3_NI = B3_ITEMS / B3_SCATTER_GROUPS;   // 3 items per group
+constexpr uint32_t B3_SCATTER_GROUPS = 32 * B3_SCATTER_WARPS / 4, B3_NI = B3_ITEMS / B3_SCATTER_GROUPS;   // 2 items per group
 static_assert(B3_SCATTER_GROUPS % 16 == 0 && B3_ITEMS % B3_SCATTER_GROUPS == 0, "a lane group walks items of one level only, as many as every other group");
+// Registers: the launch gives every thread B3_LAUNCH_REGS (65536 / B3_THREADS, down to a multiple of 8).  The scatter warpgroups then
+// drop to B3_SCATTER_REGS and the two chain warpgroups rise to B3_CHAIN_REGS, what their 40 weight-gradient accumulators, the
+// 32-register wgmma fragments and the prefetched operands need without spilling (setmaxnreg, wgmma.cuh).
+constexpr uint32_t B3_LAUNCH_REGS = 96, B3_CHAIN_REGS = 128, B3_SCATTER_REGS = 72;
+static_assert(B3_LAUNCH_REGS == 65536 / B3_THREADS / 8 * 8, "the launch count ptxas derives from __launch_bounds__(B3_THREADS, 1)");
+static_assert(B3_EPI_THREADS * B3_CHAIN_REGS + 32 * B3_SCATTER_WARPS * B3_SCATTER_REGS <= B3_THREADS * B3_LAUNCH_REGS,
+              "the registers the scatter warpgroups hand back cover what the chain warpgroups take");
 struct SmemBwd3 {
     static constexpr uint32_t coords = 0;                           // [tile][buf] 128 x 7 f32 (3584 B each)
     static constexpr uint32_t tile0 = coords + 4 * 3584;
@@ -478,11 +485,11 @@ network_bwd256_kernel(uint32_t n_max, const uint32_t* __restrict__ n_dev, const 
     uint64_t* bar_t = reinterpret_cast<uint64_t*>(smem + S::bar);
     NgpLevel* s_lv = reinterpret_cast<NgpLevel*>(smem + S::levels);
 
-    stage_weights(smem + S::w0d, wd + WD_W0, 64, 32, tid, B3_THREADS);
-    stage_weights(smem + S::woutd, wd + WD_WOUT, 16, 64, tid, B3_THREADS);
-    stage_weights(smem + S::w0r, wr + WR_W0, 64, 32, tid, B3_THREADS);
-    stage_weights(smem + S::w1r, wr + WR_W1, 64, 64, tid, B3_THREADS);
-    stage_weights(smem + S::woutr, wr + WR_WOUT, 16, 64, tid, B3_THREADS);
+    stage_weights_inline(smem + S::w0d, wd + WD_W0, 64, 32, tid, B3_THREADS);
+    stage_weights_inline(smem + S::woutd, wd + WD_WOUT, 16, 64, tid, B3_THREADS);
+    stage_weights_inline(smem + S::w0r, wr + WR_W0, 64, 32, tid, B3_THREADS);
+    stage_weights_inline(smem + S::w1r, wr + WR_W1, 64, 64, tid, B3_THREADS);
+    stage_weights_inline(smem + S::woutr, wr + WR_WOUT, 16, 64, tid, B3_THREADS);
     if (tid < N_LEVELS) s_lv[tid] = levels[tid];
     // zero both tiles once: dYr columns 4..15 are never rewritten, and 64-feature weight-gradient operands run past their slab
     for (uint32_t i = tid; i < 2 * S::tile_stride / 16; i += B3_THREADS) *reinterpret_cast<uint4*>(smem + S::tile0 + i * 16) = make_uint4(0, 0, 0, 0);
@@ -492,10 +499,13 @@ network_bwd256_kernel(uint32_t n_max, const uint32_t* __restrict__ n_dev, const 
     const uint32_t ntiles = (n_live + ROWS - 1) / ROWS, npairs = (ntiles + 1) / 2;
 
     if (warp < 4) {
+        reg_alloc<B3_CHAIN_REGS>();
         bwd_chain<0>(smem, tid, n_live, npairs, coords, enc_save, dout, w_part, dwd, dwr, err, dbg, &enc_map, enc_tma);
     } else if (warp < 8) {
+        reg_alloc<B3_CHAIN_REGS>();
         bwd_chain<1>(smem, tid, n_live, npairs, coords, enc_save, dout, w_part, dwd, dwr, err, dbg, &enc_map, enc_tma);
     } else {
+        reg_dealloc<B3_SCATTER_REGS>();
         // ------------------------------------------------------------------ scatter (HashEncode.h:339-347) of the pair's 256 rows
         // Item (level, sub) is a run of B3_RUN consecutive samples of one level, walked by a group of 4 adjacent lanes: every lane of the
         // group reads the same rows, skips the same rows and sees the same cell changes, and accumulates its own 4 (corner, feature) slots

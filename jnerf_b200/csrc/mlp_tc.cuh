@@ -12,12 +12,17 @@ constexpr uint32_t ROWS = 128;
 constexpr uint32_t GB = ROWS * 16;          // bytes of one slab feature-group (8 features x 128 rows)
 
 // ---- weights: global (out=rows, in=K) row-major  ->  smem [K/8][rows][8] (canonical K-major B operand) ----
-static __device__ __noinline__ void stage_weights(uint8_t* dst, const __half* __restrict__ W, int rows, int K, int tid, int nthr) {
+// Inlined form for kernels that move registers between warpgroups (setmaxnreg): ptxas applies the per-warpgroup counts only to a
+// kernel without calls, and otherwise compiles every warpgroup at the launch count.
+__device__ __forceinline__ void stage_weights_inline(uint8_t* dst, const __half* __restrict__ W, int rows, int K, int tid, int nthr) {
     const int kg = K / 8;
     for (int i = tid; i < rows * kg; i += nthr) {
         const int n = i / kg, g = i % kg;
         *reinterpret_cast<uint4*>(dst + (size_t)g * rows * 16 + n * 16) = __ldg(reinterpret_cast<const uint4*>(W + (size_t)n * K + g * 8));
     }
+}
+static __device__ __noinline__ void stage_weights(uint8_t* dst, const __half* __restrict__ W, int rows, int K, int tid, int nthr) {
+    stage_weights_inline(dst, W, rows, K, tid, nthr);
 }
 
 // ---- MMA issue (all 128 threads of one warpgroup) ----------------------------------------------------------

@@ -93,6 +93,15 @@ __device__ __forceinline__ bool elect_one() {
     return pred != 0;
 }
 
+// ---- register reallocation between warpgroups ------------------------------------------
+// setmaxnreg: every warp of a warpgroup sets its per-thread register count to N (a multiple of 8 in [24, 256]).  dec hands
+// registers back to the CTA's pool, inc waits until the pool holds enough.  The kernel needs a fixed launch count (launch bounds
+// or maxrregcount), and the counts after inc / dec must fit in (threads x launch count).
+template <uint32_t N>
+__device__ __forceinline__ void reg_alloc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N) : "memory"); }
+template <uint32_t N>
+__device__ __forceinline__ void reg_dealloc() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N) : "memory"); }
+
 // ---- warpgroup MMA ------------------------------------------------------------
 // wgmma_fence before the first wgmma of a batch (orders the accumulator registers and the shared-memory operands written before
 // it), then the wgmmas, wgmma_commit, and wgmma_wait<0> before the accumulators are read.
