@@ -272,6 +272,10 @@ int ngp_mesh_workspace_bytes(uint32_t n, uint64_t n_verts, uint64_t n_tris, uint
  * aabb), field_out[row] = float(int(max(sigma_raw, 0))) (:68).  Positions are made in the kernel (no coordinate buffer); sigma_raw is
  * bit-identical to ngp_density_fwd at the same positions. */
 int ngp_density_lattice(void* stream, uint32_t n, const void* grid, const void* levels_dev, const void* w_density, float* field_out);
+/* M1 on vanilla NeRF (extract_mesh.py:42-70 querying OriginNeRFNetworks, ori_nerf_network.py:58-67), csrc/nerf_lattice.cu: the same rows
+ * and positions, field_out[row] = float(int(max(alpha_raw, 0))) with alpha_raw bit-identical to ngp_nerf_density at the same position.
+ * params: the flat fp16 vector of ngp_nerf_fwd, 16-byte aligned.  Positions are made in the kernel (no coordinate buffer). */
+int ngp_nerf_density_lattice(void* stream, uint32_t n, const void* params, float* field_out);
 /* M2: mcubes.marching_cubes(sigma, iso) + the vertex frame of :78-84 (lattice position / n, first two columns swapped).  A vertex per
  * lattice edge whose endpoints straddle iso (inside: value > iso), numbered in lattice-edge order; triangles in cell order, their
  * right-hand normals pointing towards lower values in the written frame.  counts_host[0..1] = vertices, triangles, read back once.

@@ -17,6 +17,7 @@ SOURCES = {
     "mlp_tc.cu": [],
     "fused_net.cu": [],
     "nerf_mlp.cu": [],
+    "nerf_lattice.cu": [],
     "mip_mlp.cu": [],
     "mip_mlp_wide.cu": ["-fmad=false"],
     "mip_sampler.cu": ["-fmad=false"],

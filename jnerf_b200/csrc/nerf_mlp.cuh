@@ -1,5 +1,6 @@
 // The forward half of the vanilla NeRF network kernels (nerf_mlp.cu): parameter and saved-activation layouts, the weight stream, and
-// the forward kernel with its encode stage as a policy, shared by nerf_mlp.cu (FreqEnc) and mip_mlp.cu (MipEnc), and the backward bodies.
+// the forward kernel with its encode stage as a policy, shared by nerf_mlp.cu (FreqEnc), nerf_lattice.cu (LatticeEnc) and mip_mlp.cu
+// (MipEnc), and the backward bodies.
 // The encoder width is a compile-time parameter EG (8-column groups of kernel layer 0's input): 8 for NeRF and Mip-NeRF at 8 IPE
 // degrees, 12 for the 96 columns of 16 degrees (mip_mlp_wide.cu).  DESIGN.md sections 10-11.
 #pragma once
@@ -212,8 +213,9 @@ __device__ __forceinline__ void encode_rows(uint8_t* slab, X xat, uint32_t row0,
 }
 
 // The encode stage of the forward kernel is a compile-time policy: pos() fills the EG input groups of pts_linears.0 (and of the skip
-// layer), dir() the 4 view groups of views_linears.0.  FreqEnc is vanilla NeRF's FrequencyEncoder(10) / (4) of row[0:3] / row[4:7] of
-// `in` (stride floats a row); mip_mlp.cu adds the integrated positional encoding of Mip-NeRF.
+// layer), dir() the 4 view groups of views_linears.0; a policy used with DENSITY also stores the density kernel's output
+// (store_density).  FreqEnc is vanilla NeRF's FrequencyEncoder(10) / (4) of row[0:3] / row[4:7] of `in` (stride floats a row);
+// mip_mlp.cu adds the integrated positional encoding of Mip-NeRF, nerf_lattice.cu the positions of the mesh lattice.
 struct FreqEnc {
     static constexpr uint32_t EG = 8;
     __device__ __forceinline__ void pos(uint8_t* slab, const float* in, uint32_t stride, uint32_t row0, uint32_t n, uint32_t tid) const {
@@ -222,6 +224,7 @@ struct FreqEnc {
     __device__ __forceinline__ void dir(uint8_t* slab, const float* in, uint32_t stride, uint32_t row0, uint32_t n, uint32_t tid) const {
         encode_rows<4>(slab, [&](uint32_t row, uint32_t dim) { return in[(size_t)row * stride + 4 + dim]; }, row0, n, tid);
     }
+    __device__ __forceinline__ void store_density(__half* out, uint32_t row, __half alpha) const { out[row] = alpha; }
 };
 __device__ __forceinline__ void slab_to_global(const uint8_t* slab, uint32_t groups, __half* dst, uint32_t tid) {
     for (uint32_t i = tid; i < groups * ROWS; i += THREADS) reinterpret_cast<uint4*>(dst)[i] = reinterpret_cast<const uint4*>(slab)[i];
@@ -295,7 +298,7 @@ __global__ void __launch_bounds__(THREADS, 1)
                 const uint32_t row = row0 + 64 * m + frag_row(tw) + 8 * h;
                 if (row < n) {
                     const __half a = __float2half_rn(d[2 * h] + b);
-                    if (DENSITY) out[row] = a;
+                    if constexpr (DENSITY) enc.store_density(out, row, a);
                     else out[(size_t)row * 4 + 3] = a;
                 }
             }

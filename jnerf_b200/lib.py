@@ -65,6 +65,7 @@ SIGNATURES = {
     "ngp_svox_compact": (_i32, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _u32, _vp, _vp, _vp, _vp]),
     "ngp_mesh_workspace_bytes": (_i32, [_u32, _u64, _u64, _vp]),
     "ngp_density_lattice": (_i32, [_vp, _u32, _vp, _vp, _vp, _vp]),
+    "ngp_nerf_density_lattice": (_i32, [_vp, _u32, _vp, _vp]),
     "ngp_marching_cubes": (_i32, [_vp, _u32, _vp, _f32, _vp, _vp, _u64, _vp, _u64, _vp]),
     "ngp_mesh_largest_component": (_i32, [_vp, _u64, _u64, _vp, _vp, _vp, _vp, _vp, _vp]),
     "ngp_mesh_vertex_normals": (_i32, [_vp, _u64, _u64, _vp, _vp, _vp, _vp]),
@@ -109,7 +110,7 @@ KERNELS_PER_CALL = {
     "ngp_composite_bwd": 1, "ngp_composite_infer": 1, "ngp_composite_loss_bwd": 1, "ngp_grid_mark_untrained": 1,
     "ngp_grid_generate_samples": 1, "ngp_grid_splat": 1, "ngp_grid_ema": 1, "ngp_grid_update_bitfield": 7, "ngp_adam_ema": 1, "ngp_dp_exchange_step": 1, "ngp_dp_exchange_wait": 1, "ngp_raygen": 1, "ngp_prepare_batch": 1,
     "ngp_blend_target": 1,
-    "ngp_density_lattice": 1, "ngp_marching_cubes": 3, "ngp_mesh_largest_component": 18, "ngp_mesh_vertex_normals": 7,
+    "ngp_density_lattice": 1, "ngp_nerf_density_lattice": 1, "ngp_marching_cubes": 3, "ngp_mesh_largest_component": 18, "ngp_mesh_vertex_normals": 7,
     "ngp_render_init": 3, "ngp_render_march_round": 3, "ngp_render_composite_round": 3,
     "ngp_nerf_fwd": 1, "ngp_nerf_density": 1, "ngp_nerf_bwd": 3,
     "ngp_mip_rays": 1, "ngp_mip_sample": 1, "ngp_mip_resample": 1, "ngp_mip_encode": 1, "ngp_mip_fwd": 1, "ngp_mip_composite_fwd": 1,

@@ -400,6 +400,16 @@ def density_lattice(n, grid, levels, wd):
     return field
 
 
+def nerf_density_lattice(n, params):
+    """density_lattice of vanilla NeRF: the (n, n, n) fp32 field float(int(max(alpha_raw, 0))) of the flat fp16 `params` at model
+    positions (i, j, k) / (n-1), alpha_raw bit for bit nerf_density's at those positions."""
+    if not 2 <= int(n) <= 1024:
+        raise lib.NgpError(f"nerf_density_lattice: resolution {n} is outside [2, 1024]")
+    field = torch.empty((n, n, n), dtype=torch.float32, device=params.device)
+    lib.call("ngp_nerf_density_lattice", _stream(), int(n), _p(params), _p(field))
+    return field
+
+
 def marching_cubes(field, iso=0.5, workspace=None):
     """(n, n, n) fp32 field -> vertices (V, 3) f32 in the PLY frame, triangles (T, 3) int32.  One read-back of the counts per call."""
     import ctypes

@@ -60,16 +60,16 @@ def _kernel_views(flat, name, layers=REF_LAYERS, ins=IN):
     return W[r0:r0 + o], b[r0:r0 + o], cols
 
 
-def pack(ref, layers=REF_LAYERS, ins=IN):
+def pack(ref, layers=REF_LAYERS, ins=IN, dtype=torch.float16):
     """{reference name: (weight (out, in), bias (out,))} -> the flat fp16 vector of the kernels (layers: the name table, e.g. plugin/mip.py's;
-    ins: the kernel layers' padded input widths, e.g. Mip-NeRF's at 16 IPE degrees)."""
+    ins: the kernel layers' padded input widths, e.g. Mip-NeRF's at 16 IPE degrees; dtype: fp32 for optimizer state in the same layout)."""
     dev = next(iter(ref.values()))[0].device
-    flat = torch.zeros(w_offsets(ins)[-1], dtype=torch.float16, device=dev)
+    flat = torch.zeros(w_offsets(ins)[-1], dtype=dtype, device=dev)
     for name, (W, b) in ref.items():
         Wk, bk, cols = _kernel_views(flat, name, layers, ins)
         for rc, kc, n in cols:
-            Wk[:, kc:kc + n] = W[:, rc:rc + n].to(torch.float16)
-        bk.copy_(b.to(torch.float16))
+            Wk[:, kc:kc + n] = W[:, rc:rc + n].to(dtype)
+        bk.copy_(b.to(dtype))
     return flat
 
 
@@ -197,6 +197,14 @@ class OriginNeRFNetworks(Module):
             if self.using_fp16:
                 return ops.nerf_density(pos_input.contiguous(), self.params).unsqueeze(-1)
             return self.alpha_linear(self._trunk(pos_input))
+
+    @torch.no_grad()
+    def density_lattice(self, n):
+        """The (n, n, n) field of Runner.extract_mesh (ops.nerf_density_lattice): float(int(max(alpha, 0))) at (i, j, k) / (n-1), on
+        the fp16 kernels only."""
+        if not self.using_fp16:
+            raise NotImplementedError("OriginNeRFNetworks.density_lattice runs on the fused kernels (fp16=True)")
+        return ops.nerf_density_lattice(n, self.params)
 
     @torch.no_grad()
     def infer(self, rows, n_dev, out):

@@ -738,10 +738,12 @@ class Runner:
         out_dir/mesh-color.ply.  The colour ray starts 0.2 outside the vertex and runs along the unit normal into the object (towards
         higher density), in model space (DESIGN.md section 7).  mcube_smooth (:74-78): the lattice is smoothed (ops.mesh_smooth, method
         auto) and marched at 0 instead, which removes the terraces of the integer density field; the result then also holds the
-        smoothing's info under "smooth".  Returns the arrays, the counts and the device time of each stage."""
+        smoothing's info under "smooth".  Returns the arrays, the counts and the device time of each stage.  Vanilla NeRF runs it
+        through NerfRunner (nerf_runner.py)."""
         import os
         from .utils.ply import write_ply
-        if not self.fast:
+        lattice = self._density_lattice_fn()
+        if lattice is None:
             raise NotImplementedError(f"extract_mesh: mesh extraction runs on the fused NGPNetworks kernels; {type(self.model).__name__} "
                                       "(fp16 / use_fully off, or another model) has no density lattice kernel")
         self._table_ready()
@@ -755,7 +757,7 @@ class Runner:
         ev = [torch.cuda.Event(enable_timing=True) for _ in range(len(names) + 1)]
         stamps = iter(ev)                                             # one event after each stage, in the order of `names`
         next(stamps).record()
-        field = ops.density_lattice(N, m.pos_encoder.m_grid, m.pos_encoder.levels, m.density_mlp.con_weights)
+        field = lattice(N)
         next(stamps).record()
         smooth = None
         if mcube_smooth:
@@ -792,6 +794,13 @@ class Runner:
             res["smooth"] = smooth
         return res
 
+    def _density_lattice_fn(self):
+        """extract_mesh's lattice query, n -> the (n, n, n) field, or None when the model has no lattice kernel."""
+        if not self.fast:
+            return None
+        m = self.model
+        return lambda n: ops.density_lattice(n, m.pos_encoder.m_grid, m.pos_encoder.levels, m.density_mlp.con_weights)
+
     @torch.no_grad()
     def psnr(self, dataset_mode="val", max_images=None):
         """mean over images of -10 log10(mse) (runner.py:86-99, mse_loss.py:6-7)."""
@@ -823,21 +832,34 @@ class Runner:
             sampler_state["rng"] = torch.from_numpy(self._pipe["pending"]["rng_before"].astype(np.int64))
         ck = {"global_step": self.cfg.m_training_step, "model": self.model.state_dict(), "sampler": sampler_state,
               "optimizer": self.optimizer.state_dict(), "nested_optimizer": nested, "ema_optimizer": self.ema_optimizer.state_dict()}
-        if str(path).endswith(".pkl") and not hasattr(getattr(self.model, "density_mlp", None), "con_weights"):
-            raise NotImplementedError(f"the .pkl interchange format is written for the fused-MLP parameter layout (con_weights) of "
-                                      f"NGPNetworks; save {type(self.model).__name__} to a .pt path")
         if str(path).endswith(".pkl"):
             # the reference's params.pkl wire format (runner/runner.py:123-131), readable by its load_ckpt (:133-151)
             from .utils import ckpt_compat as cc
             dec = self.optimizer
-            ref = cc.native_to_reference(
+            ref = self._to_reference(
                 ck, adam_hyper=dict(lr=adam.lr, eps=adam.eps, betas=tuple(adam.betas)),
                 expdecay_hyper=dict(base_lr=dec.base_lr, decay_start=dec.decay_start, decay_interval=dec.decay_interval, decay_base=dec.decay_base,
-                                    decay_end=dec.decay_end),
-                param_dtype=np.float16 if self.model.pos_encoder.m_grid.dtype == torch.float16 else np.float32)
+                                    decay_end=dec.decay_end))
             cc.write_reference_ckpt(ref, path)
             return
         torch.save(ck, path)
+
+    def _to_reference(self, ck, adam_hyper, expdecay_hyper):
+        """save_ckpt's native dict -> the reference's params.pkl dict (the fused NGP parameter layout)."""
+        if not hasattr(getattr(self.model, "density_mlp", None), "con_weights"):
+            raise NotImplementedError(f"the .pkl interchange format is written for the fused-MLP parameter layout (con_weights) of "
+                                      f"NGPNetworks; save {type(self.model).__name__} to a .pt path")
+        from .utils import ckpt_compat as cc
+        return cc.native_to_reference(ck, adam_hyper=adam_hyper, expdecay_hyper=expdecay_hyper,
+                                      param_dtype=np.float16 if self.model.pos_encoder.m_grid.dtype == torch.float16 else np.float32)
+
+    def _from_reference_file(self, path):
+        """A params.pkl -> the native dict load_ckpt consumes, on the device."""
+        if not hasattr(getattr(self.model, "density_mlp", None), "con_weights"):
+            raise NotImplementedError("the .pkl interchange format carries the fused-MLP parameter layout; load a .pt checkpoint instead")
+        from .utils import ckpt_compat as cc
+        return cc.load_native_from_reference_file(path, self.model.pos_encoder.m_grid.numel(), "cuda",
+                                                  {k: v.dtype for k, v in self.model.state_dict().items()})
 
     def load_ckpt(self, path):
         self._table_ready()                                          # an exchange of the previous step may still be writing the table
@@ -847,12 +869,8 @@ class Runner:
         if self.world_size > 1:
             import torch.distributed as dist
             dist.barrier(group=self.pg)                              # no peer may still push into this rank's table while it is overwritten
-        if str(path).endswith(".pkl") and not hasattr(getattr(self.model, "density_mlp", None), "con_weights"):
-            raise NotImplementedError("the .pkl interchange format carries the fused-MLP parameter layout; load a .pt checkpoint instead")
         if str(path).endswith(".pkl"):
-            from .utils import ckpt_compat as cc
-            ck = cc.load_native_from_reference_file(path, self.model.pos_encoder.m_grid.numel(), "cuda",
-                                                    {k: v.dtype for k, v in self.model.state_dict().items()})
+            ck = self._from_reference_file(path)
         else:
             ck = torch.load(path, map_location="cuda", weights_only=True)      # tensors, numbers, lists and dicts only
         self.cfg.m_training_step = self.start = ck["global_step"]

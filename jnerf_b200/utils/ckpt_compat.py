@@ -21,6 +21,14 @@ Parameters are matched by element count, not by key or position: whether Jittor 
 trainable tensors of NGP have distinct sizes.  `nn.Linear` checkpoints (the reference's fp32 fallback, ngp_network.py:59-67) are
 folded into the flat `con_weights` layout of OPS/fully_fused_mlp.py:26-40.
 
+Vanilla NeRF (OriginNeRFNetworks, projects/nerf/configs/nerf_base.py) is matched by NAME instead: most of its 24 tensors are
+(256, 256), so element counts cannot tell them apart.  Its model dict holds pts_linears.{0..7}, views_linears.0, feature_linear,
+alpha_linear and rgb_linear, each .weight (out, in) and .bias, and the i-th entry of the Adam / EMA lists belongs to the i-th key of
+that dict (Jittor's state_dict() and parameters() traverse the modules in the same order).  Every entry's shape is checked against its
+key's; but a file whose lists swapped two equal-shaped tensors passes every check and loads them crossed, which cannot be detected
+without Jittor (SURVEY 8c).  Either native form maps to the same file: the fp16 kernels' flat vector through plugin/nerf.py's
+pack / unpack (padding zero), the fp32 nn.Linear chain one to one.
+
 Two reference behaviours that are NOT reproduced (documented deviations):
   * the reference excludes Adam's `n_step` from its state (optims/adam.py:13-16), so its bias correction restarts at 1 after a
     resume; here n_step is restored from the EMA step counter (the two advance together, runner.py:75-76);
@@ -138,6 +146,24 @@ def _by_size(tensors, sizes):
     return [got[s] for s in sizes]
 
 
+def _floor_second_moments(m, v):
+    """A reference-written file holds moments in the parameter dtype: with fp16, second moments below fp16's smallest subnormal
+    (6e-8) are stored as 0 while the first moment survives, and lr * m / (sqrt(0) + 1e-15) would throw the entry to inf on the next
+    step.  Floor v at m^2 (|update| <= lr, Adam's own bound) for exactly those entries; where m^2 underflows fp32 as well, drop the
+    momentum.  -> (m, v) lists in fp32."""
+    fixed = []
+    for mm, vv in zip(m, v):
+        mm32, vv32 = np.asarray(mm, np.float32), np.asarray(vv, np.float32).copy()
+        bad = (vv32 == 0) & (mm32 != 0)
+        vv32[bad] = mm32[bad] * mm32[bad]
+        still = bad & (vv32 == 0)
+        if still.any():
+            mm32 = mm32.copy()
+            mm32[still] = 0
+        fixed.append((mm32, vv32))
+    return [f[0] for f in fixed], [f[1] for f in fixed]
+
+
 # ---------------------------------------------------------------------------------------------------- whole checkpoints
 def reference_to_native(ref, n_table):
     """Reference params.pkl dict -> the dict Runner.load_ckpt consumes (numpy arrays; the loader moves them to the device).
@@ -157,26 +183,21 @@ def reference_to_native(ref, n_table):
             v = _by_size(pg["values"], sizes)
             m = _by_size(pg["m"], sizes)
             ema_vals = _by_size(ema_d["param_groups"][0]["values"], sizes)
-            # a reference-written file holds fp16 moments: second moments below fp16's smallest subnormal (6e-8) are stored as 0
-            # while the first moment survives, and lr * m / (sqrt(0) + 1e-15) would throw the entry to inf on the next step.
-            # Floor v at m^2 (|update| <= lr, Adam's own bound) for exactly those entries.
-            fixed = []
-            for mm, vv in zip(m, v):
-                mm32, vv32 = np.asarray(mm, np.float32), np.asarray(vv, np.float32).copy()
-                bad = (vv32 == 0) & (mm32 != 0)
-                vv32[bad] = mm32[bad] * mm32[bad]
-                still = bad & (vv32 == 0)                            # m^2 underflows fp32 as well: drop the momentum
-                if still.any():
-                    mm32 = mm32.copy()
-                    mm32[still] = 0
-                fixed.append((mm32, vv32))
-            m, v = [f[0] for f in fixed], [f[1] for f in fixed]
+            m, v = _floor_second_moments(m, v)
     except KeyError:
         # nn.Linear checkpoints keep one moment tensor per matrix; the flat fused layout restarts the moments and takes the
         # parameters themselves as EMA values (after every ema_step the two are equal, ema.py:33-36)
         m = [np.zeros(n, np.float32) for n in sizes]
         v = [np.zeros(n, np.float32) for n in sizes]
         ema_vals = [p["m_grid"], p["density"], p["rgb"]]
+    model = {"pos_encoder.m_grid": p["m_grid"], "density_mlp.con_weights": p["density"], "rgb_mlp.con_weights": p["rgb"]}
+    return _native_dict(ref, model, m, v, ema_vals)
+
+
+def _native_dict(ref, model, m, v, master):
+    """The native checkpoint dict around the model dict and the optimizer lists (in the model's parameter order)."""
+    nested = ref["nested_optimizer"]["defaults"]
+    ema_d = ref["ema_optimizer"]["defaults"]
     steps = int(ema_d["steps"])
     opt = ref["optimizer"]["defaults"]
     s = ref["sampler"]
@@ -191,11 +212,11 @@ def reference_to_native(ref, n_table):
     f32 = lambda a: np.asarray(a, np.float32)                                            # noqa: E731
     return {
         "global_step": int(ref["global_step"]),
-        "model": {"pos_encoder.m_grid": p["m_grid"], "density_mlp.con_weights": p["density"], "rgb_mlp.con_weights": p["rgb"]},
+        "model": model,
         "sampler": sampler,
         "optimizer": {"steps": int(opt["steps"]), "m_learning_rate_factor": float(opt["m_learning_rate_factor"])},
         "nested_optimizer": {"n_step": steps, "lr": float(nested.get("lr", 0.1)), "m": [f32(x) for x in m], "v": [f32(x) for x in v],
-                             "master": [f32(x) for x in ema_vals]},
+                             "master": [f32(x) for x in master]},
         "ema_optimizer": {"steps": steps, "decay": float(ema_d.get("decay", 0.95))},
     }
 
@@ -205,6 +226,13 @@ def native_to_reference(nat, adam_hyper=None, expdecay_hyper=None, param_dtype=n
     nat = _to_numpy(nat)
     model = {k: np.asarray(v) for k, v in nat["model"].items()}
     order = ["pos_encoder.m_grid", "density_mlp.con_weights", "rgb_mlp.con_weights"]
+    nested = nat["nested_optimizer"]
+    return _reference_dict(nat, {k: model[k] for k in order}, nested["m"], nested["v"], nested["master"], adam_hyper, expdecay_hyper, param_dtype)
+
+
+def _reference_dict(nat, model, m, v, master, adam_hyper, expdecay_hyper, param_dtype):
+    """The reference's params.pkl structure around its model dict and the optimizer lists (one entry per model key, in its order);
+    nat: the native dict (numpy) the counters, learning rates and sampler state come from."""
     nested, ema = nat["nested_optimizer"], nat["ema_optimizer"]
     cast = lambda a: np.asarray(a).astype(param_dtype)                                   # noqa: E731  Jittor keeps m / values in the parameter dtype
     f32 = lambda a: np.asarray(a, np.float32)                                            # noqa: E731
@@ -222,23 +250,111 @@ def native_to_reference(nat, adam_hyper=None, expdecay_hyper=None, param_dtype=n
             sampler[k] = np.asarray(s[k])
     return {
         "global_step": int(nat["global_step"]),
-        "model": {k: model[k] for k in order},
+        "model": model,
         "sampler": sampler,
         "optimizer": {"defaults": dict(dec, steps=int(nat["optimizer"]["steps"]), m_learning_rate_factor=nat["optimizer"]["m_learning_rate_factor"])},
         # "values"/"m" in the parameter dtype are what the reference's load_ckpt reads (runner.py:133-151); the *_f32 keys are ignored
         # by it and preferred by reference_to_native, so a save -> load in this repo is lossless (fp16 flushes most second moments to 0)
-        "nested_optimizer": {"defaults": dict(hyper, param_groups=[{"values": [cast(x) for x in nested["v"]], "m": [cast(x) for x in nested["m"]],
-                                                                    "values_f32": [f32(x) for x in nested["v"]], "m_f32": [f32(x) for x in nested["m"]]}])},
+        "nested_optimizer": {"defaults": dict(hyper, param_groups=[{"values": [cast(x) for x in v], "m": [cast(x) for x in m],
+                                                                    "values_f32": [f32(x) for x in v], "m_f32": [f32(x) for x in m]}])},
         "ema_optimizer": {"defaults": {"lr": 0, "decay": float(ema["decay"]), "steps": int(ema["steps"]),
-                                       "param_groups": [{"values": [cast(x) for x in nested["master"]],
-                                                         "values_f32": [f32(x) for x in nested["master"]]}]}},
+                                       "param_groups": [{"values": [cast(x) for x in master],
+                                                         "values_f32": [f32(x) for x in master]}]}},
     }
 
 
-def load_native_from_reference_file(path, n_table, device, model_dtypes=None):
-    """params.pkl -> the dict Runner.load_ckpt consumes, with torch tensors on `device` (model tensors cast to model_dtypes[key])."""
+# ---------------------------------------------------------------------------------------------------- vanilla NeRF (OriginNeRFNetworks)
+def nerf_reference_shapes():
+    """{reference key: shape} of OriginNeRFNetworks' 24 tensors in its state_dict() order (ori_nerf_network.py:21-26)."""
+    from ..plugin.nerf import REF_LAYERS, REF_ORDER
+    return {f"{name}.{part}": (REF_LAYERS[name][0] if part == "weight" else REF_LAYERS[name][0][:1]) for name in REF_ORDER for part in ("weight", "bias")}
+
+
+def _nerf_split(entries, flat):
+    """Native NeRF tensors -> {reference key: fp32 array of the reference shape}.  flat: entries is [the one flat vector of the fp16
+    kernels' layout] (mapped through plugin/nerf.py's unpack); else one entry per reference key, in nerf_reference_shapes() order."""
+    shapes = nerf_reference_shapes()
+    if not flat:
+        return {k: np.asarray(e, np.float32).reshape(shp) for (k, shp), e in zip(shapes.items(), entries)}
     import torch
-    nat = reference_to_native(read_reference_ckpt(path), n_table)
+    from ..plugin.nerf import unpack
+    out = {}
+    for name, (W, b) in unpack(torch.from_numpy(np.ascontiguousarray(np.asarray(entries[0])).reshape(-1))).items():
+        out[f"{name}.weight"], out[f"{name}.bias"] = W.numpy(), b.numpy()
+    return {k: out[k] for k in shapes}
+
+
+def _nerf_join(tensors, flat, half=False):
+    """Inverse of _nerf_split: {reference key: array} -> [one flat vector, fp16 if half else fp32, zero padding] (flat) or one flat fp32
+    entry per key."""
+    if not flat:
+        return [np.asarray(t, np.float32).reshape(-1) for t in tensors.values()]
+    import torch
+    from ..plugin.nerf import REF_ORDER, pack
+    t = {name: (torch.from_numpy(np.asarray(tensors[f"{name}.weight"], np.float32)), torch.from_numpy(np.asarray(tensors[f"{name}.bias"], np.float32)))
+         for name in REF_ORDER}
+    return [pack(t, dtype=torch.float16 if half else torch.float32).numpy()]
+
+
+def nerf_native_to_reference(nat, adam_hyper=None, expdecay_hyper=None, param_dtype=np.float16):
+    """native_to_reference for OriginNeRFNetworks: the model dict and every optimizer list as the reference's 24 tensors by name, from
+    either native form (fp16: the flat `params` vector and flat moments; fp32: the nn.Linear chain, already under the reference names)."""
+    nat = _to_numpy(nat)
+    flat = "params" in nat["model"]
+    model = _nerf_split(list(nat["model"].values()), flat)
+    nested = nat["nested_optimizer"]
+    m, v, master = (list(_nerf_split(nested[k], flat).values()) for k in ("m", "v", "master"))
+    return _reference_dict(nat, {k: t.astype(param_dtype) for k, t in model.items()}, m, v, master, adam_hyper, expdecay_hyper, param_dtype)
+
+
+def nerf_reference_to_native(ref, fp16):
+    """A params.pkl of OriginNeRFNetworks -> the native dict of the fp16 kernels' model (fp16=True: the flat `params` vector and flat
+    fp32 moments, zero padding) or of the nn.Linear chain (fp16=False).  Tensors are matched by name: the i-th entry of the Adam and
+    EMA lists belongs to the i-th key of the model dict, and each must have that key's shape."""
+    model = ref["model"]
+    keys = list(model)
+    shapes = nerf_reference_shapes()
+    missing = [k for k in shapes if k not in model]
+    if missing:
+        raise KeyError(f"the checkpoint's model dict is not OriginNeRFNetworks' (D=8, W=256, skips=[4]): no {missing[:3]}"
+                       f"{' ...' if len(missing) > 3 else ''}; it holds {keys[:4]}{' ...' if len(keys) > 4 else ''}")
+    for k, shp in shapes.items():
+        if tuple(np.shape(model[k])) != shp:
+            raise ValueError(f"params.pkl: model tensor {k} has shape {tuple(np.shape(model[k]))}, OriginNeRFNetworks' is {shp}")
+    pg = ref["nested_optimizer"]["defaults"]["param_groups"][0]
+    ema_pg = ref["ema_optimizer"]["defaults"]["param_groups"][0]
+    lossless = "values_f32" in pg                                      # written by nerf_native_to_reference
+
+    def by_key(what, lst):
+        if len(lst) != len(keys):
+            raise ValueError(f"params.pkl: {what} holds {len(lst)} tensors, the model dict {len(keys)}")
+        for k, t in zip(keys, lst):
+            if tuple(np.shape(t)) != tuple(np.shape(model[k])):
+                raise ValueError(f"params.pkl: the {what} entry of {k} has shape {tuple(np.shape(t))}, the parameter {tuple(np.shape(model[k]))}")
+        got = dict(zip(keys, lst))
+        return [np.asarray(got[k], np.float32) for k in shapes]
+
+    if lossless:
+        v, m = by_key("Adam values_f32", pg["values_f32"]), by_key("Adam m_f32", pg["m_f32"])
+        master = by_key("EMA values_f32", ema_pg.get("values_f32", ema_pg["values"]))
+    else:
+        m, v = _floor_second_moments(by_key("Adam m", pg["m"]), by_key("Adam values", pg["values"]))
+        master = by_key("EMA values", ema_pg["values"])
+    params = {k: np.asarray(model[k]) for k in shapes}
+    if fp16:
+        native_model = {"params": _nerf_join(params, True, half=True)[0]}
+    else:
+        native_model = {k: t.astype(np.float32) for k, t in params.items()}
+    lists = [_nerf_join(dict(zip(shapes, x)), fp16) for x in (m, v, master)]
+    return _native_dict(ref, native_model, *lists)
+
+
+def load_native_from_reference_file(path, n_table, device, model_dtypes=None, nerf_fp16=None):
+    """params.pkl -> the dict Runner.load_ckpt consumes, with torch tensors on `device` (model tensors cast to model_dtypes[key]).
+    nerf_fp16: None for NGPNetworks (hash table of n_table entries); True / False for OriginNeRFNetworks with that fp16 setting."""
+    import torch
+    ref = read_reference_ckpt(path)
+    nat = reference_to_native(ref, n_table) if nerf_fp16 is None else nerf_reference_to_native(ref, nerf_fp16)
 
     def dev(x):
         if isinstance(x, np.ndarray):

@@ -1,11 +1,13 @@
 #!/usr/bin/env python
 """Export a trained model as a coloured mesh: the reference's tools/extract_mesh.py on the device (Runner.extract_mesh).
 
-    python tools/extract_mesh.py --ckpt CKPT (--config-file CFG | --workload lego|fox) [--resolution 512] [--mcube_smooth] [--out DIR]
-    python tools/extract_mesh.py --workload lego --train-steps 3000 [--resolution 512] [--mcube_smooth] [--out DIR]
+    python tools/extract_mesh.py --ckpt CKPT (--config-file CFG | --workload lego|fox|nerf) [--resolution 512] [--mcube_smooth] [--out DIR]
+    python tools/extract_mesh.py --workload lego|nerf --train-steps 3000 [--resolution 512] [--mcube_smooth] [--out DIR]
 
---ckpt takes this project's .pt checkpoints or the reference's params.pkl.  Without --ckpt, --train-steps trains the stand-in first
-(the configuration of tools/train_psnr.py).  Writes DIR/mesh-origin.ply and DIR/mesh-color.ply and prints one JSON line: vertex and
+--ckpt takes this project's .pt checkpoints or the reference's params.pkl (NGP configs and projects/nerf/configs/nerf_base.py).
+Without --ckpt, --train-steps trains the stand-in first (the configuration of tools/train_psnr.py); --workload nerf is nerf_base.py
+(vanilla NeRF, fp16 kernels, through NerfRunner) on the lego stand-in, trained at Adam lr 5e-4: nerf_base.py's 1e-2 diverges on the
+stand-in.  Writes DIR/mesh-origin.ply and DIR/mesh-color.ply and prints one JSON line: vertex and
 triangle counts before and after the component filter and the device time of every stage (CUDA events); with --mcube_smooth also
 the smoothing method, its iterations and its band variables."""
 import argparse
@@ -21,7 +23,8 @@ sys.path.insert(0, ROOT)
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--config-file", default="", help="a JNeRF config (projects/ngp/configs/*.py)")
-    ap.add_argument("--workload", default="lego", choices=["lego", "fox"], help="the synthetic stand-ins, as in tools/train_psnr.py")
+    ap.add_argument("--workload", default="lego", choices=["lego", "fox", "nerf"],
+                    help="the synthetic stand-ins, as in tools/train_psnr.py; nerf: nerf_base.py on the lego stand-in")
     ap.add_argument("--ckpt", default=None, help=".pt checkpoint of this project or the reference's .pkl")
     ap.add_argument("--train-steps", type=int, default=0, help="without --ckpt: train the stand-in for this many steps first")
     ap.add_argument("--images", type=int, default=100)
@@ -36,7 +39,7 @@ def main():
 
     import torch
     from jnerf_b200 import lib, plugin  # noqa: F401
-    from jnerf_b200.runner import Runner, fox_cfg, lego_cfg
+    from jnerf_b200.runner import Runner, fox_cfg, lego_cfg, nerf_cfg
     from jnerf_b200.utils.config import get_cfg, init_cfg, update_cfg
 
     lib.load()
@@ -47,7 +50,10 @@ def main():
         update_cfg(**fox_cfg(fp16=True, synthetic=True, seed=1))
         get_cfg().dataset.val = None
     else:
-        update_cfg(**lego_cfg(fp16=True, synthetic=True, seed=1))
+        if args.workload == "nerf":
+            update_cfg(**nerf_cfg(fp16=True, synthetic=True, seed=1, optim=dict(type="Adam", lr=5e-4, eps=1e-15, betas=(0.9, 0.99))))
+        else:
+            update_cfg(**lego_cfg(fp16=True, synthetic=True, seed=1))
         cfg = get_cfg()
         for split in ("train", "val"):
             d = cfg.dataset[split]
@@ -55,12 +61,14 @@ def main():
             d.H = d.W = args.res
             d.pop("root_dir", None)
         cfg.dataset.test = None
-    runner = Runner()
+    from jnerf_b200.nerf_runner import NerfRunner
+    runner = (NerfRunner if get_cfg().model.type == "OriginNeRFNetworks" else Runner)()
     if args.ckpt:
         runner.load_ckpt(args.ckpt)
     elif args.train_steps:
+        step = runner.train_step if runner.fast else runner.train_step_autograd
         for _ in range(args.train_steps):
-            runner.train_step()
+            step()
     torch.cuda.synchronize()
     t0 = time.perf_counter()
     res = runner.extract_mesh(args.out, resolution=args.resolution, mcube_smooth=args.mcube_smooth)
