@@ -473,6 +473,88 @@ __device__ __forceinline__ void bwd_chain(uint8_t* smem, uint32_t tid, uint32_t 
     }
 }
 
+// ------------------------------------------------------------------------ scatter (HashEncode.h:339-347) of a pair's 256 rows
+// FX_ALL: the fixed-point scratch holds every entry of the table, so the scatter reduces through red_add_fx alone, with no per-entry
+// test and no warp-synchronous f16x2 fallback in its loop.
+template <bool FX_ALL>
+__device__ __forceinline__ void bwd_scatter(const uint8_t* smem, uint32_t tid, uint32_t n_live, uint32_t npairs, __half* __restrict__ grid_grad,
+                                            unsigned long long* __restrict__ grid_fx, uint32_t fx_entries, uint32_t dbg) {
+    using S = SmemBwd3;
+    // Item (level, sub) is a run of B3_RUN consecutive samples of one level, walked by a group of 4 adjacent lanes: every lane of the
+    // group reads the same rows, skips the same rows and sees the same cell changes, and accumulates its own 4 (corner, feature) slots
+    // in fp32 registers while the grid cell stays the same.  Lane bit 0 is the feature f, bit 1 picks the corner 2j + h of each
+    // x-neighbour pair (2j, 2j + 1).  At a cell change slot j of the 4 lanes is reduced by one instruction: both features of both
+    // x-neighbours, 32 bytes of the fixed-point copy, which are one aligned sector whenever the pair's entries are 2k and 2k + 1.
+    const uint32_t ts = tid - B3_EPI_THREADS, grp = ts >> 2, f = ts & 1, h = (ts >> 1) & 1;
+    const uint32_t level = grp & 15;                                         // item = grp + k * B3_SCATTER_GROUPS: level = item & 15
+    const NgpLevel lv = reinterpret_cast<const NgpLevel*>(smem + S::levels)[level];
+    const uint64_t lv_m = fastmod_m(lv.size);                                // the dense levels' base index without a division
+    const bool reduce = !(dbg & 1), scatter = !(dbg & 2);
+    unsigned long long* fx = grid_fx + 2 * (size_t)lv.offset;
+    auto reduce_slots = [&](const uint32_t (&idx)[4], const float (&acc)[4]) {
+#pragma unroll
+        for (uint32_t j = 0; j < 4; ++j) {
+            if constexpr (FX_ALL) {
+                red_add_fx(fx + 2 * (size_t)idx[j] + f, acc[j]);
+            } else {
+                const uint32_t fx_live = fx_entries > lv.offset ? fx_entries - lv.offset : 0u;   // entries of this level the scratch holds
+                red_add_entry_lane(fx, fx_live, reinterpret_cast<__half2*>(grid_grad) + lv.offset, idx[j], f, acc[j]);
+            }
+        }
+    };
+    // The group's B3_NI items (grp + i * B3_SCATTER_GROUPS) are walked side by side, row k of each in the same iteration: their
+    // shared-memory reads and cell arithmetic are independent, so they overlap instead of adding up.  Each item still sees its rows
+    // in order, so its run sums are the same; only the order of the (integer, order-free) reductions across items changes.
+    uint32_t it = 0;
+    for (uint32_t pair = blockIdx.x; pair < npairs; pair += gridDim.x, ++it) {
+        const uint32_t buf = it & 1;
+        named_bar_sync(B3_FULL, B3_EPI_THREADS + 32 * B3_SCATTER_WARPS);
+        uint32_t cgx[B3_NI], cgy[B3_NI], cgz[B3_NI], idx[B3_NI][4];
+        float acc[B3_NI][4];
+        bool live[B3_NI], dirty[B3_NI];
+#pragma unroll
+        for (uint32_t i = 0; i < B3_NI; ++i) { cgx[i] = 0xffffffffu; cgy[i] = cgz[i] = 0; live[i] = scatter; dirty[i] = false; }
+#pragma unroll 1
+        for (uint32_t k = 0; k < B3_RUN; ++k) {
+            float2 df[B3_NI];
+            HashCell hc[B3_NI];
+#pragma unroll
+            for (uint32_t i = 0; i < B3_NI; ++i) {
+                const uint32_t r = B3_RUN * ((grp + i * B3_SCATTER_GROUPS) >> 4) + k;   // row of the pair: tile r >> 7, row r & 127
+                live[i] = live[i] && r < 2 * ROWS && 2 * pair * ROWS + r < n_live;        // rows past the pair or the live rows end the run
+                const uint32_t rc = min(r, 2 * ROWS - 1), T = rc >> 7, p = rc & 127;       // read in bounds either way
+                const uint8_t* denc = smem + S::tile0 + T * S::tile_stride + B3_G_DENC * GB;
+                const float* s_coords = reinterpret_cast<const float*>(smem + S::coords + (2 * T + buf) * 3584);
+                df[i] = __half22float2(*reinterpret_cast<const __half2*>(denc + (size_t)(level >> 2) * GB + p * 16 + (level & 3) * 4));
+                hc[i] = hash_cell(lv, s_coords[p * 7], s_coords[p * 7 + 1], s_coords[p * 7 + 2]);
+            }
+#pragma unroll
+            for (uint32_t i = 0; i < B3_NI; ++i) {
+                if (!live[i] || (df[i].x == 0.f && df[i].y == 0.f)) continue;
+                if (hc[i].gx != cgx[i] || hc[i].gy != cgy[i] || hc[i].gz != cgz[i]) {
+                    if (dirty[i]) reduce_slots(idx[i], acc[i]);
+                    cgx[i] = hc[i].gx; cgy[i] = hc[i].gy; cgz[i] = hc[i].gz;
+                    hash_cell_indices_x(lv, lv_m, cgx[i], cgy[i], cgz[i], h, idx[i]);
+#pragma unroll
+                    for (uint32_t j = 0; j < 4; ++j) acc[i][j] = 0.f;
+                    dirty[i] = reduce;                                           // NGP_BWD_DEBUG bit 0: never reduce
+                }
+                // weight of corner 2j + h, formed as hash_cell_weights forms it, so that every per-run sum stays bit for bit the same
+                const float dv = f ? df[i].y : df[i].x;
+                const float wx = h ? hc[i].fx : 1.0f - hc[i].fx;
+                const float wy[2] = {1.0f - hc[i].fy, hc[i].fy}, wz[2] = {1.0f - hc[i].fz, hc[i].fz};
+#pragma unroll
+                for (uint32_t j = 0; j < 4; ++j) acc[i][j] = fmaf(dv, (1.0f * wx) * wy[j & 1] * wz[j >> 1], acc[i][j]);
+            }
+        }
+#pragma unroll
+        for (uint32_t i = 0; i < B3_NI; ++i)
+            if (dirty[i]) reduce_slots(idx[i], acc[i]);
+        if (pair + gridDim.x < npairs) named_bar_arrive(B3_EMPTY, B3_EPI_THREADS + 32 * B3_SCATTER_WARPS);
+    }
+}
+
+template <bool FX_ALL>
 __global__ void __launch_bounds__(B3_THREADS, 1)
 network_bwd256_kernel(uint32_t n_max, const uint32_t* __restrict__ n_dev, const float* __restrict__ coords, const __half* __restrict__ enc_save,
                       const NgpLevel* __restrict__ levels, const __half* __restrict__ wd, const __half* __restrict__ wr,
@@ -506,76 +588,7 @@ network_bwd256_kernel(uint32_t n_max, const uint32_t* __restrict__ n_dev, const 
         bwd_chain<1>(smem, tid, n_live, npairs, coords, enc_save, dout, w_part, dwd, dwr, err, dbg, &enc_map, enc_tma);
     } else {
         reg_dealloc<B3_SCATTER_REGS>();
-        // ------------------------------------------------------------------ scatter (HashEncode.h:339-347) of the pair's 256 rows
-        // Item (level, sub) is a run of B3_RUN consecutive samples of one level, walked by a group of 4 adjacent lanes: every lane of the
-        // group reads the same rows, skips the same rows and sees the same cell changes, and accumulates its own 4 (corner, feature) slots
-        // in fp32 registers while the grid cell stays the same.  Lane bit 0 is the feature f, bit 1 picks the corner 2j + h of each
-        // x-neighbour pair (2j, 2j + 1).  At a cell change slot j of the 4 lanes is reduced by one instruction: both features of both
-        // x-neighbours, 32 bytes of the fixed-point copy, which are one aligned sector whenever the pair's entries are 2k and 2k + 1.
-        const uint32_t ts = tid - B3_EPI_THREADS, grp = ts >> 2, f = ts & 1, h = (ts >> 1) & 1;
-        const uint32_t level = grp & 15;                                         // item = grp + k * B3_SCATTER_GROUPS: level = item & 15
-        const NgpLevel lv = s_lv[level];
-        unsigned long long* fx = grid_fx + 2 * (size_t)lv.offset;
-        const uint32_t fx_live = fx_entries > lv.offset ? fx_entries - lv.offset : 0u;     // entries of this level the scratch holds
-        __half2* gg = reinterpret_cast<__half2*>(grid_grad) + lv.offset;
-        // The group's B3_NI items (grp + i * B3_SCATTER_GROUPS) are walked side by side, row k of each in the same iteration: their
-        // shared-memory reads and cell arithmetic are independent, so they overlap instead of adding up.  Each item still sees its rows
-        // in order, so its run sums are the same; only the order of the (integer, order-free) reductions across items changes.
-        uint32_t it = 0;
-        for (uint32_t pair = blockIdx.x; pair < npairs; pair += gridDim.x, ++it) {
-            const uint32_t buf = it & 1;
-            named_bar_sync(B3_FULL, B3_EPI_THREADS + 32 * B3_SCATTER_WARPS);
-            uint32_t cgx[B3_NI], cgy[B3_NI], cgz[B3_NI], idx[B3_NI][4];
-            float acc[B3_NI][4];
-            bool live[B3_NI], dirty[B3_NI];
-#pragma unroll
-            for (uint32_t i = 0; i < B3_NI; ++i) { cgx[i] = 0xffffffffu; cgy[i] = cgz[i] = 0; live[i] = !(dbg & 2); dirty[i] = false; }
-#pragma unroll 1
-            for (uint32_t k = 0; k < B3_RUN; ++k) {
-                float2 df[B3_NI];
-                HashCell hc[B3_NI];
-#pragma unroll
-                for (uint32_t i = 0; i < B3_NI; ++i) {
-                    const uint32_t r = B3_RUN * ((grp + i * B3_SCATTER_GROUPS) >> 4) + k;   // row of the pair: tile r >> 7, row r & 127
-                    live[i] = live[i] && r < 2 * ROWS && 2 * pair * ROWS + r < n_live;        // rows past the pair or the live rows end the run
-                    const uint32_t rc = min(r, 2 * ROWS - 1), T = rc >> 7, p = rc & 127;       // read in bounds either way
-                    const uint8_t* denc = smem + S::tile0 + T * S::tile_stride + B3_G_DENC * GB;
-                    const float* s_coords = reinterpret_cast<const float*>(smem + S::coords + (2 * T + buf) * 3584);
-                    df[i] = __half22float2(*reinterpret_cast<const __half2*>(denc + (size_t)(level >> 2) * GB + p * 16 + (level & 3) * 4));
-                    hc[i] = hash_cell(lv, s_coords[p * 7], s_coords[p * 7 + 1], s_coords[p * 7 + 2]);
-                }
-#pragma unroll
-                for (uint32_t i = 0; i < B3_NI; ++i) {
-                    if (!live[i] || (df[i].x == 0.f && df[i].y == 0.f)) continue;
-                    if (hc[i].gx != cgx[i] || hc[i].gy != cgy[i] || hc[i].gz != cgz[i]) {
-                        if (dirty[i] && !(dbg & 1)) {
-#pragma unroll
-                            for (uint32_t j = 0; j < 4; ++j) red_add_entry_lane(fx, fx_live, gg, idx[i][j], f, acc[i][j]);
-                        }
-                        cgx[i] = hc[i].gx; cgy[i] = hc[i].gy; cgz[i] = hc[i].gz;
-                        uint32_t ci[8];
-                        hash_cell_indices(lv, cgx[i], cgy[i], cgz[i], ci);
-#pragma unroll
-                        for (uint32_t j = 0; j < 4; ++j) { idx[i][j] = h ? ci[2 * j + 1] : ci[2 * j]; acc[i][j] = 0.f; }
-                        dirty[i] = true;
-                    }
-                    // weight of corner 2j + h, formed as hash_cell_weights forms it, so that every per-run sum stays bit for bit the same
-                    const float dv = f ? df[i].y : df[i].x;
-                    const float wx = h ? hc[i].fx : 1.0f - hc[i].fx;
-                    const float wy[2] = {1.0f - hc[i].fy, hc[i].fy}, wz[2] = {1.0f - hc[i].fz, hc[i].fz};
-#pragma unroll
-                    for (uint32_t j = 0; j < 4; ++j) acc[i][j] = fmaf(dv, (1.0f * wx) * wy[j & 1] * wz[j >> 1], acc[i][j]);
-                }
-            }
-#pragma unroll
-            for (uint32_t i = 0; i < B3_NI; ++i) {
-                if (dirty[i] && !(dbg & 1)) {
-#pragma unroll
-                    for (uint32_t j = 0; j < 4; ++j) red_add_entry_lane(fx, fx_live, gg, idx[i][j], f, acc[i][j]);
-                }
-            }
-            if (pair + gridDim.x < npairs) named_bar_arrive(B3_EMPTY, B3_EPI_THREADS + 32 * B3_SCATTER_WARPS);
-        }
+        bwd_scatter<FX_ALL>(smem, tid, n_live, npairs, grid_grad, grid_fx, fx_entries, dbg);
     }
 }
 
@@ -669,20 +682,21 @@ int bwd_scratch(cudaStream_t s, const void* levels_dev, BwdScratch** out) {
 }
 
 // One launch of network_bwd256_kernel: with fx / w_part into the fixed-point scratch and the per-CTA slots, without them straight
-// into grid_grad / dwd / dwr.
+// into grid_grad / dwd / dwr.  fx_all: fx holds every entry of the level table, so the scatter needs no fallback.
 int bwd_launch(cudaStream_t s, uint32_t n_max, const uint32_t* n_dev, const float* coords, const void* enc_save, const void* levels_dev,
                const void* w_density, const void* w_rgb, const void* dout, void* grid_grad, float* dw_density, float* dw_rgb,
-               unsigned long long* fx, uint32_t fx_entries, float* w_part) {
+               unsigned long long* fx, uint32_t fx_entries, bool fx_all, float* w_part) {
     // timing experiments only (results are wrong with any bit set): 1 = no atomics, 2 = no scatter, 4 = no weight-gradient MMAs
     static const uint32_t dbg = getenv("NGP_BWD_DEBUG") ? (uint32_t)atoi(getenv("NGP_BWD_DEBUG")) : 0u;
-    if (ngp_first_use((const void*)network_bwd256_kernel)) NGP_CHECK_CUDA(cudaFuncSetAttribute(network_bwd256_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SmemBwd3::total));
+    const auto kernel = fx_all ? network_bwd256_kernel<true> : network_bwd256_kernel<false>;
+    if (ngp_first_use((const void*)kernel)) NGP_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SmemBwd3::total));
     NgpTensorMap enc_map{};
     static const bool no_tma = getenv("NGP_NO_TMA") != nullptr;           // A/B switch
     const uint32_t enc_tma = (!no_tma && ngp_make_rows32_tensormap(&enc_map, enc_save, n_max)) ? 1u : 0u;
-    network_bwd256_kernel<<<bwd_ctas(n_max), B3_THREADS, SmemBwd3::total, s>>>(n_max, n_dev, coords, (const __half*)enc_save, (const NgpLevel*)levels_dev,
-                                                                              (const __half*)w_density, (const __half*)w_rgb, (const __half*)dout,
-                                                                              (__half*)grid_grad, dw_density, dw_rgb, fx, fx_entries, w_part,
-                                                                              ngp_err_flag(), dbg, enc_map, enc_tma);
+    kernel<<<bwd_ctas(n_max), B3_THREADS, SmemBwd3::total, s>>>(n_max, n_dev, coords, (const __half*)enc_save, (const NgpLevel*)levels_dev,
+                                                               (const __half*)w_density, (const __half*)w_rgb, (const __half*)dout,
+                                                               (__half*)grid_grad, dw_density, dw_rgb, fx, fx_entries, w_part,
+                                                               ngp_err_flag(), dbg, enc_map, enc_tma);
     NGP_LAUNCH_CHECK();
     return 0;
 }
@@ -740,8 +754,10 @@ int ngp_network_bwd(void* stream, uint32_t n_max, const uint32_t* n_dev, const f
     cudaStream_t s = (cudaStream_t)stream;
     BwdScratch* b = nullptr;
     if (int rc = bwd_scratch(s, levels_dev, &b)) return rc;
+    // the scratch is kept per level-table address, and a later table at the same address may hold more entries than it: the
+    // scatter keeps its per-entry test and the f16x2 fallback for them
     if (int rc = bwd_launch(s, n_max, n_dev, coords, enc_save, levels_dev, w_density, w_rgb, dout, grid_grad, dw_density, dw_rgb, b ? b->fx : nullptr,
-                            b ? b->fx_entries : 0u, b ? b->part : nullptr))
+                            b ? b->fx_entries : 0u, false, b ? b->part : nullptr))
         return rc;
     if (b) {
         wgrad_reduce_kernel<<<(W_PART + 255) / 256, 256, 0, s>>>(b->part, bwd_ctas(n_max), dw_density, dw_rgb);
@@ -768,7 +784,7 @@ int ngp_network_bwd_fx(void* stream, uint32_t n_max, const uint32_t* n_dev, cons
                 "ngp_network_bwd_fx: the weight-gradient slots are smaller than ngp_network_bwd_fx_bytes gives");
     if (n_max == 0) return 0;
     return bwd_launch((cudaStream_t)stream, n_max, n_dev, coords, enc_save, levels_dev, w_density, w_rgb, dout, nullptr, nullptr, nullptr,
-                      (unsigned long long*)fx, n_entries, w_part);
+                      (unsigned long long*)fx, n_entries, true, w_part);
 }
 
 }  // extern "C"

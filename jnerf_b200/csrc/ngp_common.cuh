@@ -130,6 +130,47 @@ __device__ __forceinline__ void hash_cell_indices(const NgpLevel& lv, uint32_t g
         }
     }
 }
+// n % d for every 32-bit n and d > 0 without a divide sequence (Lemire, Kaser, Kurz, "Faster remainder by direct computation", 2019):
+// with m = floor((2^64 - 1) / d) + 1, n % d = floor(((m * n) mod 2^64) * d / 2^64).  fastmod_m forms m from 32-bit operations only,
+// since a 64-bit division is a subroutine call, which a kernel that moves registers between warpgroups (setmaxnreg) must not contain.
+__host__ __device__ __forceinline__ uint64_t fastmod_m(uint32_t d) {
+    const uint32_t q_hi = 0xffffffffu / d;
+    uint32_t r = 0xffffffffu - q_hi * d, q_lo = 0;                      // (2^64 - 1) / d = q_hi * 2^32 + (r * 2^32 + 2^32 - 1) / d
+#pragma unroll 1
+    for (int b = 0; b < 32; ++b) {                                       // restoring division by d of the low word, all ones
+        const uint64_t t = ((uint64_t)r << 1) | 1u;                      // < 2d
+        const bool ge = t >= d;
+        r = (uint32_t)(ge ? t - d : t);
+        q_lo = (q_lo << 1) | (ge ? 1u : 0u);
+    }
+    return (((uint64_t)q_hi << 32) | q_lo) + 1;                          // wraps to 0 for d = 1, which fastmod then maps to 0 as it must
+}
+__host__ __device__ __forceinline__ uint32_t fastmod(uint32_t n, uint64_t m, uint32_t d) {
+    const uint64_t lo = m * n;
+    // the high 64 bits of the 96-bit product lo * d, from two 32 x 32 -> 64 multiplies (cannot carry out of 64 bits)
+    return (uint32_t)(((lo >> 32) * d + (((lo & 0xffffffffu) * d) >> 32)) >> 32);
+}
+// The 4 corners 2j + h of the cell (j = 0..3: bit 0 -> +1 in y, bit 1 -> +1 in z) at x-offset h: the entries hash_cell_indices
+// gives for them, formed without the other 4.  m = fastmod_m(lv.size) takes the place of the division on dense levels.
+__device__ __forceinline__ void hash_cell_indices_x(const NgpLevel& lv, uint64_t m, uint32_t gx, uint32_t gy, uint32_t gz, uint32_t h,
+                                                    uint32_t idx[4]) {
+    if (lv.hashed) {
+        const uint32_t mask = lv.size - 1, hx = (gx + h) * lv.prime[0];
+        const uint32_t hy0 = gy * lv.prime[1], hy1 = (gy + 1) * lv.prime[1];
+        const uint32_t hz0 = gz * lv.prime[2], hz1 = (gz + 1) * lv.prime[2];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) idx[j] = (hx ^ ((j & 1) ? hy1 : hy0) ^ ((j & 2) ? hz1 : hz0)) & mask;
+    } else {
+        const uint32_t res = lv.resolution, res2 = res * res;
+        const uint32_t b = fastmod(gx + gy * res + gz * res2, m, lv.size) + h;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            uint32_t v = b + ((j & 1) ? res : 0u) + ((j & 2) ? res2 : 0u);
+            v -= (v >= lv.size) ? lv.size : 0u;
+            idx[j] = v;
+        }
+    }
+}
 // A full-occupancy scatter is bound by the number of L2 reduction REQUESTS (one per lane and instruction), not by bytes.  Corners c and
 // c+1 of a cell are x-neighbours: whenever their entries share an aligned 8-byte word -- dense levels: even index; hashed levels:
 // even x, because (x+1) ^ h = (x ^ h) ^ 1 then -- one REDG.F16x4 serves both.  Half of all cells qualify, i.e. 6 requests per cell
