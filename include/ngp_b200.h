@@ -366,6 +366,15 @@ int ngp_render_march_round(void* stream, uint32_t n_rays, uint32_t capacity, voi
 int ngp_render_composite_round(void* stream, uint32_t n_rays, uint32_t capacity, void* workspace, uint32_t n_alive, uint32_t k_steps,
                                float min_transmittance, uint32_t cascades, float* rgb_out, float* alpha_out, uint32_t* n_samples_out,
                                uint32_t* n_alive_host);
+/* V5: ngp_render_composite_round that also accumulates depth_out[g] += w_i * t_i over the samples it composites: the same weights
+ * w_i = alpha_i * T_i, the same samples in the same order and the same stopping rule, with t_i the sample's ray parameter in model (NGP)
+ * units.  The reference has no counterpart (its renderer returns colour only); the convention is pixelNeRF's depth_map = sum(w * z)
+ * (render_rays), unnormalised: divide by alpha and by the dataset's scale for the expected distance in NeRF world units.  The caller zeroes
+ * depth_out (n_rays floats) before the first round; rays that miss the box are never composited and keep 0.  Call it in place of V4 in
+ * every round of a frame; rgb, alpha and sample counts are bit-identical to V4's.  A NULL depth_out is an error. */
+int ngp_render_composite_round_depth(void* stream, uint32_t n_rays, uint32_t capacity, void* workspace, uint32_t n_alive, uint32_t k_steps,
+                                     float min_transmittance, uint32_t cascades, float* rgb_out, float* alpha_out, uint32_t* n_samples_out,
+                                     float* depth_out, uint32_t* n_alive_host);
 
 /* ---- R10 occupancy-grid maintenance (DGS/density_grid_sampler.py:204-264 + five headers) ------------- */
 int ngp_grid_mark_untrained(void* stream, uint32_t n_elements, float* grid, uint32_t n_images, const float* focal_lengths,

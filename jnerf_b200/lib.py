@@ -75,6 +75,7 @@ SIGNATURES = {
     "ngp_render_init": (_i32, [_vp, _u32, _u32, _vp, _f32, _f32, _vp, _vp, _f32, _f32, _u32, _i32, _u64, _u64, _u32, _vp, _vp, _vp, _vp]),
     "ngp_render_march_round": (_i32, [_vp, _u32, _u32, _vp, _u32, _u32, _f32, _f32, _vp, _vp, _vp, _f32, _u32, _i32]),
     "ngp_render_composite_round": (_i32, [_vp, _u32, _u32, _vp, _u32, _u32, _f32, _u32, _vp, _vp, _vp, _vp]),
+    "ngp_render_composite_round_depth": (_i32, [_vp, _u32, _u32, _vp, _u32, _u32, _f32, _u32, _vp, _vp, _vp, _vp, _vp]),
     "ngp_march_workspace_bytes": (_u64, [_u32]),
     "ngp_march": (_i32, [_vp, _u32, _f32, _f32, _u32, _vp, _vp, _vp, _f32, _f32, _u32, _i32, _u64, _u64, _vp, _vp, _vp, _vp, _vp]),
     "ngp_compact": (_i32, [_vp, _u32, _u32, _vp, _vp, _vp, _vp, _vp, _i32]),
@@ -111,7 +112,7 @@ KERNELS_PER_CALL = {
     "ngp_grid_generate_samples": 1, "ngp_grid_splat": 1, "ngp_grid_ema": 1, "ngp_grid_update_bitfield": 7, "ngp_adam_ema": 1, "ngp_dp_exchange_step": 1, "ngp_dp_exchange_wait": 1, "ngp_raygen": 1, "ngp_prepare_batch": 1,
     "ngp_blend_target": 1,
     "ngp_density_lattice": 1, "ngp_nerf_density_lattice": 1, "ngp_marching_cubes": 3, "ngp_mesh_largest_component": 18, "ngp_mesh_vertex_normals": 7,
-    "ngp_render_init": 3, "ngp_render_march_round": 3, "ngp_render_composite_round": 3,
+    "ngp_render_init": 3, "ngp_render_march_round": 3, "ngp_render_composite_round": 3, "ngp_render_composite_round_depth": 3,
     "ngp_nerf_fwd": 1, "ngp_nerf_density": 1, "ngp_nerf_bwd": 3,
     "ngp_mip_rays": 1, "ngp_mip_sample": 1, "ngp_mip_resample": 1, "ngp_mip_encode": 1, "ngp_mip_fwd": 1, "ngp_mip_composite_fwd": 1,
     "ngp_mip_composite_loss_bwd": 1, "ngp_mip_rays_multi": 1, "ngp_mip_encode_deg": 1, "ngp_mip_fwd_deg": 1,

@@ -477,7 +477,7 @@ def mesh_smooth(field, method="auto", max_iters=250, workspace=None):
     return out, dict(method=SMOOTH_METHODS[int(info[0])], iterations=int(info[1]), band_variables=int(info[2]))
 
 
-# ---- whole-frame renderer with early ray termination (include/ngp_b200.h V1-V4) ----
+# ---- whole-frame renderer with early ray termination (include/ngp_b200.h V1-V5) ----
 RENDER_CAPACITY = 1 << 22          # default rows per round: 4 Mi rows = 112 MB of coordinates + 32 MB of network outputs
 RENDER_MAX_K = 64
 
@@ -505,12 +505,14 @@ def render_workspace(n_rays, workspace=None, capacity=RENDER_CAPACITY):
 
 
 def render_rays(rays_o, rays_d, bitfield, aabb, cone_angle, near, cascades, const_dt, rng, grid, levels, wd, wr, jitter_tile,
-                min_transmittance=0.0, capacity=RENDER_CAPACITY, workspace=None, net=None):
+                min_transmittance=0.0, capacity=RENDER_CAPACITY, workspace=None, net=None, depth=False):
     """Render R rays (model space) to (rgb (R,3) without background, alpha (R,1) = 1 - T, n_samples (R,) int32, rounds).
     Each ray composites the samples ngp_march gives it under the jitter layout of `jitter_tile`-ray tiles, in order, and stops after the
     first sample that brings its transmittance below `min_transmittance` (0: never).  `rng` is not advanced here: the caller moves it
     on by ceil(R / jitter_tile) * 2^32, as the tiled renderer would.  One 4-byte read-back per round.
-    net: the network as net(rows, n_dev, out) instead of the fused NGP network of (grid, levels, wd, wr), e.g. OriginNeRFNetworks.infer."""
+    net: the network as net(rows, n_dev, out) instead of the fused NGP network of (grid, levels, wd, wr), e.g. OriginNeRFNetworks.infer.
+    depth: also return depth (R,) float32 = sum(w t) over the composited samples, t in model units along rays_d (0 for rays that miss
+    the box), as a fifth element; the other four are bit-identical to those of depth=False."""
     import ctypes
     R, dev = rays_o.shape[0], rays_o.device
     nbytes, off_rows, off_net, off_cnt = render_workspace_layout(R, capacity)
@@ -522,6 +524,7 @@ def render_rays(rays_o, rays_d, bitfield, aabb, cone_angle, near, cascades, cons
     rgb = torch.empty((R, 3), dtype=torch.float32, device=dev)
     alpha = torch.empty((R, 1), dtype=torch.float32, device=dev)
     n_samples = torch.empty(R, dtype=torch.int32, device=dev)
+    depth_out = torch.zeros(R, dtype=torch.float32, device=dev) if depth else None
     alive = np.zeros(1, np.uint32)
     ap = alive.ctypes.data_as(ctypes.c_void_p)
     lib.call("ngp_render_init", _stream(), R, int(capacity), _p(workspace), float(aabb[0]), float(aabb[1]), _p(rays_o), _p(rays_d), float(cone_angle),
@@ -537,9 +540,15 @@ def render_rays(rays_o, rays_d, bitfield, aabb, cone_angle, near, cascades, cons
             network_fwd(rows[:bound], grid, levels, wd, wr, n_dev=n_rows, save_enc=False, out=out_rows[:bound])
         else:
             net(rows[:bound], n_rows, out_rows[:bound])
-        lib.call("ngp_render_composite_round", _stream(), R, int(capacity), _p(workspace), n_alive, k, float(min_transmittance), int(cascades),
-                 _p(rgb), _p(alpha), _p(n_samples), ap)
+        if depth:
+            lib.call("ngp_render_composite_round_depth", _stream(), R, int(capacity), _p(workspace), n_alive, k, float(min_transmittance),
+                     int(cascades), _p(rgb), _p(alpha), _p(n_samples), _p(depth_out), ap)
+        else:
+            lib.call("ngp_render_composite_round", _stream(), R, int(capacity), _p(workspace), n_alive, k, float(min_transmittance),
+                     int(cascades), _p(rgb), _p(alpha), _p(n_samples), ap)
         rounds += 1
+    if depth:
+        return rgb, alpha, n_samples, rounds, depth_out
     return rgb, alpha, n_samples, rounds
 
 

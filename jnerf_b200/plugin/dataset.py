@@ -239,6 +239,7 @@ class LLFFDataset(_RayBatcher):
         self._cx, self._cy = self.W / 2, self.H / 2                                                                   # :106-107
         poses = poses[:, :3, :4].astype(np.float32)
         self.poses = [poses[i].copy() for i in self.i_select]                                  # NeRF camera-to-world, recentred and rescaled
+        self.bounds = bds[self.i_select]                                # (n, 2) near / far of each view, rescaled like the poses (path_spiral)
         self._xforms = [matrix_nerf2ngp(p, self.scale, self.offset, self.correct_pose) for p in self.poses]
         imgs = [first if i == 0 else read(files[i]) for i in self.i_select]
         self.image_data = torch.from_numpy(np.stack(imgs)).to(DEVICE).reshape(len(imgs), self.H * self.W, -1)

@@ -589,11 +589,12 @@ class Runner:
 
     # ------------------------------------------------------------------------------------------ rendering (runner.py:86-121, 162-264)
     @torch.no_grad()
-    def render_rays(self, rays_o, rays_d, min_transmittance=1e-4):
+    def render_rays(self, rays_o, rays_d, min_transmittance=1e-4, depth=False):
         """Whole-frame renderer (ops.render_rays): every ray at once in rounds, each ray dropped after the first sample that brings its
         transmittance below min_transmittance (0: never, and then every ray composites the samples render_img_nosync gives it).  The
         jitter and the sampler rng advance exactly as render_img_nosync's n_rays_per_batch tiles would have them.
-        Returns (rgb (R,3) without background, alpha (R,1), n_samples (R,), rounds).
+        Returns (rgb (R,3) without background, alpha (R,1), n_samples (R,), rounds); with depth=True also the weighted sum of the
+        samples' ray parameters, sum(w t) (R,) in model units (depth_from_sum turns it into a distance).
         The renderer's workspace (per-ray state, and 144 MB of round rows and network outputs at the default capacity) is kept for the
         next frame; render() and test() release it when they finish, and release_render_workspace() does so at any time."""
         assert self._can_infer, "render_rays needs the fused NGP model or a model with an inference forward (infer)"
@@ -604,12 +605,13 @@ class Runner:
         self._render_ws = ops.render_workspace(R, self._render_ws)
         args = (rays_o.contiguous(), rays_d.contiguous(), s.density_grid_bitfield, s.aabb_range, s.cone_angle_constant, s.near_distance,
                 s.NERF_CASCADES, s.const_dt, s.rng)
+        kw = {"depth": True} if depth else {}
         if self.fast:
             out = ops.render_rays(*args, m.pos_encoder.m_grid, m.pos_encoder.levels, m.density_mlp.con_weights, m.rgb_mlp.con_weights, tile,
-                                  min_transmittance=min_transmittance, workspace=self._render_ws)
+                                  min_transmittance=min_transmittance, workspace=self._render_ws, **kw)
         else:
             out = ops.render_rays(*args, None, None, None, None, tile, min_transmittance=min_transmittance, workspace=self._render_ws,
-                                  net=m.infer)
+                                  net=m.infer, **kw)
         ops.pcg32_advance(s.rng, ((R + tile - 1) // tile) << 32)       # one rng.advance() per tile (ray_sampler.py:61)
         return out
 
@@ -617,12 +619,17 @@ class Runner:
         """Free the whole-frame renderer's workspace (the next render_rays allocates a new one), e.g. before training on."""
         self._render_ws = None
 
-    def _render_frame(self, rays_o, rays_d, W, H, min_transmittance):
-        """(img (H,W,3) with the background blended in unless alpha_image, alpha (H,W,1), n_samples (H,W), rounds)"""
-        rgb, alpha, n, rounds = self.render_rays(rays_o, rays_d, min_transmittance)
+    def _render_frame(self, rays_o, rays_d, W, H, min_transmittance, depth_scale=None):
+        """(img (H,W,3) with the background blended in unless alpha_image, alpha (H,W,1), n_samples (H,W), rounds); with a
+        depth_scale (the scale of the dataset the rays come from) also depth (H,W) in NeRF world units, from the same render."""
+        if depth_scale:
+            rgb, alpha, n, rounds, S = self.render_rays(rays_o, rays_d, min_transmittance, depth=True)
+        else:
+            rgb, alpha, n, rounds = self.render_rays(rays_o, rays_d, min_transmittance)
         if not getattr(self.cfg, "alpha_image", False):
             rgb = rgb + torch.tensor(self.background_color, dtype=torch.float32, device=rgb.device) * (1 - alpha)
-        return rgb.reshape(H, W, 3), alpha.reshape(H, W, 1), n.reshape(H, W), rounds
+        frame = (rgb.reshape(H, W, 3), alpha.reshape(H, W, 1), n.reshape(H, W), rounds)
+        return frame + (depth_from_sum(S, alpha, depth_scale).reshape(H, W),) if depth_scale else frame
 
     def pose_rays(self, pose):
         """generate_rays_with_pose (dataset.py:236-253): the rays of every pixel, row-major, of a camera at `pose` (3x4 or 4x4 NeRF
@@ -645,6 +652,31 @@ class Runner:
         o, d = self.pose_rays(pose)
         return self._render_frame(o, d, W, H, min_transmittance)[0]
 
+    @torch.no_grad()
+    def render_depth_with_pose(self, pose, min_transmittance=1e-4):
+        """render_img_with_pose with the depth map of the same render: (img (H,W,3), depth (H,W), alpha (H,W,1)), depth in NeRF world
+        units as depth_from_sum defines it (0 where alpha is 0)."""
+        ds = self.dataset["train"]
+        W, H = ds.resolution
+        o, d = self.pose_rays(pose)
+        img, alpha, _, _, depth = self._render_frame(o, d, W, H, min_transmittance, depth_scale=float(ds.scale))
+        return img, depth, alpha
+
+    def depth_range(self, poses, ds=None):
+        """(near, far) in NeRF world units for the grey scale of depth images (depth_to_grey): the capture's bounds for a dataset that
+        carries them (LLFFDataset.bounds), else the nearest and the farthest distance from any of the cameras `poses` (NeRF
+        camera-to-world) to the scene's box (the sampler's aabb)."""
+        from .plugin.dataset import matrix_nerf2ngp
+        ds = self.dataset["train"] if ds is None else ds
+        if getattr(ds, "bounds", None) is not None:
+            return float(np.min(ds.bounds)), float(np.max(ds.bounds))
+        lo, hi = (float(v) for v in self.sampler.aabb_range)
+        cp = getattr(ds, "correct_pose", (1, -1, -1))
+        org = np.stack([matrix_nerf2ngp(np.asarray(p, np.float32)[:3, :4], ds.scale, ds.offset, cp)[:, 3] for p in poses]).astype(np.float64)
+        near = np.linalg.norm(org - np.clip(org, lo, hi), axis=1).min()
+        far = np.linalg.norm(np.maximum(np.abs(org - lo), np.abs(org - hi)), axis=1).max()
+        return float(near / ds.scale), float(far / ds.scale)
+
     def _save_path(self):
         return os.path.join(self.cfg.log_dir or ".", self.cfg.exp_name or "exp")
 
@@ -659,9 +691,13 @@ class Runner:
         Image.fromarray((img * 255 + 0.5).clip(0, 255).astype(np.uint8)).save(path)
 
     @torch.no_grad()
-    def render(self, save_path=None, load_ckpt=False, min_transmittance=1e-4):
+    def render(self, save_path=None, load_ckpt=False, min_transmittance=1e-4, depth=False, poses=None):
         """runner.py:101-121: the 80-frame spherical camera path (utils/camera_path.py) as an mp4 (OpenCV, mp4v, 28 fps), by default
-        log_dir/exp_name/demo.mp4.  Returns the path."""
+        log_dir/exp_name/demo.mp4.  Returns the path.
+        poses: another camera path (NeRF camera-to-world matrices), e.g. utils.camera_path.path_spiral for a forward-facing capture.
+        depth: also write the depth video of the same frames beside it ({stem}_depth.mp4, e.g. demo_depth.mp4), grey = alpha *
+        clip((far - depth) / (far - near), 0, 1) with one (near, far) for the whole video, depth_range(poses): nearer is brighter and a
+        shade is the same distance in every frame; empty pixels are black."""
         try:
             import cv2
         except ImportError as e:
@@ -675,22 +711,35 @@ class Runner:
             raise ValueError(f"Runner.render: the video path must end in .mp4, got {save_path}")
         os.makedirs(os.path.dirname(os.path.abspath(save_path)), exist_ok=True)
         W, H = self.dataset["train"].resolution
-        writer = cv2.VideoWriter(str(save_path), cv2.VideoWriter_fourcc(*"mp4v"), 28, (W, H))
+        poses = path_spherical() if poses is None else list(poses)
+        fourcc = cv2.VideoWriter_fourcc(*"mp4v")
+        writer = cv2.VideoWriter(str(save_path), fourcc, 28, (W, H))
+        depth_writer = cv2.VideoWriter(str(save_path)[:-4] + "_depth.mp4", fourcc, 28, (W, H)) if depth else None
         try:
-            for pose in path_spherical():
-                img = self.render_img_with_pose(pose, min_transmittance)
+            near, far = self.depth_range(poses) if depth else (0.0, 0.0)
+            for pose in poses:
+                if depth:
+                    img, dep, alpha = self.render_depth_with_pose(pose, min_transmittance)
+                    g = depth_to_grey(dep, alpha, near, far)
+                    depth_writer.write(np.ascontiguousarray(np.repeat(g[..., None], 3, -1)))
+                else:
+                    img = self.render_img_with_pose(pose, min_transmittance)
                 u8 = (img.cpu().numpy() * 255 + 0.5).clip(0, 255).astype(np.uint8)
                 writer.write(np.ascontiguousarray(u8[..., ::-1]))    # OpenCV takes BGR: the file shows the true colours (DESIGN.md section 7)
         finally:
             writer.release()
+            if depth_writer is not None:
+                depth_writer.release()
             self.release_render_workspace()
         return save_path
 
     @torch.no_grad()
-    def render_test(self, save_img=True, save_path=None, min_transmittance=1e-4):
+    def render_test(self, save_img=True, save_path=None, min_transmittance=1e-4, depth=False):
         """runner.py:162-178: every view of the test split on the whole-frame renderer; saves {exp_name}_r_{i}.png (RGBA when
         alpha_image is set) and, when the split has images, {exp_name}_gt_{i}.png; returns the per-view mse against the target with the
-        background blended in (an empty list for a split without images, as the reference computes no PSNR then)."""
+        background blended in (an empty list for a split without images, as the reference computes no PSNR then).
+        depth: with save_img also {exp_name}_depth_{i}.npy (float32 (H,W), NeRF world units, depth_from_sum) and {exp_name}_depth_{i}.png
+        (8-bit grey, nearer is brighter, one depth_range over the test views, as in render's depth video), from the same render."""
         ds = self.dataset["test"]
         save_path = self._save_path() if save_path is None else save_path
         if save_img:
@@ -698,12 +747,20 @@ class Runner:
         exp = self.cfg.exp_name
         W, H = ds.resolution
         have_img = getattr(ds, "have_img", True)
+        near, far = self.depth_range(ds.poses, ds) if depth else (0.0, 0.0)
         mse = []
         for i in range(ds.n_images):
             o, d = ds.generate_rays_total_test(i)
-            img, alpha, _, _ = self._render_frame(o, d, W, H, min_transmittance)
+            if depth:
+                img, alpha, _, _, dep = self._render_frame(o, d, W, H, min_transmittance, depth_scale=float(ds.scale))
+            else:
+                img, alpha, _, _ = self._render_frame(o, d, W, H, min_transmittance)
             if save_img:
                 self.save_img(os.path.join(save_path, f"{exp}_r_{i}.png"), img, alpha if getattr(self.cfg, "alpha_image", False) else None)
+                if depth:
+                    from PIL import Image
+                    np.save(os.path.join(save_path, f"{exp}_depth_{i}.npy"), dep.cpu().numpy().astype(np.float32))
+                    Image.fromarray(depth_to_grey(dep, alpha, near, far), "L").save(os.path.join(save_path, f"{exp}_depth_{i}.png"))
             if not have_img:                                          # runner.py:173: no target, no gt image, no mse
                 continue
             tar = self._target_img(ds, i)
@@ -713,15 +770,16 @@ class Runner:
         return mse
 
     @torch.no_grad()
-    def test(self, load_ckpt=False, min_transmittance=1e-4):
+    def test(self, load_ckpt=False, min_transmittance=1e-4, depth=False):
         """runner.py:86-99: render the test split into log_dir/exp_name/test and print the mean test PSNR, which is returned (None for
-        a split without images, as the reference prints none then).  Releases the renderer's workspace when done."""
+        a split without images, as the reference prints none then).  depth: also the depth maps of the views (render_test).  Releases
+        the renderer's workspace when done."""
         if load_ckpt:
             self.load_ckpt(self.cfg.ckpt_path)
         if self.dataset["test"] is None:
             self.dataset["test"] = build_from_cfg(self.cfg.dataset.test, DATASETS)
         try:
-            mse = self.render_test(save_path=os.path.join(self._save_path(), "test"), min_transmittance=min_transmittance)
+            mse = self.render_test(save_path=os.path.join(self._save_path(), "test"), min_transmittance=min_transmittance, depth=depth)
         finally:
             self.release_render_workspace()
         if not getattr(self.dataset["test"], "have_img", True):
@@ -887,6 +945,25 @@ class Runner:
             self._slice_param.copy_(self._table[self._lo:self._hi])
         self.optimizer._nested_optimizer.load_state_dict(nested)
         self.ema_optimizer.load_state_dict(ck["ema_optimizer"])
+
+
+def depth_from_sum(S, alpha, scale):
+    """The depth of a pixel from the renderer's sum S = sum(w t) (Runner.render_rays(depth=True)): the opacity-normalised expected
+    distance along the ray, S / (scale * alpha), in NeRF world units, and 0 where alpha is 0.  Rays are unit length in model space and
+    matrix_nerf2ngp scales positions but not rotations, so a model-space t is t / scale NeRF units; `scale` is the dataset's (0.33 by
+    default, set by the config for some scenes).  Mip-NeRF's `distance` (mip_sampler.cu) normalises the same way but also clips to the
+    sampled interval; this does not."""
+    a = alpha.reshape(S.shape)
+    return torch.where(a > 0, S / (float(scale) * a), torch.zeros_like(S))
+
+
+def depth_to_grey(depth, alpha, near, far):
+    """8-bit grey image of a depth map: alpha * clip((far - depth) / (far - near), 0, 1), so nearer is brighter and empty pixels are
+    black.  depth (H,W), alpha (H,W,1) or (H,W) -> (H,W) uint8."""
+    d = depth.float().cpu().numpy()
+    a = alpha.float().cpu().numpy().reshape(d.shape)
+    g = a * np.clip((far - d) / max(far - near, 1e-12), 0.0, 1.0)
+    return (g * 255 + 0.5).clip(0, 255).astype(np.uint8)
 
 
 def lego_cfg(fp16=True, synthetic=True, **over):

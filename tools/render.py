@@ -1,21 +1,28 @@
 #!/usr/bin/env python
 """Render a trained model on the whole-frame renderer (Runner.render_rays): one view, the camera-path video or the test split.
 
-    python tools/render.py --ckpt CKPT (--config-file CFG | --workload lego|fox) --task pose|video|test [--min-transmittance 1e-4] [--out DIR]
+    python tools/render.py --ckpt CKPT (--config-file CFG | --workload lego|fox|llff) --task pose|video|test [--min-transmittance 1e-4] [--out DIR]
     python tools/render.py --workload lego --train-steps 3000 --task test --compare
+    python tools/render.py --workload llff --train-steps 2000 --task video --path spiral --depth
 
 --ckpt takes this project's .pt checkpoints or the reference's params.pkl.  Without --ckpt, --train-steps trains the stand-in first
 (the configuration of tools/train_psnr.py).  --task pose renders the first training view's pose, video the 80-frame spherical path
 (DIR/demo.mp4), test every test view (PNGs in DIR, mean PSNR).  Prints one JSON line: frames, W, H, per-frame ms between CUDA events
 recorded before and after each frame (median, min, max; for the whole-frame renderer this includes the host read-back of the alive
 count after every round), rounds and mean composited samples per pixel.  --compare also times render_img_nosync and the renderer at
-min_transmittance 0 on the same views with the same jitter, the three alternating frame by frame."""
+min_transmittance 0 on the same views with the same jitter, the three alternating frame by frame.  --depth also renders depth maps:
+the video gains DIR/demo_depth.mp4 and its timing is of the depth renders; pose and test render every view with and without depth,
+alternating, write the depth maps ({exp}_depth_{i}.npy / .png, pose_depth.*) and add the depth-on timing to the JSON line.  --path
+spiral flies the spiral of a forward-facing capture (utils/camera_path.path_spiral) instead of the spherical path; it needs a dataset
+with near / far bounds (LLFF).  --workload llff is the forward-facing stand-in of tools/train_psnr.py, written to a temporary directory."""
 import argparse
 import json
 import os
 import statistics
 import sys
 import time
+
+import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
@@ -28,7 +35,7 @@ def summary(ms):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--config-file", default="", help="a JNeRF config (projects/ngp/configs/*.py)")
-    ap.add_argument("--workload", default="lego", choices=["lego", "fox"], help="the synthetic stand-ins, as in tools/train_psnr.py")
+    ap.add_argument("--workload", default="lego", choices=["lego", "fox", "llff"], help="the synthetic stand-ins, as in tools/train_psnr.py")
     ap.add_argument("--ckpt", default=None, help=".pt checkpoint of this project or the reference's .pkl")
     ap.add_argument("--train-steps", type=int, default=0, help="without --ckpt: train the stand-in for this many steps first")
     ap.add_argument("--images", type=int, default=100)
@@ -36,22 +43,33 @@ def main():
     ap.add_argument("--task", default="test", choices=["pose", "video", "test"])
     ap.add_argument("--min-transmittance", type=float, default=1e-4)
     ap.add_argument("--compare", action="store_true", help="also time render_img_nosync and min_transmittance 0, alternating")
+    ap.add_argument("--depth", action="store_true", help="also render depth maps (and time them)")
+    ap.add_argument("--path", default="spherical", choices=["spherical", "spiral"], help="camera path of --task video")
     ap.add_argument("--out", default="render_out")
     args = ap.parse_args()
     if args.compare and args.task == "video":
         ap.error("--compare needs --task pose or test (render_img_nosync renders dataset views)")
+    if args.path != "spherical" and args.task != "video":
+        ap.error("--path is the camera path of --task video")
 
     import torch
     from jnerf_b200 import lib, plugin  # noqa: F401
     from jnerf_b200.plugin import losses as L
-    from jnerf_b200.runner import Runner, fox_cfg, lego_cfg
+    from jnerf_b200.runner import Runner, fox_cfg, lego_cfg, llff_cfg
     from jnerf_b200.utils.config import get_cfg, init_cfg, update_cfg
     from jnerf_b200.utils.registry import DATASETS, build_from_cfg
 
     lib.load()
     get_cfg().clear()
+    tmp = None
     if args.config_file:
         init_cfg(args.config_file)
+    elif args.workload == "llff":
+        import tempfile
+        from jnerf_b200.plugin.dataset import write_synthetic_llff
+        tmp = tempfile.TemporaryDirectory()
+        write_synthetic_llff(tmp.name, n_images=args.images if args.images != 100 else 20, H=8 * 192, W=8 * 256)   # read at 192 x 256
+        update_cfg(**llff_cfg(tmp.name, fp16=True, seed=1))
     elif args.workload == "fox":
         update_cfg(**fox_cfg(fp16=True, synthetic=True, seed=1))
         get_cfg().dataset.val = None
@@ -79,11 +97,18 @@ def main():
     if args.task == "video":
         ms, rounds, spp = [], [], []
         real = runner.render_rays
+        poses = None
+        if args.path == "spiral":
+            from jnerf_b200.utils.camera_path import path_spiral
+            tr = runner.dataset["train"]
+            if getattr(tr, "bounds", None) is None:
+                sys.exit(f"--path spiral needs a forward-facing capture with near / far bounds (LLFFDataset); {type(tr).__name__} has none")
+            poses = path_spiral(tr.poses, tr.bounds)
 
-        def timed(o, d, m):                                          # per frame: raygen + every round, CUDA events
+        def timed(o, d, m, **kw):                                    # per frame: raygen + every round, CUDA events
             a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             a.record()
-            out = real(o, d, m)
+            out = real(o, d, m, **kw)
             b.record()
             b.synchronize()
             ms.append(a.elapsed_time(b))
@@ -91,10 +116,10 @@ def main():
             spp.append(float(out[2].float().mean()))
             return out
         runner.render_rays = timed
-        path = runner.render(save_path=os.path.join(args.out, "demo.mp4"), min_transmittance=eps)
+        path = runner.render(save_path=os.path.join(args.out, "demo.mp4"), min_transmittance=eps, depth=args.depth, poses=poses)
         W, H = runner.dataset["train"].resolution
         row.update(frames=len(ms), W=W, H=H, ms=summary(ms), rounds=round(statistics.mean(rounds), 2), spp=round(statistics.mean(spp), 3),
-                   out=os.path.abspath(path))
+                   out=os.path.abspath(path), path=args.path, depth=args.depth)
     else:
         if args.task == "test":
             if runner.dataset["test"] is None:
@@ -106,7 +131,7 @@ def main():
             views = [0]
         W, H = ds.resolution
         bgc = torch.tensor(runner.background_color, dtype=torch.float32, device="cuda")
-        variants = [("new", eps)] + ([("eps0", 0.0), ("nosync", None)] if args.compare else [])
+        variants = [("new", eps)] + ([("depth", eps)] if args.depth else []) + ([("eps0", 0.0), ("nosync", None)] if args.compare else [])
         res = {k: dict(ms=[], rounds=[], spp=[], psnr=[]) for k, _ in variants}
 
         def run(kind, m, i):
@@ -117,11 +142,19 @@ def main():
                 o, d = runner.pose_rays(ds.poses[i])
             else:
                 o, d = ds.generate_rays_total_test(i)
-            img, _, n, rounds = runner._render_frame(o, d, W, H, m)
+            if kind == "depth":
+                img, alpha, n, rounds, dep = runner._render_frame(o, d, W, H, m, depth_scale=float(ds.scale))
+            else:
+                img, alpha, n, rounds = runner._render_frame(o, d, W, H, m)
+                dep = None
             tar = ds.rgba_for(torch.arange(H * W, device="cuda", dtype=torch.int32) + i * H * W)
             tar = (tar[:, :3] * tar[:, 3:] + bgc * (1 - tar[:, 3:])).reshape(H, W, 3)
-            return img, tar, (n, rounds)
+            return img, tar, (n, rounds, dep, alpha)
 
+        if args.depth:
+            from PIL import Image
+            from jnerf_b200.runner import depth_to_grey
+            near, far = runner.depth_range([ds.poses[i] for i in views], ds)
         rng0 = s.rng.copy()
         for kind, m in variants:                                     # warm-up: modules, allocations
             s.rng[:] = rng0
@@ -146,10 +179,19 @@ def main():
                     runner.save_img(os.path.join(args.out, f"{runner.cfg.exp_name}_gt_{i}.png"), tar)
                 elif kind == "new":
                     runner.save_img(os.path.join(args.out, "pose.png"), img)
+                elif kind == "depth":
+                    stem = os.path.join(args.out, f"{runner.cfg.exp_name}_depth_{i}" if args.task == "test" else "pose_depth")
+                    np.save(stem + ".npy", extra[2].cpu().numpy())
+                    Image.fromarray(depth_to_grey(extra[2], extra[3], near, far), "L").save(stem + ".png")
             rng0 = s.rng.copy()
         new = res["new"]
         row.update(frames=len(views), W=W, H=H, ms=summary(new["ms"]), rounds=round(statistics.mean(new["rounds"]), 2),
                    spp=round(statistics.mean(new["spp"]), 3), psnr=round(statistics.mean(new["psnr"]), 3))
+        if args.depth:
+            dp = res["depth"]
+            over = [x - y for x, y in zip(dp["ms"], new["ms"])]
+            row["depth"] = dict(ms=summary(dp["ms"]), overhead_ms=summary(over), psnr=round(statistics.mean(dp["psnr"]), 3),
+                                near_far=[round(near, 4), round(far, 4)])
         if args.compare:
             e0, ns = res["eps0"], res["nosync"]
             row["compare"] = {"eps0": dict(ms=summary(e0["ms"]), rounds=round(statistics.mean(e0["rounds"]), 2),
@@ -157,6 +199,8 @@ def main():
                               "render_img_nosync": dict(ms=summary(ns["ms"]), psnr=round(statistics.mean(ns["psnr"]), 3))}
     row.update(wall_s=round(time.perf_counter() - t0, 3), gpu=torch.cuda.get_device_name(0), timeout_flag=int(lib.load().ngp_debug_timeout_flag()))
     print(json.dumps(row), flush=True)
+    if tmp is not None:
+        tmp.cleanup()
 
 
 if __name__ == "__main__":
