@@ -115,6 +115,14 @@ int ngp_network_bwd_fx(void* stream, uint32_t n_max, const uint32_t* n_dev, cons
 /* NGPNetworks.density (ngp_network.py:86-89): pos (n,3) f32 -> sigma_raw (n) fp16 */
 int ngp_density_fwd(void* stream, uint32_t n, const float* pos, const void* grid, const void* levels_dev,
                     const void* w_density, void* sigma_out);
+/* The gradient of sigma_raw (the density MLP's first output, before exp) with respect to the position row[0:3] of NerfCoordinate rows
+ * coords (n_max,7) f32 -> grad_out (n_max,3) f32, for normal maps (V6).  The reference has no counterpart (it differentiates the density
+ * only with respect to the table and the weights).  Per row, sum over levels of J_l^T dsigma/denc_l: J_l the 2x3 derivative of level l's
+ * trilinear interpolation, dsigma/denc = W0d^T (relu'(hd) .* Woutd[0, :]), with the ReLU mask of the forward's own fp16 density layer 0
+ * (hd is formed as ngp_network_fwd forms it, bit for bit) and everything else in fp32.  Hashed and dense levels alike.  n_dev as for
+ * ngp_network_fwd: rows at or past it are not written.  A NULL coords, grid, levels, w_density or grad_out with n_max > 0 is an error. */
+int ngp_density_grad(void* stream, uint32_t n_max, const uint32_t* n_dev, const float* coords, const void* grid, const void* levels_dev,
+                     const void* w_density, float* grad_out);
 
 /* ---- F1-F4  vanilla NeRF: FrequencyEncoder + OriginNeRFNetworks (position_encoders/freq_encoder/freq_encoder.py:22-50,
  * models/networks/ori_nerf_network.py:10-70), csrc/nerf_mlp.cu, DESIGN.md section 10 ---------------------------------------------
@@ -338,7 +346,7 @@ int ngp_composite_loss_bwd(void* stream, uint32_t n_rays, uint32_t n_elements, c
                            const float* target, float huber_delta, const float* density_grid_mean, uint32_t cascades,
                            float* rgb_out, float* loss_out, void* dnet_out, float reg_scale);
 
-/* ---- V1-V4  whole-frame renderer with early ray termination (runner/runner.py:197-264: render_img / render_img_with_pose) ------------
+/* ---- V1-V6  whole-frame renderer with early ray termination (runner/runner.py:197-264: render_img / render_img_with_pose) ------------
  * Stands in for the tiled inference path of the reference -- ray_sampler.h per n_rays_per_batch tile, the network, then
  * compute_rgbs_inference (calc_rgb.h:151-212) over every sample -- with a wavefront loop over rounds that drops a ray once it is opaque
  * (DESIGN.md section 4, "Rendering").  Per ray: rgb without background, alpha = 1 - T, and the number of composited samples.
@@ -375,6 +383,16 @@ int ngp_render_composite_round(void* stream, uint32_t n_rays, uint32_t capacity,
 int ngp_render_composite_round_depth(void* stream, uint32_t n_rays, uint32_t capacity, void* workspace, uint32_t n_alive, uint32_t k_steps,
                                      float min_transmittance, uint32_t cascades, float* rgb_out, float* alpha_out, uint32_t* n_samples_out,
                                      float* depth_out, uint32_t* n_alive_host);
+/* V6: ngp_render_composite_round that also accumulates normal_out[3g .. 3g+3) += w_i * n_i over the samples it composites, n_i =
+ * -grad_i / |grad_i| (0 where grad_i is 0) with grad_i row i of grad_rows: the round's (capacity,3) f32 density gradients, written by
+ * ngp_density_grad over the round's rows after the network.  The same weights, samples, order and stopping rule as V4, so the sum is
+ * the opacity-weighted mean outward normal in model (NGP) axes, unnormalised: normalise it, and cycle the axes back for NeRF world axes.
+ * The reference has no counterpart.  depth_out may be NULL; if not, it accumulates as in V5, so one render gives colour, depth and
+ * normals.  The caller zeroes normal_out (3 n_rays floats) and depth_out before the first round.  rgb, alpha, sample counts and depth
+ * are bit-identical to V4's and V5's.  A NULL grad_rows or normal_out is an error. */
+int ngp_render_composite_round_normals(void* stream, uint32_t n_rays, uint32_t capacity, void* workspace, uint32_t n_alive, uint32_t k_steps,
+                                       float min_transmittance, uint32_t cascades, float* rgb_out, float* alpha_out, uint32_t* n_samples_out,
+                                       const float* grad_rows, float* normal_out, float* depth_out, uint32_t* n_alive_host);
 
 /* ---- R10 occupancy-grid maintenance (DGS/density_grid_sampler.py:204-264 + five headers) ------------- */
 int ngp_grid_mark_untrained(void* stream, uint32_t n_elements, float* grid, uint32_t n_images, const float* focal_lengths,

@@ -16,6 +16,7 @@ SOURCES = {
     "hash_encode.cu": [],
     "mlp_tc.cu": [],
     "fused_net.cu": [],
+    "density_grad.cu": [],
     "nerf_mlp.cu": [],
     "nerf_lattice.cu": [],
     "mip_mlp.cu": [],

@@ -11,7 +11,8 @@
 //   composite round each alive ray composites its rows one after another; it stops after the first sample that brings T below
 //                   min_transmittance, or when its march has ended; the others form the next round's alive list (order-preserving
 //                   compaction).  The alive count is read back: 4 bytes a round.  The depth variant also sums w t per ray, t read from
-//                   the round's ts slots (V5; the colour-only kernel is the DEPTH = false instantiation, unchanged).
+//                   the round's ts slots (V5; the colour-only kernel is the DEPTH = false instantiation, unchanged); the normal variant
+//                   sums w n per ray from the round's density gradients (V6).
 // The result does not depend on K or on the row capacity: the march resumes exactly where it stopped and the stopping rule is
 // applied sample by sample.  No float atomics anywhere: every scan is a fixed-order block scan.
 #include "march_common.cuh"
@@ -179,14 +180,18 @@ __global__ void __launch_bounds__(RB) render_emit_kernel(uint32_t m, uint32_t K,
 // round and stay alive unchanged.  flags[k] = 1: the ray goes on into the next round.
 // DEPTH: also depth_out[g] += w t per sample, with the same weights, in the same order; t is the sample's ray parameter, which this
 // round's march left in the entry's ts slots.  DEPTH = false is the colour-only kernel, instruction for instruction.
-template <bool DEPTH>
+// NORMAL: also normal_out[g] += w n per sample, n = -g / |g| (0 where g = 0) of the sample's density gradient g, row base + s of
+// grad_rows (ngp_density_grad over the round's rows).  |g| is formed from g scaled by its largest component, so that it neither
+// underflows nor overflows.
+template <bool DEPTH, bool NORMAL>
 __global__ void __launch_bounds__(RB) render_composite_kernel(uint32_t n_alive, uint32_t m, uint32_t K, const uint32_t* __restrict__ alive,
                                                               const uint32_t* __restrict__ counts, const uint32_t* __restrict__ base_in,
                                                               const float* __restrict__ rows, const __half* __restrict__ net, uint32_t cascades,
                                                               float min_transmittance, float* __restrict__ ray_T, float* __restrict__ rgb_out,
                                                               float* __restrict__ alpha_out, uint32_t* __restrict__ n_out,
                                                               uint32_t* __restrict__ flags, uint32_t* __restrict__ sums,
-                                                              const float* __restrict__ ts, float* __restrict__ depth_out) {
+                                                              const float* __restrict__ ts, float* __restrict__ depth_out,
+                                                              const float* __restrict__ grad_rows, float* __restrict__ normal_out) {
     const uint32_t k = blockIdx.x * RB + threadIdx.x;
     uint32_t go_on = 0;
     if (k < n_alive) {
@@ -197,6 +202,8 @@ __global__ void __launch_bounds__(RB) render_composite_kernel(uint32_t n_alive, 
             float rgb[3] = {rgb_out[3 * (size_t)g], rgb_out[3 * (size_t)g + 1], rgb_out[3 * (size_t)g + 2]};
             uint32_t done = n_out[g];
             float S = DEPTH ? depth_out[g] : 0.f;
+            float nsum[3] = {0.f, 0.f, 0.f};
+            if (NORMAL) { nsum[0] = normal_out[3 * (size_t)g]; nsum[1] = normal_out[3 * (size_t)g + 1]; nsum[2] = normal_out[3 * (size_t)g + 2]; }
             const float* my_ts = ts + (size_t)k * K;
             bool stopped = false;
             for (uint32_t s = 0; s < n; ++s) {
@@ -206,6 +213,17 @@ __global__ void __launch_bounds__(RB) render_composite_kernel(uint32_t n_alive, 
                 const float w = smp.alpha * T;
                 rgb[0] = __fmaf_rn(w, smp.rgb[0], rgb[0]); rgb[1] = __fmaf_rn(w, smp.rgb[1], rgb[1]); rgb[2] = __fmaf_rn(w, smp.rgb[2], rgb[2]);
                 if (DEPTH) S = __fmaf_rn(w, __ldg(my_ts + s), S);
+                if (NORMAL) {
+                    const float* gr = grad_rows + (size_t)(base + s) * 3;
+                    const float g3[3] = {__ldg(gr), __ldg(gr + 1), __ldg(gr + 2)};
+                    const float mx = fmaxf(fabsf(g3[0]), fmaxf(fabsf(g3[1]), fabsf(g3[2])));
+                    if (mx > 0.f) {
+                        const float q[3] = {g3[0] / mx, g3[1] / mx, g3[2] / mx};
+                        const float len = sqrtf(q[0] * q[0] + q[1] * q[1] + q[2] * q[2]);
+#pragma unroll
+                        for (int a = 0; a < 3; ++a) nsum[a] = __fmaf_rn(w, -(q[a] / len), nsum[a]);
+                    }
+                }
                 T *= 1.f - smp.alpha;
                 ++done;
                 if (T < min_transmittance) { stopped = true; break; }                   // the rest of the ray cannot change the pixel
@@ -215,6 +233,7 @@ __global__ void __launch_bounds__(RB) render_composite_kernel(uint32_t n_alive, 
             alpha_out[g] = 1.f - T;
             n_out[g] = done;
             if (DEPTH) depth_out[g] = S;
+            if (NORMAL) { normal_out[3 * (size_t)g] = nsum[0]; normal_out[3 * (size_t)g + 1] = nsum[1]; normal_out[3 * (size_t)g + 2] = nsum[2]; }
             go_on = (!stopped && n == K) ? 1u : 0u;                                      // fewer than K samples: the march has ended
         }
         flags[k] = go_on;
@@ -260,11 +279,11 @@ int render_next_list(cudaStream_t s, void* ws, const RenderLayout& L, uint32_t n
     return 0;
 }
 
-// V4 / V4d: the composite kernel over the round's alive list, then the next alive list
-template <bool DEPTH>
+// V4 / V5 / V6: the composite kernel over the round's alive list, then the next alive list
+template <bool DEPTH, bool NORMAL>
 int render_composite_round(const char* fn, void* stream, uint32_t n_rays, uint32_t capacity, void* workspace, uint32_t n_alive, uint32_t k_steps,
                            float min_transmittance, uint32_t cascades, float* rgb_out, float* alpha_out, uint32_t* n_samples_out, float* depth_out,
-                           uint32_t* n_alive_host) {
+                           const float* grad_rows, float* normal_out, uint32_t* n_alive_host) {
     NGP_REQUIRE(capacity > 0, std::string(fn) + ": the row capacity must be positive");
     NGP_REQUIRE(workspace != nullptr, std::string(fn) + ": workspace is required (ngp_render_workspace_bytes)");
     NGP_REQUIRE(k_steps >= 1 && k_steps <= capacity, std::string(fn) + ": k_steps must be in [1, capacity]");
@@ -275,11 +294,12 @@ int render_composite_round(const char* fn, void* stream, uint32_t n_rays, uint32
     cudaStream_t s = (cudaStream_t)stream;
     const RenderLayout L = render_layout(n_rays, capacity);
     const uint32_t m = min(n_alive, capacity / k_steps);
-    render_composite_kernel<DEPTH><<<blocks_for(n_alive), RB, 0, s>>>(n_alive, m, k_steps, at<uint32_t>(workspace, L.alive), at<uint32_t>(workspace, L.counts),
+    render_composite_kernel<DEPTH, NORMAL><<<blocks_for(n_alive), RB, 0, s>>>(n_alive, m, k_steps, at<uint32_t>(workspace, L.alive), at<uint32_t>(workspace, L.counts),
                                                                       at<uint32_t>(workspace, L.base), at<float>(workspace, L.rows),
                                                                       at<__half>(workspace, L.net), cascades, min_transmittance, at<float>(workspace, L.ray_T),
                                                                       rgb_out, alpha_out, n_samples_out, at<uint32_t>(workspace, L.flags),
-                                                                      at<uint32_t>(workspace, L.sums), at<float>(workspace, L.ts), depth_out);
+                                                                      at<uint32_t>(workspace, L.sums), at<float>(workspace, L.ts), depth_out,
+                                                                      grad_rows, normal_out);
     NGP_LAUNCH_CHECK();
     return render_next_list(s, workspace, L, n_alive, at<uint32_t>(workspace, L.alive), n_alive_host);
 }
@@ -352,16 +372,29 @@ int ngp_render_march_round(void* stream, uint32_t n_rays, uint32_t capacity, voi
 int ngp_render_composite_round(void* stream, uint32_t n_rays, uint32_t capacity, void* workspace, uint32_t n_alive, uint32_t k_steps,
                                float min_transmittance, uint32_t cascades, float* rgb_out, float* alpha_out, uint32_t* n_samples_out,
                                uint32_t* n_alive_host) {
-    return render_composite_round<false>("ngp_render_composite_round", stream, n_rays, capacity, workspace, n_alive, k_steps, min_transmittance,
-                                         cascades, rgb_out, alpha_out, n_samples_out, nullptr, n_alive_host);
+    return render_composite_round<false, false>("ngp_render_composite_round", stream, n_rays, capacity, workspace, n_alive, k_steps,
+                                                min_transmittance, cascades, rgb_out, alpha_out, n_samples_out, nullptr, nullptr, nullptr, n_alive_host);
 }
 
 int ngp_render_composite_round_depth(void* stream, uint32_t n_rays, uint32_t capacity, void* workspace, uint32_t n_alive, uint32_t k_steps,
                                      float min_transmittance, uint32_t cascades, float* rgb_out, float* alpha_out, uint32_t* n_samples_out,
                                      float* depth_out, uint32_t* n_alive_host) {
     NGP_REQUIRE(depth_out != nullptr, "ngp_render_composite_round_depth: depth_out is required");
-    return render_composite_round<true>("ngp_render_composite_round_depth", stream, n_rays, capacity, workspace, n_alive, k_steps,
-                                        min_transmittance, cascades, rgb_out, alpha_out, n_samples_out, depth_out, n_alive_host);
+    return render_composite_round<true, false>("ngp_render_composite_round_depth", stream, n_rays, capacity, workspace, n_alive, k_steps,
+                                               min_transmittance, cascades, rgb_out, alpha_out, n_samples_out, depth_out, nullptr, nullptr, n_alive_host);
+}
+
+int ngp_render_composite_round_normals(void* stream, uint32_t n_rays, uint32_t capacity, void* workspace, uint32_t n_alive, uint32_t k_steps,
+                                       float min_transmittance, uint32_t cascades, float* rgb_out, float* alpha_out, uint32_t* n_samples_out,
+                                       const float* grad_rows, float* normal_out, float* depth_out, uint32_t* n_alive_host) {
+    static const char* fn = "ngp_render_composite_round_normals";
+    NGP_REQUIRE(grad_rows != nullptr, std::string(fn) + ": grad_rows is required (ngp_density_grad over the round's rows)");
+    NGP_REQUIRE(normal_out != nullptr, std::string(fn) + ": normal_out is required");
+    if (depth_out)
+        return render_composite_round<true, true>(fn, stream, n_rays, capacity, workspace, n_alive, k_steps, min_transmittance, cascades, rgb_out,
+                                                  alpha_out, n_samples_out, depth_out, grad_rows, normal_out, n_alive_host);
+    return render_composite_round<false, true>(fn, stream, n_rays, capacity, workspace, n_alive, k_steps, min_transmittance, cascades, rgb_out,
+                                               alpha_out, n_samples_out, nullptr, grad_rows, normal_out, n_alive_host);
 }
 
 }  // extern "C"

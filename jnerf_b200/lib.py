@@ -29,6 +29,7 @@ SIGNATURES = {
     "ngp_network_bwd_fx_bytes": (_i32, [_u64, _vp, _vp]),
     "ngp_network_bwd_fx": (_i32, [_vp, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _u32, _vp, _u64, _vp, _u64]),
     "ngp_density_fwd": (_i32, [_vp, _u32, _vp, _vp, _vp, _vp, _vp]),
+    "ngp_density_grad": (_i32, [_vp, _u32, _vp, _vp, _vp, _vp, _vp, _vp]),
     "ngp_nerf_param_count": (_i32, [_vp]),
     "ngp_nerf_workspace_bytes": (_i32, [_u32, _vp, _vp]),
     "ngp_nerf_fwd": (_i32, [_vp, _u32, _vp, _vp, _vp, _vp, _vp]),
@@ -76,6 +77,7 @@ SIGNATURES = {
     "ngp_render_march_round": (_i32, [_vp, _u32, _u32, _vp, _u32, _u32, _f32, _f32, _vp, _vp, _vp, _f32, _u32, _i32]),
     "ngp_render_composite_round": (_i32, [_vp, _u32, _u32, _vp, _u32, _u32, _f32, _u32, _vp, _vp, _vp, _vp]),
     "ngp_render_composite_round_depth": (_i32, [_vp, _u32, _u32, _vp, _u32, _u32, _f32, _u32, _vp, _vp, _vp, _vp, _vp]),
+    "ngp_render_composite_round_normals": (_i32, [_vp, _u32, _u32, _vp, _u32, _u32, _f32, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "ngp_march_workspace_bytes": (_u64, [_u32]),
     "ngp_march": (_i32, [_vp, _u32, _f32, _f32, _u32, _vp, _vp, _vp, _f32, _f32, _u32, _i32, _u64, _u64, _vp, _vp, _vp, _vp, _vp]),
     "ngp_compact": (_i32, [_vp, _u32, _u32, _vp, _vp, _vp, _vp, _vp, _i32]),
@@ -113,6 +115,7 @@ KERNELS_PER_CALL = {
     "ngp_blend_target": 1,
     "ngp_density_lattice": 1, "ngp_nerf_density_lattice": 1, "ngp_marching_cubes": 3, "ngp_mesh_largest_component": 18, "ngp_mesh_vertex_normals": 7,
     "ngp_render_init": 3, "ngp_render_march_round": 3, "ngp_render_composite_round": 3, "ngp_render_composite_round_depth": 3,
+    "ngp_render_composite_round_normals": 3, "ngp_density_grad": 1,
     "ngp_nerf_fwd": 1, "ngp_nerf_density": 1, "ngp_nerf_bwd": 3,
     "ngp_mip_rays": 1, "ngp_mip_sample": 1, "ngp_mip_resample": 1, "ngp_mip_encode": 1, "ngp_mip_fwd": 1, "ngp_mip_composite_fwd": 1,
     "ngp_mip_composite_loss_bwd": 1, "ngp_mip_rays_multi": 1, "ngp_mip_encode_deg": 1, "ngp_mip_fwd_deg": 1,

@@ -505,15 +505,21 @@ def render_workspace(n_rays, workspace=None, capacity=RENDER_CAPACITY):
 
 
 def render_rays(rays_o, rays_d, bitfield, aabb, cone_angle, near, cascades, const_dt, rng, grid, levels, wd, wr, jitter_tile,
-                min_transmittance=0.0, capacity=RENDER_CAPACITY, workspace=None, net=None, depth=False):
+                min_transmittance=0.0, capacity=RENDER_CAPACITY, workspace=None, net=None, depth=False, normals=False):
     """Render R rays (model space) to (rgb (R,3) without background, alpha (R,1) = 1 - T, n_samples (R,) int32, rounds).
     Each ray composites the samples ngp_march gives it under the jitter layout of `jitter_tile`-ray tiles, in order, and stops after the
     first sample that brings its transmittance below `min_transmittance` (0: never).  `rng` is not advanced here: the caller moves it
     on by ceil(R / jitter_tile) * 2^32, as the tiled renderer would.  One 4-byte read-back per round.
     net: the network as net(rows, n_dev, out) instead of the fused NGP network of (grid, levels, wd, wr), e.g. OriginNeRFNetworks.infer.
     depth: also return depth (R,) float32 = sum(w t) over the composited samples, t in model units along rays_d (0 for rays that miss
-    the box), as a fifth element; the other four are bit-identical to those of depth=False."""
+    the box), as a fifth element; the other four are bit-identical to those of depth=False.
+    normals: also return the (R, 3) float32 sum of w n over the composited samples, n the unit outward normal -grad sigma / |grad sigma|
+    of the fused NGP density in model axes (ngp_density_grad after the network in every round), as the last element; the others are
+    bit-identical to those of normals=False.  It needs a (capacity, 3) float32 gradient buffer (48 MB at the default capacity) and the
+    fused network: with `net` it raises NotImplementedError."""
     import ctypes
+    if normals and net is not None:
+        raise NotImplementedError("render_rays(normals=True) differentiates the fused NGP density network; a `net` model has no input gradient")
     R, dev = rays_o.shape[0], rays_o.device
     nbytes, off_rows, off_net, off_cnt = render_workspace_layout(R, capacity)
     if workspace is None or workspace.numel() < nbytes:
@@ -525,6 +531,8 @@ def render_rays(rays_o, rays_d, bitfield, aabb, cone_angle, near, cascades, cons
     alpha = torch.empty((R, 1), dtype=torch.float32, device=dev)
     n_samples = torch.empty(R, dtype=torch.int32, device=dev)
     depth_out = torch.zeros(R, dtype=torch.float32, device=dev) if depth else None
+    normal_out = torch.zeros((R, 3), dtype=torch.float32, device=dev) if normals else None
+    grad_rows = torch.empty((capacity, 3), dtype=torch.float32, device=dev) if normals else None
     alive = np.zeros(1, np.uint32)
     ap = alive.ctypes.data_as(ctypes.c_void_p)
     lib.call("ngp_render_init", _stream(), R, int(capacity), _p(workspace), float(aabb[0]), float(aabb[1]), _p(rays_o), _p(rays_d), float(cone_angle),
@@ -540,16 +548,28 @@ def render_rays(rays_o, rays_d, bitfield, aabb, cone_angle, near, cascades, cons
             network_fwd(rows[:bound], grid, levels, wd, wr, n_dev=n_rows, save_enc=False, out=out_rows[:bound])
         else:
             net(rows[:bound], n_rows, out_rows[:bound])
-        if depth:
+        if normals:
+            density_grad(rows[:bound], grid, levels, wd, n_dev=n_rows, out=grad_rows[:bound])
+            lib.call("ngp_render_composite_round_normals", _stream(), R, int(capacity), _p(workspace), n_alive, k, float(min_transmittance),
+                     int(cascades), _p(rgb), _p(alpha), _p(n_samples), _p(grad_rows), _p(normal_out), _p(depth_out), ap)
+        elif depth:
             lib.call("ngp_render_composite_round_depth", _stream(), R, int(capacity), _p(workspace), n_alive, k, float(min_transmittance),
                      int(cascades), _p(rgb), _p(alpha), _p(n_samples), _p(depth_out), ap)
         else:
             lib.call("ngp_render_composite_round", _stream(), R, int(capacity), _p(workspace), n_alive, k, float(min_transmittance),
                      int(cascades), _p(rgb), _p(alpha), _p(n_samples), ap)
         rounds += 1
-    if depth:
-        return rgb, alpha, n_samples, rounds, depth_out
-    return rgb, alpha, n_samples, rounds
+    return (rgb, alpha, n_samples, rounds) + ((depth_out,) if depth else ()) + ((normal_out,) if normals else ())
+
+
+def density_grad(coords, grid, levels, wd, n_dev=None, out=None):
+    """ngp_density_grad: d sigma_raw / d position (n, 3) float32 of NerfCoordinate rows coords (n, 7), position = row[0:3] (warped model
+    space), for the fused NGP density network of (grid, levels, wd).  n_dev: optional device row count (rows past it are not written)."""
+    n = coords.shape[0]
+    if out is None:
+        out = torch.empty((n, 3), dtype=torch.float32, device=coords.device)
+    lib.call("ngp_density_grad", _stream(), n, _p(n_dev), _p(coords), _p(grid), _p(levels.table), _p(wd), _p(out))
+    return out
 
 
 def march(rays_o, rays_d, bitfield, aabb, max_samples, cone_angle, near, cascades, const_dt, rng, coords=None, workspace=None):

@@ -377,9 +377,10 @@ class SyntheticNerfDataset(_RayBatcher):
             out[i] = (self.shade(o, d) * 255.0 + 0.5).clamp(0, 255).to(torch.uint8)
         return out
 
-    def shade(self, o, d, return_t=False):
+    def shade(self, o, d, return_t=False, return_normal=False):
         """RGBA in [0,1] of the analytic scene along rays (o,d) given in NGP coordinates; with `return_t` also the distance to the
-        hit (inf where the ray leaves the scene)."""
+        hit (inf where the ray leaves the scene), with `return_normal` (last) also the unit outward normal of the surface hit, in NGP
+        axes (0 where the ray leaves the scene)."""
         n = o.shape[0]
         t_best = torch.full((n,), float("inf"), device=o.device)
         col = torch.zeros((n, 3), device=o.device)
@@ -440,7 +441,8 @@ class SyntheticNerfDataset(_RayBatcher):
         lam = 0.35 + 0.65 * (nrm * light).sum(-1).clamp_min(0)
         rgb = (col * lam[:, None]).clamp(0, 1) * alpha[:, None]
         rgba = torch.cat([rgb, alpha[:, None]], -1)
-        return (rgba, t_best) if return_t else rgba
+        out = (rgba,) + ((t_best,) if return_t else ()) + ((nrm,) if return_normal else ())
+        return out if len(out) > 1 else rgba
 
 
 MULTISCALE_LEVELS = 4                  # full, 1/2, 1/4 and 1/8 resolution, as mip-NeRF's multiscale NeRF-synthetic

@@ -589,15 +589,19 @@ class Runner:
 
     # ------------------------------------------------------------------------------------------ rendering (runner.py:86-121, 162-264)
     @torch.no_grad()
-    def render_rays(self, rays_o, rays_d, min_transmittance=1e-4, depth=False):
+    def render_rays(self, rays_o, rays_d, min_transmittance=1e-4, depth=False, normals=False):
         """Whole-frame renderer (ops.render_rays): every ray at once in rounds, each ray dropped after the first sample that brings its
         transmittance below min_transmittance (0: never, and then every ray composites the samples render_img_nosync gives it).  The
         jitter and the sampler rng advance exactly as render_img_nosync's n_rays_per_batch tiles would have them.
         Returns (rgb (R,3) without background, alpha (R,1), n_samples (R,), rounds); with depth=True also the weighted sum of the
-        samples' ray parameters, sum(w t) (R,) in model units (depth_from_sum turns it into a distance).
+        samples' ray parameters, sum(w t) (R,) in model units (depth_from_sum turns it into a distance); with normals=True also (last)
+        the weighted sum of the samples' unit normals, sum(w n) (R,3) in model axes (normal_from_sum turns it into a NeRF-axes normal).
+        Normals differentiate the fused NGP density network: other models raise NotImplementedError.
         The renderer's workspace (per-ray state, and 144 MB of round rows and network outputs at the default capacity) is kept for the
         next frame; render() and test() release it when they finish, and release_render_workspace() does so at any time."""
         assert self._can_infer, "render_rays needs the fused NGP model or a model with an inference forward (infer)"
+        if normals and not self.fast:
+            raise NotImplementedError("normal maps need the gradient of the fused NGP density network; this model has none")
         self._table_ready()
         self._sync_front()
         s, m = self.sampler, self.model
@@ -605,7 +609,7 @@ class Runner:
         self._render_ws = ops.render_workspace(R, self._render_ws)
         args = (rays_o.contiguous(), rays_d.contiguous(), s.density_grid_bitfield, s.aabb_range, s.cone_angle_constant, s.near_distance,
                 s.NERF_CASCADES, s.const_dt, s.rng)
-        kw = {"depth": True} if depth else {}
+        kw = dict(({"depth": True} if depth else {}), **({"normals": True} if normals else {}))
         if self.fast:
             out = ops.render_rays(*args, m.pos_encoder.m_grid, m.pos_encoder.levels, m.density_mlp.con_weights, m.rgb_mlp.con_weights, tile,
                                   min_transmittance=min_transmittance, workspace=self._render_ws, **kw)
@@ -619,17 +623,20 @@ class Runner:
         """Free the whole-frame renderer's workspace (the next render_rays allocates a new one), e.g. before training on."""
         self._render_ws = None
 
-    def _render_frame(self, rays_o, rays_d, W, H, min_transmittance, depth_scale=None):
+    def _render_frame(self, rays_o, rays_d, W, H, min_transmittance, depth_scale=None, normals=False):
         """(img (H,W,3) with the background blended in unless alpha_image, alpha (H,W,1), n_samples (H,W), rounds); with a
-        depth_scale (the scale of the dataset the rays come from) also depth (H,W) in NeRF world units, from the same render."""
-        if depth_scale:
-            rgb, alpha, n, rounds, S = self.render_rays(rays_o, rays_d, min_transmittance, depth=True)
-        else:
-            rgb, alpha, n, rounds = self.render_rays(rays_o, rays_d, min_transmittance)
+        depth_scale (the scale of the dataset the rays come from) also depth (H,W) in NeRF world units, and with normals also the unit
+        normal (H,W,3) in NeRF world axes (normal_from_sum), from the same render."""
+        out = self.render_rays(rays_o, rays_d, min_transmittance, depth=bool(depth_scale), normals=normals)
+        rgb, alpha, n, rounds = out[:4]
         if not getattr(self.cfg, "alpha_image", False):
             rgb = rgb + torch.tensor(self.background_color, dtype=torch.float32, device=rgb.device) * (1 - alpha)
         frame = (rgb.reshape(H, W, 3), alpha.reshape(H, W, 1), n.reshape(H, W), rounds)
-        return frame + (depth_from_sum(S, alpha, depth_scale).reshape(H, W),) if depth_scale else frame
+        if depth_scale:
+            frame += (depth_from_sum(out[4], alpha, depth_scale).reshape(H, W),)
+        if normals:
+            frame += (normal_from_sum(out[-1], alpha).reshape(H, W, 3),)
+        return frame
 
     def pose_rays(self, pose):
         """generate_rays_with_pose (dataset.py:236-253): the rays of every pixel, row-major, of a camera at `pose` (3x4 or 4x4 NeRF
@@ -662,6 +669,15 @@ class Runner:
         img, alpha, _, _, depth = self._render_frame(o, d, W, H, min_transmittance, depth_scale=float(ds.scale))
         return img, depth, alpha
 
+    @torch.no_grad()
+    def render_normal_with_pose(self, pose, min_transmittance=1e-4):
+        """render_img_with_pose with the normal map of the same render: (img (H,W,3), normal (H,W,3), alpha (H,W,1)), normal the unit
+        opacity-weighted outward normal of the density in NeRF world axes (normal_from_sum; 0 where alpha is 0).  Fused NGP model only."""
+        W, H = self.dataset["train"].resolution
+        o, d = self.pose_rays(pose)
+        img, alpha, _, _, normal = self._render_frame(o, d, W, H, min_transmittance, normals=True)
+        return img, normal, alpha
+
     def depth_range(self, poses, ds=None):
         """(near, far) in NeRF world units for the grey scale of depth images (depth_to_grey): the capture's bounds for a dataset that
         carries them (LLFFDataset.bounds), else the nearest and the farthest distance from any of the cameras `poses` (NeRF
@@ -691,13 +707,17 @@ class Runner:
         Image.fromarray((img * 255 + 0.5).clip(0, 255).astype(np.uint8)).save(path)
 
     @torch.no_grad()
-    def render(self, save_path=None, load_ckpt=False, min_transmittance=1e-4, depth=False, poses=None):
+    def render(self, save_path=None, load_ckpt=False, min_transmittance=1e-4, depth=False, poses=None, normals=False):
         """runner.py:101-121: the 80-frame spherical camera path (utils/camera_path.py) as an mp4 (OpenCV, mp4v, 28 fps), by default
         log_dir/exp_name/demo.mp4.  Returns the path.
         poses: another camera path (NeRF camera-to-world matrices), e.g. utils.camera_path.path_spiral for a forward-facing capture.
         depth: also write the depth video of the same frames beside it ({stem}_depth.mp4, e.g. demo_depth.mp4), grey = alpha *
         clip((far - depth) / (far - near), 0, 1) with one (near, far) for the whole video, depth_range(poses): nearer is brighter and a
-        shade is the same distance in every frame; empty pixels are black."""
+        shade is the same distance in every frame; empty pixels are black.
+        normals: also write the normal video of the same frames ({stem}_normal.mp4), RGB = alpha * (n + 1) / 2 of the NeRF-axes normal
+        (normal_to_rgb).  Fused NGP model only."""
+        if normals and not self.fast:
+            raise NotImplementedError("normal maps need the gradient of the fused NGP density network; this model has none")
         try:
             import cv2
         except ImportError as e:
@@ -715,31 +735,42 @@ class Runner:
         fourcc = cv2.VideoWriter_fourcc(*"mp4v")
         writer = cv2.VideoWriter(str(save_path), fourcc, 28, (W, H))
         depth_writer = cv2.VideoWriter(str(save_path)[:-4] + "_depth.mp4", fourcc, 28, (W, H)) if depth else None
+        normal_writer = cv2.VideoWriter(str(save_path)[:-4] + "_normal.mp4", fourcc, 28, (W, H)) if normals else None
         try:
             near, far = self.depth_range(poses) if depth else (0.0, 0.0)
             for pose in poses:
-                if depth:
+                if normals:                                           # colour, normals and (with depth) depth from one render
+                    o, d = self.pose_rays(pose)
+                    frame = self._render_frame(o, d, W, H, min_transmittance, depth_scale=float(self.dataset["train"].scale) if depth else None,
+                                               normals=True)
+                    img, alpha, dep = frame[0], frame[1], frame[4] if depth else None
+                    normal_writer.write(np.ascontiguousarray(normal_to_rgb(frame[-1], alpha)[..., ::-1]))
+                elif depth:
                     img, dep, alpha = self.render_depth_with_pose(pose, min_transmittance)
-                    g = depth_to_grey(dep, alpha, near, far)
-                    depth_writer.write(np.ascontiguousarray(np.repeat(g[..., None], 3, -1)))
                 else:
                     img = self.render_img_with_pose(pose, min_transmittance)
+                if depth:
+                    g = depth_to_grey(dep, alpha, near, far)
+                    depth_writer.write(np.ascontiguousarray(np.repeat(g[..., None], 3, -1)))
                 u8 = (img.cpu().numpy() * 255 + 0.5).clip(0, 255).astype(np.uint8)
                 writer.write(np.ascontiguousarray(u8[..., ::-1]))    # OpenCV takes BGR: the file shows the true colours (DESIGN.md section 7)
         finally:
             writer.release()
-            if depth_writer is not None:
-                depth_writer.release()
+            for w in (depth_writer, normal_writer):
+                if w is not None:
+                    w.release()
             self.release_render_workspace()
         return save_path
 
     @torch.no_grad()
-    def render_test(self, save_img=True, save_path=None, min_transmittance=1e-4, depth=False):
+    def render_test(self, save_img=True, save_path=None, min_transmittance=1e-4, depth=False, normals=False):
         """runner.py:162-178: every view of the test split on the whole-frame renderer; saves {exp_name}_r_{i}.png (RGBA when
         alpha_image is set) and, when the split has images, {exp_name}_gt_{i}.png; returns the per-view mse against the target with the
         background blended in (an empty list for a split without images, as the reference computes no PSNR then).
         depth: with save_img also {exp_name}_depth_{i}.npy (float32 (H,W), NeRF world units, depth_from_sum) and {exp_name}_depth_{i}.png
-        (8-bit grey, nearer is brighter, one depth_range over the test views, as in render's depth video), from the same render."""
+        (8-bit grey, nearer is brighter, one depth_range over the test views, as in render's depth video), from the same render.
+        normals: with save_img also {exp_name}_normal_{i}.npy (float32 (H,W,3), unit NeRF-axes normals, normal_from_sum) and
+        {exp_name}_normal_{i}.png (RGB = alpha * (n + 1) / 2, normal_to_rgb), from the same render.  Fused NGP model only."""
         ds = self.dataset["test"]
         save_path = self._save_path() if save_path is None else save_path
         if save_img:
@@ -751,16 +782,19 @@ class Runner:
         mse = []
         for i in range(ds.n_images):
             o, d = ds.generate_rays_total_test(i)
-            if depth:
-                img, alpha, _, _, dep = self._render_frame(o, d, W, H, min_transmittance, depth_scale=float(ds.scale))
-            else:
-                img, alpha, _, _ = self._render_frame(o, d, W, H, min_transmittance)
+            frame = self._render_frame(o, d, W, H, min_transmittance, depth_scale=float(ds.scale) if depth else None, normals=normals)
+            img, alpha = frame[0], frame[1]
             if save_img:
+                from PIL import Image
                 self.save_img(os.path.join(save_path, f"{exp}_r_{i}.png"), img, alpha if getattr(self.cfg, "alpha_image", False) else None)
                 if depth:
-                    from PIL import Image
+                    dep = frame[4]
                     np.save(os.path.join(save_path, f"{exp}_depth_{i}.npy"), dep.cpu().numpy().astype(np.float32))
                     Image.fromarray(depth_to_grey(dep, alpha, near, far), "L").save(os.path.join(save_path, f"{exp}_depth_{i}.png"))
+                if normals:
+                    nrm = frame[-1]
+                    np.save(os.path.join(save_path, f"{exp}_normal_{i}.npy"), nrm.cpu().numpy().astype(np.float32))
+                    Image.fromarray(normal_to_rgb(nrm, alpha), "RGB").save(os.path.join(save_path, f"{exp}_normal_{i}.png"))
             if not have_img:                                          # runner.py:173: no target, no gt image, no mse
                 continue
             tar = self._target_img(ds, i)
@@ -770,16 +804,18 @@ class Runner:
         return mse
 
     @torch.no_grad()
-    def test(self, load_ckpt=False, min_transmittance=1e-4, depth=False):
+    def test(self, load_ckpt=False, min_transmittance=1e-4, depth=False, normals=False):
         """runner.py:86-99: render the test split into log_dir/exp_name/test and print the mean test PSNR, which is returned (None for
-        a split without images, as the reference prints none then).  depth: also the depth maps of the views (render_test).  Releases
+        a split without images, as the reference prints none then).  depth / normals: also the depth / normal maps of the views
+        (render_test).  Releases
         the renderer's workspace when done."""
         if load_ckpt:
             self.load_ckpt(self.cfg.ckpt_path)
         if self.dataset["test"] is None:
             self.dataset["test"] = build_from_cfg(self.cfg.dataset.test, DATASETS)
         try:
-            mse = self.render_test(save_path=os.path.join(self._save_path(), "test"), min_transmittance=min_transmittance, depth=depth)
+            mse = self.render_test(save_path=os.path.join(self._save_path(), "test"), min_transmittance=min_transmittance, depth=depth,
+                                   normals=normals)
         finally:
             self.release_render_workspace()
         if not getattr(self.dataset["test"], "have_img", True):
@@ -955,6 +991,27 @@ def depth_from_sum(S, alpha, scale):
     sampled interval; this does not."""
     a = alpha.reshape(S.shape)
     return torch.where(a > 0, S / (float(scale) * a), torch.zeros_like(S))
+
+
+def normal_from_sum(N, alpha):
+    """The normal of a pixel from the renderer's sum N = sum(w n) (Runner.render_rays(normals=True)), (R,3) in model axes: N / |N| as a
+    unit vector in NeRF world axes, and 0 where alpha or |N| is 0.  Every dataset maps NeRF world to model space with matrix_nerf2ngp,
+    whose linear part is the axis cycle model = (nerf[1], nerf[2], nerf[0]) times the scale (correct_pose flips camera axes, not world
+    ones), so the inverse is nerf = (model[2], model[0], model[1]); the scale does not change a direction."""
+    n = N.reshape(-1, 3)
+    m = n.abs().amax(dim=1, keepdim=True)                             # scaled by its largest component first: |N| cannot underflow
+    ok = (alpha.reshape(-1, 1) > 0) & (m > 0)
+    q = n / torch.where(ok, m, torch.ones_like(m))
+    unit = torch.where(ok, q / q.norm(dim=1, keepdim=True).clamp_min(1), torch.zeros_like(n))
+    return unit[:, [2, 0, 1]].reshape(N.shape)
+
+
+def normal_to_rgb(normal, alpha):
+    """8-bit RGB image of a normal map: alpha * (n + 1) / 2, so the x, y and z of the NeRF-axes normal show as red, green and blue and
+    empty pixels are black.  normal (H,W,3), alpha (H,W,1) or (H,W) -> (H,W,3) uint8."""
+    n = normal.float().cpu().numpy()
+    a = alpha.float().cpu().numpy().reshape(n.shape[:-1] + (1,))
+    return (a * (n + 1.0) * 0.5 * 255 + 0.5).clip(0, 255).astype(np.uint8)
 
 
 def depth_to_grey(depth, alpha, near, far):

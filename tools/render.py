@@ -14,7 +14,11 @@ min_transmittance 0 on the same views with the same jitter, the three alternatin
 the video gains DIR/demo_depth.mp4 and its timing is of the depth renders; pose and test render every view with and without depth,
 alternating, write the depth maps ({exp}_depth_{i}.npy / .png, pose_depth.*) and add the depth-on timing to the JSON line.  --path
 spiral flies the spiral of a forward-facing capture (utils/camera_path.path_spiral) instead of the spherical path; it needs a dataset
-with near / far bounds (LLFF).  --workload llff is the forward-facing stand-in of tools/train_psnr.py, written to a temporary directory."""
+with near / far bounds (LLFF).  --workload llff is the forward-facing stand-in of tools/train_psnr.py, written to a temporary directory.
+--normals also renders normal maps (fused NGP models only), as --depth does depth maps: the video gains DIR/demo_normal.mp4, pose and
+test render every view with and without normals, alternating, and write {exp}_normal_{i}.npy / .png (pose_normal.*); the JSON line
+gains the normal-on timing and, for pose and test, ngp_density_grad alone against the fused forward (ngp_network_fwd) on the same
+march rows of the first view, in rows per second."""
 import argparse
 import json
 import os
@@ -32,6 +36,37 @@ def summary(ms):
     return {"median": round(statistics.median(ms), 3), "min": round(min(ms), 3), "max": round(max(ms), 3)}
 
 
+def density_grad_rate(runner, ds, i, mode, reps=20):
+    """ngp_density_grad and ngp_network_fwd over the same rows, the march samples of view i (ray-ordered, as a render round holds them):
+    rows and median ms of each over `reps` alternating launches (CUDA events), and rows per second."""
+    import torch
+    from jnerf_b200 import ops
+    s, m = runner.sampler, runner.model
+    o, d = runner.pose_rays(ds.poses[i]) if mode == "train" else ds.generate_rays_total_test(i)
+    rng = s.rng.copy()
+    coords, _, _, counters = ops.march(o.contiguous(), d.contiguous(), s.density_grid_bitfield, s.aabb_range, 1 << 23, s.cone_angle_constant,
+                                       s.near_distance, s.NERF_CASCADES, s.const_dt, rng)
+    rows = coords[:int(counters[1].item())].contiguous()                      # the compacted samples, at most the buffer's 2^23
+    n = rows.shape[0]
+    grid, lv, wd, wr = m.pos_encoder.m_grid, m.pos_encoder.levels, m.density_mlp.con_weights, m.rgb_mlp.con_weights
+    out = torch.empty((n, 4), dtype=torch.float16, device="cuda")
+    grad = torch.empty((n, 3), dtype=torch.float32, device="cuda")
+    kernels = {"density_grad": lambda: ops.density_grad(rows, grid, lv, wd, out=grad),
+               "network_fwd": lambda: ops.network_fwd(rows, grid, lv, wd, wr, save_enc=False, out=out)}
+    ms = {k: [] for k in kernels}
+    for f in kernels.values():
+        f()
+    for _ in range(reps):
+        for k, f in kernels.items():
+            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            a.record()
+            f()
+            b.record()
+            b.synchronize()
+            ms[k].append(a.elapsed_time(b))
+    return {"rows": n, **{k: dict(ms=round(statistics.median(v), 4), rows_per_s=round(n / statistics.median(v) * 1e3, 1)) for k, v in ms.items()}}
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--config-file", default="", help="a JNeRF config (projects/ngp/configs/*.py)")
@@ -44,6 +79,7 @@ def main():
     ap.add_argument("--min-transmittance", type=float, default=1e-4)
     ap.add_argument("--compare", action="store_true", help="also time render_img_nosync and min_transmittance 0, alternating")
     ap.add_argument("--depth", action="store_true", help="also render depth maps (and time them)")
+    ap.add_argument("--normals", action="store_true", help="also render normal maps (and time them and the density-gradient kernel)")
     ap.add_argument("--path", default="spherical", choices=["spherical", "spiral"], help="camera path of --task video")
     ap.add_argument("--out", default="render_out")
     args = ap.parse_args()
@@ -116,10 +152,12 @@ def main():
             spp.append(float(out[2].float().mean()))
             return out
         runner.render_rays = timed
-        path = runner.render(save_path=os.path.join(args.out, "demo.mp4"), min_transmittance=eps, depth=args.depth, poses=poses)
+        path = runner.render(save_path=os.path.join(args.out, "demo.mp4"), min_transmittance=eps, depth=args.depth, poses=poses,
+                              normals=args.normals)
         W, H = runner.dataset["train"].resolution
         row.update(frames=len(ms), W=W, H=H, ms=summary(ms), rounds=round(statistics.mean(rounds), 2), spp=round(statistics.mean(spp), 3),
-                   out=os.path.abspath(path), path=args.path, depth=args.depth)
+                   out=os.path.abspath(path), path=args.path, depth=args.depth,
+                   normals=args.normals)
     else:
         if args.task == "test":
             if runner.dataset["test"] is None:
@@ -131,7 +169,7 @@ def main():
             views = [0]
         W, H = ds.resolution
         bgc = torch.tensor(runner.background_color, dtype=torch.float32, device="cuda")
-        variants = [("new", eps)] + ([("depth", eps)] if args.depth else []) + ([("eps0", 0.0), ("nosync", None)] if args.compare else [])
+        variants = [("new", eps)] + ([("depth", eps)] if args.depth else []) + ([("normal", eps)] if args.normals else []) + ([("eps0", 0.0), ("nosync", None)] if args.compare else [])
         res = {k: dict(ms=[], rounds=[], spp=[], psnr=[]) for k, _ in variants}
 
         def run(kind, m, i):
@@ -144,6 +182,8 @@ def main():
                 o, d = ds.generate_rays_total_test(i)
             if kind == "depth":
                 img, alpha, n, rounds, dep = runner._render_frame(o, d, W, H, m, depth_scale=float(ds.scale))
+            elif kind == "normal":
+                img, alpha, n, rounds, dep = runner._render_frame(o, d, W, H, m, normals=True)     # dep: the normal map
             else:
                 img, alpha, n, rounds = runner._render_frame(o, d, W, H, m)
                 dep = None
@@ -151,9 +191,10 @@ def main():
             tar = (tar[:, :3] * tar[:, 3:] + bgc * (1 - tar[:, 3:])).reshape(H, W, 3)
             return img, tar, (n, rounds, dep, alpha)
 
-        if args.depth:
+        if args.depth or args.normals:
             from PIL import Image
-            from jnerf_b200.runner import depth_to_grey
+            from jnerf_b200.runner import depth_to_grey, normal_to_rgb
+        if args.depth:
             near, far = runner.depth_range([ds.poses[i] for i in views], ds)
         rng0 = s.rng.copy()
         for kind, m in variants:                                     # warm-up: modules, allocations
@@ -183,6 +224,10 @@ def main():
                     stem = os.path.join(args.out, f"{runner.cfg.exp_name}_depth_{i}" if args.task == "test" else "pose_depth")
                     np.save(stem + ".npy", extra[2].cpu().numpy())
                     Image.fromarray(depth_to_grey(extra[2], extra[3], near, far), "L").save(stem + ".png")
+                elif kind == "normal":
+                    stem = os.path.join(args.out, f"{runner.cfg.exp_name}_normal_{i}" if args.task == "test" else "pose_normal")
+                    np.save(stem + ".npy", extra[2].cpu().numpy())
+                    Image.fromarray(normal_to_rgb(extra[2], extra[3]), "RGB").save(stem + ".png")
             rng0 = s.rng.copy()
         new = res["new"]
         row.update(frames=len(views), W=W, H=H, ms=summary(new["ms"]), rounds=round(statistics.mean(new["rounds"]), 2),
@@ -192,6 +237,11 @@ def main():
             over = [x - y for x, y in zip(dp["ms"], new["ms"])]
             row["depth"] = dict(ms=summary(dp["ms"]), overhead_ms=summary(over), psnr=round(statistics.mean(dp["psnr"]), 3),
                                 near_far=[round(near, 4), round(far, 4)])
+        if args.normals:
+            nm = res["normal"]
+            over = [x - y for x, y in zip(nm["ms"], new["ms"])]
+            row["normals"] = dict(ms=summary(nm["ms"]), overhead_ms=summary(over), psnr=round(statistics.mean(nm["psnr"]), 3),
+                                  kernel=density_grad_rate(runner, ds, views[0], mode))
         if args.compare:
             e0, ns = res["eps0"], res["nosync"]
             row["compare"] = {"eps0": dict(ms=summary(e0["ms"]), rounds=round(statistics.mean(e0["rounds"]), 2),
