@@ -447,6 +447,17 @@ int ngp_prepare_batch(void* stream, uint32_t n, const uint32_t* pix_index, uint3
                       const float* focal, const float* principal, const void* images_rgba, int image_is_u8, const float* bg,
                       uint32_t* img_id_out, float* rays_o, float* rays_d, float* target);
 
+/* ngp_raygen / ngp_prepare_batch through a radial-tangential lens (extends dataset/dataset.py:123-126 and ray_sampler.h:37, which read
+ * k1, k2, p1, p2 into camera_distortion and never apply them): distortion is a 16-byte aligned (n_img, 4) f32 device array of every
+ * image's (k1, k2, p1, p2).  Each pixel's normalised coordinate ((u - cx)/fx, (v - cy)/fy) is undistorted by Newton's method in fp32
+ * (OpenCV's model, y down) before it is turned into a direction.  prepare_batch_lens gives the rays of raygen_lens bit for bit and the
+ * targets of ngp_prepare_batch bit for bit.  A NULL distortion is an error; for a pinhole capture call the entry points above. */
+int ngp_raygen_lens(void* stream, uint32_t n, const uint32_t* pix_index, uint32_t W, uint32_t H, const float* xforms,
+                    const float* focal, const float* principal, const float* distortion, uint32_t* img_id_out, float* rays_o, float* rays_d);
+int ngp_prepare_batch_lens(void* stream, uint32_t n, const uint32_t* pix_index, uint32_t W, uint32_t H, const float* xforms,
+                           const float* focal, const float* principal, const float* distortion, const void* images_rgba, int image_is_u8,
+                           const float* bg, uint32_t* img_id_out, float* rays_o, float* rays_d, float* target);
+
 /* target = rgb*a + bg*(1-a) (runner/runner.py:68) for a batch whose RGBA (n,4) f32 is already gathered (host-fed ray batches) */
 int ngp_blend_target(void* stream, uint32_t n, const float* rgba, const float* bg, float* target);
 

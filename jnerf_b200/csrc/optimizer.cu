@@ -7,6 +7,7 @@
 // = 30 B/param for the fp16 table -> HBM-bound (DESIGN.md).  Optimizer state is fp32; `master` is the EMA's
 // `values` buffer and doubles as the fp32 master copy of fp16 parameters (documented deviation, SURVEY.md 8c).
 #include "train_common.cuh"
+#include "lens.cuh"
 #include <cmath>
 #include <cstring>
 
@@ -156,15 +157,19 @@ __global__ void __launch_bounds__(SWEEP_THREADS) train_sweep_kernel(uint64_t n_e
     }
 }
 
+// LENS: the pixel's normalised coordinate is undistorted through image id's (k1, k2, p1, p2) = lens[id] first (lens.cuh); without it,
+// a pinhole ray, as the reference builds every ray.
+template <bool LENS>
 __global__ void raygen_kernel(uint32_t n, const uint32_t* __restrict__ pix, uint32_t W, uint32_t H, const float* __restrict__ xforms,
                               const float* __restrict__ focal, const float* __restrict__ principal, uint32_t* __restrict__ img_id,
-                              float* __restrict__ rays_o, float* __restrict__ rays_d) {
+                              float* __restrict__ rays_o, float* __restrict__ rays_d, const float4* __restrict__ lens) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const uint32_t id = pix[i] / (H * W), off = pix[i] % (H * W);                  // dataset.py:173-174
     const float* m = xforms + 12 * (size_t)id;                                     // column-major 3x4
     const float x = ((off % W) + 0.5f) / W, y = ((off / W) + 0.5f) / H;            // :180-181
-    const float dx = (x - principal[2 * id]) * W / focal[2 * id], dy = (y - principal[2 * id + 1]) * H / focal[2 * id + 1];
+    float dx = (x - principal[2 * id]) * W / focal[2 * id], dy = (y - principal[2 * id + 1]) * H / focal[2 * id + 1];
+    if constexpr (LENS) lens_undistort(dx, dy, lens[id]);
     const float d0 = m[0] * dx + m[3] * dy + m[6], d1 = m[1] * dx + m[4] * dy + m[7], d2 = m[2] * dx + m[5] * dy + m[8];
     const float nrm = fmaxf(sqrtf(d0 * d0 + d1 * d1 + d2 * d2), 1e-12f);           // jt.normalize
     img_id[i] = id;
@@ -173,18 +178,20 @@ __global__ void raygen_kernel(uint32_t n, const uint32_t* __restrict__ pix, uint
 }
 
 // N2 fused: ray generation + RGBA gather + target = rgb*a + bg*(1-a)  (dataset.py:172-188, runner.py:66-68) in one launch.
-template <typename IMG>
+// LENS as in raygen_kernel: the same rays, bit for bit; the target lookup and blend do not depend on it.
+template <typename IMG, bool LENS>
 __global__ void prepare_batch_kernel(uint32_t n, const uint32_t* __restrict__ pix, uint32_t W, uint32_t H, const float* __restrict__ xforms,
                                      const float* __restrict__ focal, const float* __restrict__ principal, const IMG* __restrict__ images,
                                      const float* __restrict__ bg, uint32_t* __restrict__ img_id, float* __restrict__ rays_o,
-                                     float* __restrict__ rays_d, float* __restrict__ target) {
+                                     float* __restrict__ rays_d, float* __restrict__ target, const float4* __restrict__ lens) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const uint32_t px = pix[i];
     const uint32_t id = px / (H * W), off = px % (H * W);
     const float* m = xforms + 12 * (size_t)id;
     const float x = ((off % W) + 0.5f) / W, y = ((off / W) + 0.5f) / H;
-    const float dx = (x - principal[2 * id]) * W / focal[2 * id], dy = (y - principal[2 * id + 1]) * H / focal[2 * id + 1];
+    float dx = (x - principal[2 * id]) * W / focal[2 * id], dy = (y - principal[2 * id + 1]) * H / focal[2 * id + 1];
+    if constexpr (LENS) lens_undistort(dx, dy, lens[id]);
     const float d0 = m[0] * dx + m[3] * dy + m[6], d1 = m[1] * dx + m[4] * dy + m[7], d2 = m[2] * dx + m[5] * dy + m[8];
     const float nrm = fmaxf(sqrtf(d0 * d0 + d1 * d1 + d2 * d2), 1e-12f);
     img_id[i] = id;
@@ -349,6 +356,14 @@ __global__ void dp_wait_kernel(const uint32_t* my_flags, int W, uint32_t epoch) 
     if (threadIdx.x < W) wait_flag(my_flags + DP_FLAG_DONE + threadIdx.x, epoch);
 }
 
+template <bool LENS>
+void launch_prepare_batch(cudaStream_t s, uint32_t n, const uint32_t* pix_index, uint32_t W, uint32_t H, const float* xforms,
+                                 const float* focal, const float* principal, const void* images_rgba, int image_is_u8, const float* bg,
+                                 uint32_t* img_id_out, float* rays_o, float* rays_d, float* target, const float4* lens) {
+    if (image_is_u8) prepare_batch_kernel<uint8_t, LENS><<<(n + 127) / 128, 128, 0, s>>>(n, pix_index, W, H, xforms, focal, principal, (const uint8_t*)images_rgba, bg, img_id_out, rays_o, rays_d, target, lens);
+    else prepare_batch_kernel<float, LENS><<<(n + 127) / 128, 128, 0, s>>>(n, pix_index, W, H, xforms, focal, principal, (const float*)images_rgba, bg, img_id_out, rays_o, rays_d, target, lens);
+}
+
 }  // namespace
 
 extern "C" {
@@ -463,9 +478,20 @@ int ngp_prepare_batch(void* stream, uint32_t n, const uint32_t* pix_index, uint3
                       const float* principal, const void* images_rgba, int image_is_u8, const float* bg, uint32_t* img_id_out, float* rays_o,
                       float* rays_d, float* target) {
     if (n == 0) return 0;
-    cudaStream_t s = (cudaStream_t)stream;
-    if (image_is_u8) prepare_batch_kernel<uint8_t><<<(n + 127) / 128, 128, 0, s>>>(n, pix_index, W, H, xforms, focal, principal, (const uint8_t*)images_rgba, bg, img_id_out, rays_o, rays_d, target);
-    else prepare_batch_kernel<float><<<(n + 127) / 128, 128, 0, s>>>(n, pix_index, W, H, xforms, focal, principal, (const float*)images_rgba, bg, img_id_out, rays_o, rays_d, target);
+    launch_prepare_batch<false>((cudaStream_t)stream, n, pix_index, W, H, xforms, focal, principal, images_rgba, image_is_u8, bg, img_id_out, rays_o,
+                                rays_d, target, nullptr);
+    NGP_LAUNCH_CHECK();
+    return 0;
+}
+
+int ngp_prepare_batch_lens(void* stream, uint32_t n, const uint32_t* pix_index, uint32_t W, uint32_t H, const float* xforms, const float* focal,
+                           const float* principal, const float* distortion, const void* images_rgba, int image_is_u8, const float* bg,
+                           uint32_t* img_id_out, float* rays_o, float* rays_d, float* target) {
+    if (n == 0) return 0;
+    NGP_REQUIRE(distortion != nullptr && (reinterpret_cast<uintptr_t>(distortion) & 15) == 0,
+                "ngp_prepare_batch_lens: distortion must be a 16-byte aligned (n_images, 4) float array");
+    launch_prepare_batch<true>((cudaStream_t)stream, n, pix_index, W, H, xforms, focal, principal, images_rgba, image_is_u8, bg, img_id_out, rays_o,
+                               rays_d, target, reinterpret_cast<const float4*>(distortion));
     NGP_LAUNCH_CHECK();
     return 0;
 }
@@ -480,7 +506,19 @@ int ngp_blend_target(void* stream, uint32_t n, const float* rgba, const float* b
 int ngp_raygen(void* stream, uint32_t n, const uint32_t* pix_index, uint32_t W, uint32_t H, const float* xforms, const float* focal,
                const float* principal, uint32_t* img_id_out, float* rays_o, float* rays_d) {
     if (n == 0) return 0;
-    raygen_kernel<<<(n + 127) / 128, 128, 0, (cudaStream_t)stream>>>(n, pix_index, W, H, xforms, focal, principal, img_id_out, rays_o, rays_d);
+    raygen_kernel<false><<<(n + 127) / 128, 128, 0, (cudaStream_t)stream>>>(n, pix_index, W, H, xforms, focal, principal, img_id_out, rays_o, rays_d,
+                                                                            nullptr);
+    NGP_LAUNCH_CHECK();
+    return 0;
+}
+
+int ngp_raygen_lens(void* stream, uint32_t n, const uint32_t* pix_index, uint32_t W, uint32_t H, const float* xforms, const float* focal,
+                    const float* principal, const float* distortion, uint32_t* img_id_out, float* rays_o, float* rays_d) {
+    if (n == 0) return 0;
+    NGP_REQUIRE(distortion != nullptr && (reinterpret_cast<uintptr_t>(distortion) & 15) == 0,
+                "ngp_raygen_lens: distortion must be a 16-byte aligned (n_images, 4) float array");
+    raygen_kernel<true><<<(n + 127) / 128, 128, 0, (cudaStream_t)stream>>>(n, pix_index, W, H, xforms, focal, principal, img_id_out, rays_o, rays_d,
+                                                                           reinterpret_cast<const float4*>(distortion));
     NGP_LAUNCH_CHECK();
     return 0;
 }

@@ -53,6 +53,11 @@ SRC = {
     "grid_splat": "NGP_OK(ngp_grid_splat(0, in0_shape0, (uint32_t*)in0_p, in1_p, {dtype}, out0_p));",
     "grid_ema": "NGP_OK(ngp_grid_ema(0, out0_shape0, (float){decay}, out0_p, in0_p));",
     "grid_update_bitfield": "NGP_OK(ngp_grid_update_bitfield(0, in0_p, out1_p, (uint8_t*)out0_p, NERF_CASCADES()));",
+    # dataset/dataset.py:172-188 through the capture's lens (INTEGRATION.md section 17): inputs pix, xforms, focal, principal, distortion
+    "raygen_lens": ("NGP_OK(ngp_raygen_lens(0, in0_shape0, (uint32_t*)in0_p, {W}, {H}, in1_p, in2_p, in3_p, in4_p, (uint32_t*)out0_p, out1_p, "
+                    "out2_p));"),
+    "prepare_batch_lens": ("NGP_OK(ngp_prepare_batch_lens(0, in0_shape0, (uint32_t*)in0_p, {W}, {H}, in1_p, in2_p, in3_p, in4_p, in5_p, 1, in6_p, "
+                           "(uint32_t*)out0_p, out1_p, out2_p, out3_p));"),
     # optims/adam.py + optims/ema.py in one sweep per parameter tensor
     "adam_ema": "NGP_OK(ngp_adam_ema(0, in0_shape0, in0_p, NGP_F16, in1_p, NGP_F16, 1.0f, in2_p, in3_p, in4_p, (float){lr}, 0.9f, 0.99f, 1e-15f, {step}, 0.95f, 1));",
     # contrib/plenoxel: volume_render_cuvol.py (forward, and forward + MSE + backward fused), tv_grad_sparse.py, optims/svox2_optim.py,
@@ -253,3 +258,18 @@ def adam_ema(param, grad, m, v, master, lr, step):
     """optims/adam.py + optims/ema.py in one sweep (in place on all five tensors)."""
     jt = _jt()
     return jt.code(inputs=[param, grad, m, v, master], outputs=[param], cuda_header=CUDA_HEADER, cuda_src=SRC["adam_ema"].format(lr=float(lr), step=int(step)))
+
+
+def raygen_lens(pix, W, H, xforms, focal, principal, distortion):
+    """The rays of the flat pixel indices pix (uint32) through every image's (k1, k2, p1, p2) = distortion (n_img, 4): (img_ids, rays_o,
+    rays_d)."""
+    n = pix.shape[0]
+    return _code([(n,), (n, 3), (n, 3)], ["uint32", "float32", "float32"], [pix, xforms, focal, principal, distortion],
+                 SRC["raygen_lens"].format(W=int(W), H=int(H)))
+
+
+def prepare_batch_lens(pix, W, H, xforms, focal, principal, distortion, images_u8, bg):
+    """raygen_lens + the pixels' uint8 RGBA blended over bg (n, 3): (img_ids, rays_o, rays_d, target)."""
+    n = pix.shape[0]
+    return _code([(n,), (n, 3), (n, 3), (n, 3)], ["uint32", "float32", "float32", "float32"],
+                 [pix, xforms, focal, principal, distortion, images_u8, bg], SRC["prepare_batch_lens"].format(W=int(W), H=int(H)))

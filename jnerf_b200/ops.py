@@ -663,25 +663,50 @@ def adam_ema(param, grad, m, v, master, lr, step, beta1=0.9, beta2=0.99, eps=1e-
              float(lr), float(beta1), float(beta2), float(eps), int(step), float(ema_decay), int(zero_grad))
 
 
-def raygen(pix, W, H, xforms, focal, principal):
+def lens_of(distortion):
+    """`distortion` -- None or an (n_images, 4) f32 device tensor of (k1, k2, p1, p2) -- when it has a non-zero coefficient, else None:
+    a lens of zeros takes the pinhole kernels, bit for bit.  The answer is read from the device once per version of the tensor (kept on
+    the tensor), so a training step that passes the same lens again does not synchronise."""
+    if distortion is None:
+        return None
+    seen = getattr(distortion, "_ngp_lens_nonzero", None)
+    if seen is None or seen[0] != distortion._version:
+        seen = (distortion._version, bool(distortion.any()))
+        distortion._ngp_lens_nonzero = seen
+    return distortion if seen[1] else None
+
+
+def raygen(pix, W, H, xforms, focal, principal, distortion=None):
+    """(img_ids, rays_o, rays_d) of the flat pixel indices pix (image * H * W + row * W + column); with a non-zero `distortion` (see
+    lens_of) every pixel is undistorted through its image's lens first (ngp_raygen_lens)."""
     n = pix.numel()
     dev = pix.device
     img = torch.empty(n, dtype=torch.int32, device=dev)
     o = torch.empty((n, 3), dtype=torch.float32, device=dev)
     d = torch.empty((n, 3), dtype=torch.float32, device=dev)
-    lib.call("ngp_raygen", _stream(), n, _p(pix), W, H, _p(xforms), _p(focal), _p(principal), _p(img), _p(o), _p(d))
+    lens = lens_of(distortion)
+    if lens is None:
+        lib.call("ngp_raygen", _stream(), n, _p(pix), W, H, _p(xforms), _p(focal), _p(principal), _p(img), _p(o), _p(d))
+    else:
+        lib.call("ngp_raygen_lens", _stream(), n, _p(pix), W, H, _p(xforms), _p(focal), _p(principal), _p(lens), _p(img), _p(o), _p(d))
     return img, o, d
 
 
-def prepare_batch(pix, W, H, xforms, focal, principal, images, bg):
+def prepare_batch(pix, W, H, xforms, focal, principal, images, bg, distortion=None):
+    """raygen + the pixels' RGBA blended over bg in one launch: (img_ids, rays_o, rays_d, target)."""
     n = pix.numel()
     dev = pix.device
     img = torch.empty(n, dtype=torch.int32, device=dev)
     o = torch.empty((n, 3), dtype=torch.float32, device=dev)
     d = torch.empty((n, 3), dtype=torch.float32, device=dev)
     target = torch.empty((n, 3), dtype=torch.float32, device=dev)
-    lib.call("ngp_prepare_batch", _stream(), n, _p(pix), W, H, _p(xforms), _p(focal), _p(principal), _p(images), int(images.dtype == torch.uint8),
-             _p(bg), _p(img), _p(o), _p(d), _p(target))
+    lens = lens_of(distortion)
+    if lens is None:
+        lib.call("ngp_prepare_batch", _stream(), n, _p(pix), W, H, _p(xforms), _p(focal), _p(principal), _p(images), int(images.dtype == torch.uint8),
+                 _p(bg), _p(img), _p(o), _p(d), _p(target))
+    else:
+        lib.call("ngp_prepare_batch_lens", _stream(), n, _p(pix), W, H, _p(xforms), _p(focal), _p(principal), _p(lens), _p(images),
+                 int(images.dtype == torch.uint8), _p(bg), _p(img), _p(o), _p(d), _p(target))
     return img, o, d, target
 
 

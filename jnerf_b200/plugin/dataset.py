@@ -4,7 +4,9 @@ reference downloads it at run time, dataset_util.py:101-109); write_synthetic_ll
 
 All expose what the sampler / runner read: n_images, resolution [W,H], aabb_scale, aabb_range, metadata (n,11),
 focal_lengths (n,2), transforms_gpu (n, 3x4 stored column-major = 12 floats, dataset.py:164-165), image_data
-(n, H*W, 4), batch_size and __next__() -> (img_ids, rays_o, rays_d, rgba)."""
+(n, H*W, 4), batch_size and __next__() -> (img_ids, rays_o, rays_d, rgba).  With `undistort=True` (NerfDataset, SyntheticNerfDataset) also
+distortion (n,4) = every image's (k1, k2, p1, p2), in metadata[:, 0:4] too, and, for a non-zero lens, focal_eff (n,2); otherwise distortion
+is None and metadata[:, 0:4] stays 0, as in the reference."""
 import json
 import math
 import os
@@ -33,6 +35,90 @@ def matrix_nerf2ngp(matrix, scale, offset, correct_pose=(1, -1, -1)):
     return m[[1, 2, 0]]
 
 
+LENS_KEYS = ("k1", "k2", "p1", "p2")
+
+
+def read_lens(json_data):
+    """(k1, k2, p1, p2) of an Instant-NGP transforms.json (a missing key counts as 0).  The radial-tangential model below is all the ray
+    kernels invert: a fisheye camera or a non-zero k3 / k4 raises NotImplementedError."""
+    model = str(json_data.get("camera_model", ""))
+    if json_data.get("is_fisheye", False) or "FISHEYE" in model.upper():
+        raise NotImplementedError(f"undistort: fisheye cameras (camera_model {model!r}, is_fisheye {json_data.get('is_fisheye', False)}) are not "
+                                  "supported; only the radial-tangential model k1, k2, p1, p2 is")
+    for k in ("k3", "k4"):
+        if float(json_data.get(k, 0.0)) != 0.0:
+            raise NotImplementedError(f"undistort: {k} = {json_data[k]} is not supported; only the radial-tangential model k1, k2, p1, p2 is")
+    return tuple(float(json_data.get(k, 0.0)) for k in LENS_KEYS)
+
+
+def lens_distort(x, y, k):
+    """OpenCV's radial-tangential model (k3 = 0) in fp64: undistorted normalised camera coordinates (x right, y down) -> distorted ones,
+    the ((u - cx)/fx, (v - cy)/fy) of the pixel (u, v).  csrc/lens.cuh is the device form."""
+    k1, k2, p1, p2 = k
+    x, y = np.asarray(x, np.float64), np.asarray(y, np.float64)
+    r2 = x * x + y * y
+    rad = 1 + r2 * (k1 + r2 * k2)
+    return x * rad + 2 * p1 * x * y + p2 * (r2 + 2 * x * x), y * rad + p1 * (r2 + 2 * y * y) + 2 * p2 * x * y
+
+
+def _lens_jacobian(x, y, k):
+    k1, k2, p1, p2 = k
+    r2 = x * x + y * y
+    rad, drad = 1 + r2 * (k1 + r2 * k2), 2 * (k1 + 2 * k2 * r2)
+    return (rad + x * x * drad + 2 * p1 * y + 6 * p2 * x, x * y * drad + 2 * p1 * x + 2 * p2 * y,
+            rad + y * y * drad + 6 * p1 * y + 2 * p2 * x)                # j11, j12 = j21, j22
+
+
+def lens_undistort(xd, yd, k, iters=50):
+    """The inverse of lens_distort in fp64: Newton's method from the distorted point, run to convergence."""
+    xd, yd = np.asarray(xd, np.float64), np.asarray(yd, np.float64)
+    x, y = xd.copy(), yd.copy()
+    for _ in range(iters):
+        fx, fy = lens_distort(x, y, k)
+        fx, fy = fx - xd, fy - yd
+        j11, j12, j22 = _lens_jacobian(x, y, k)
+        det = j11 * j22 - j12 * j12
+        sx, sy = (j22 * fx - j12 * fy) / det, (j11 * fy - j12 * fx) / det
+        x, y = x - sx, y - sy
+        if np.max(np.abs(sx) + np.abs(sy), initial=0.0) < 1e-15:
+            break
+    return x, y
+
+
+def check_lens(k, W, H, focal, c, n_angles=512, n_radii=2048):
+    """ValueError unless the lens k maps the undistorted plane one to one onto the whole image: along every direction from the optical
+    axis, the Jacobian determinant of lens_distort stays positive (fp64) until the distorted point is as far out as the image's farthest
+    corner.  A lens that folds over inside the image has pixels with two undistorted directions, and the kernels' Newton solve may land
+    on either."""
+    xs, ys = (np.array([0.0, W]) - c[0]) / focal[0], (np.array([0.0, H]) - c[1]) / focal[1]
+    reach = math.hypot(np.abs(xs).max(), np.abs(ys).max())
+    th = np.linspace(0, 2 * math.pi, n_angles, endpoint=False)[:, None]
+    r = np.linspace(0, 4 * reach, n_radii)[None, :]
+    x, y = r * np.cos(th), r * np.sin(th)
+    j11, j12, j22 = _lens_jacobian(x, y, k)
+    xd, yd = lens_distort(x, y, k)
+    out = np.hypot(xd, yd) >= reach
+    first_out = np.where(out.any(1), out.argmax(1), n_radii)                       # first sample of every direction beyond the corner
+    inside = np.arange(n_radii)[None, :] <= first_out[:, None]
+    named = ", ".join(f"{n} = {v:g}" for n, v in zip(LENS_KEYS, k))
+    if (first_out == n_radii).any():
+        raise ValueError(f"undistort: the lens ({named}) never reaches the image's farthest corner; it cannot be inverted over the image")
+    if ((j11 * j22 - j12 * j12 <= 0) & inside).any():
+        raise ValueError(f"undistort: the lens ({named}) folds over inside the {W}x{H} image (its Jacobian determinant reaches 0 before the "
+                         "farthest corner); the ray kernels cannot invert it reliably")
+
+
+def lens_extent(k, W, H, focal, c):
+    """(max |x_u|, max |y_u|): the undistorted extent, in fp64, of the pixel centres and corners of a W x H image.  check_lens makes the
+    map one to one, so the extremes lie on the image's border: its corners and the centres of its outer pixels are solved."""
+    cu, cv = np.arange(W + 1.0), np.arange(H + 1.0)                                  # corners
+    pu, pv = np.arange(W) + 0.5, np.arange(H) + 0.5                                  # centres
+    bu = np.concatenate([cu, cu, np.zeros(H + 1), np.full(H + 1, float(W)), pu, pu, np.full(H, 0.5), np.full(H, W - 0.5)])
+    bv = np.concatenate([np.zeros(W + 1), np.full(W + 1, float(H)), cv, cv, np.full(W, 0.5), np.full(W, H - 0.5), pv, pv])
+    x, y = lens_undistort((bu - c[0]) / focal[0], (bv - c[1]) / focal[1], k)
+    return float(np.abs(x).max()), float(np.abs(y).max())
+
+
 class _RayBatcher:
     """Pixel shuffling + device ray generation shared by both datasets (dataset.py:57-66,172-188)."""
 
@@ -46,6 +132,16 @@ class _RayBatcher:
         md = np.zeros((self.n_images, 11), np.float32)
         md[:, 4], md[:, 5] = self._cx / self.W, self._cy / self.H
         md[:, 6], md[:, 7] = self._focal
+        lens = getattr(self, "_lens", None)                                  # (k1, k2, p1, p2) with undistort=True, else None
+        self.distortion = None
+        if lens is not None:
+            md[:, 0:4] = lens                                                # the reference's slots (dataset.py:123-126)
+            self.distortion = torch.tensor([lens] * self.n_images, dtype=torch.float32, device=dev)
+            if any(lens):
+                # the occupancy grid's visibility frustum (grid_mark_untrained) is symmetric, |x| < (W/2) / f: with these focal lengths
+                # it holds every direction a pixel of the capture sees through the lens
+                ex, ey = lens_extent(lens, self.W, self.H, self._focal, (self._cx, self._cy))
+                self.focal_eff = torch.tensor([[self.W / 2 / ex, self.H / 2 / ey]] * self.n_images, dtype=torch.float32, device=dev)
         self.metadata = torch.from_numpy(md).to(dev)
         self.principal = self.metadata[:, 4:6].contiguous()
         self.aabb_range = (0.5 - self.aabb_scale / 2, 0.5 + self.aabb_scale / 2)    # dataset.py:155-156
@@ -63,8 +159,11 @@ class _RayBatcher:
         self.idx_now += n
         return self.shuffle_index[start:start + n]
 
-    def rays_for(self, pix):
-        return ops.raygen(pix.contiguous(), self.W, self.H, self.transforms_gpu, self.focal_lengths, self.principal)
+    def rays_for(self, pix, distortion=None):
+        """(img_ids, rays_o, rays_d) of the flat pixel indices pix, through the dataset's lens (or `distortion`) when it has one."""
+        distortion = self.distortion if distortion is None else distortion
+        lens = {} if distortion is None else dict(distortion=distortion)
+        return ops.raygen(pix.contiguous(), self.W, self.H, self.transforms_gpu, self.focal_lengths, self.principal, **lens)
 
     def rgba_for(self, pix):
         v = self.image_data.reshape(-1, 4)[pix.long()]
@@ -85,7 +184,9 @@ class _RayBatcher:
 @DATASETS.register_module()
 class NerfDataset(_RayBatcher):
     def __init__(self, root_dir, batch_size, mode="train", H=0, W=0, correct_pose=(1, -1, -1), aabb_scale=None, scale=None, offset=None,
-                 img_alpha=True, to_jt=True, have_img=True, preload_shuffle=True, seed=0):
+                 img_alpha=True, to_jt=True, have_img=True, preload_shuffle=True, seed=0, undistort=False):
+        """undistort: read k1, k2, p1, p2 from the split's json and make every ray of its images through that lens (check_lens); off,
+        as in the reference, every ray is a pinhole ray."""
         from PIL import Image
         assert mode in ("train", "val", "test")
         self.root_dir, self.batch_size, self.mode, self.seed = root_dir, batch_size, mode, seed
@@ -138,6 +239,9 @@ class NerfDataset(_RayBatcher):
         else:
             raise RuntimeError("Couldn't read fov.")
         self._cx, self._cy = json_data.get("cx", self.W / 2), json_data.get("cy", self.H / 2)
+        if undistort:
+            self._lens = read_lens(json_data)
+            check_lens(self._lens, self.W, self.H, self._focal, (self._cx, self._cy))
         self.aabb_scale = json_data.get("aabb_scale", 1) if aabb_scale is None else aabb_scale
         self.have_img = have_img
         self._finish_init()
@@ -333,7 +437,9 @@ class SyntheticNerfDataset(_RayBatcher):
                elevation=(-8.0, 30.0), obj_scale=2.2, backdrop_radius=1.9)
 
     def __init__(self, batch_size=4096, mode="train", n_images=100, H=800, W=800, camera_angle_x=0.6911112070083618, aabb_scale=1, seed=0,
-                 root_dir=None, preload_shuffle=True, style="lego"):
+                 root_dir=None, preload_shuffle=True, style="lego", distortion=None, undistort=False):
+        """distortion: (k1, k2, p1, p2) of the lens the images are taken through (None: a pinhole camera); undistort: make the rays
+        through that lens, as NerfDataset(undistort=True) does with a capture's json."""
         assert style in ("lego", "fox")
         self.batch_size, self.mode, self.seed, self.style = batch_size, mode, seed, style
         self.scale, self.offset = NERF_SCALE, [0.5, 0.5, 0.5]
@@ -362,18 +468,28 @@ class SyntheticNerfDataset(_RayBatcher):
         self.correct_pose = (1, -1, -1)
         self._xforms = [matrix_nerf2ngp(m, self.scale, self.offset) for m in mats]
         self.have_img = True
+        capture = None if distortion is None else tuple(float(v) for v in distortion)
+        if capture is not None:
+            check_lens(capture, self.W, self.H, self._focal, (self._cx, self._cy))
+        if undistort:
+            self._lens = capture or (0.0, 0.0, 0.0, 0.0)
         self._finish_init()
-        self.image_data = self._render_all()
+        self.image_data = self._render_all(capture)
 
     # -- analytic renderer (NGP coordinates: world * 0.33 + 0.5, axes cycled like matrix_nerf2ngp) --------------
     def _to_ngp(self, p):
         p = np.asarray(p, np.float32) * self.scale + 0.5
         return p[[1, 2, 0]]
 
-    def _render_all(self):
+    def _render_all(self, lens=None):
+        """The images, every pixel's ray through `lens` (k1, k2, p1, p2) when one is given, whatever rays the dataset trains on."""
         out = torch.empty((self.n_images, self.H * self.W, 4), dtype=torch.uint8, device=DEVICE)
+        lens = None if lens is None or not any(lens) else torch.tensor([lens] * self.n_images, dtype=torch.float32, device=DEVICE)
         for i in range(self.n_images):
-            o, d = self.generate_rays_total_test(i)
+            if lens is None:
+                o, d = self.generate_rays_total_test(i)
+            else:
+                _, o, d = self.rays_for(torch.arange(self.H * self.W, device=DEVICE, dtype=torch.int32) + i * self.H * self.W, lens)
             out[i] = (self.shade(o, d) * 255.0 + 0.5).clamp(0, 255).to(torch.uint8)
         return out
 

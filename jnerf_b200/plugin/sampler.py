@@ -165,7 +165,10 @@ class DensityGridSampler(Module):
     def update_density_grid_nerf(self, decay, n_uniform, n_nonuniform):
         if self.cfg.m_training_step == 0:
             self.density_grid.zero_()
-            ops.grid_mark_untrained(self.density_grid, self.dataset.focal_lengths, self.dataset.transforms_gpu, self.image_resolutions)
+            # through a lens the images see further out than a pinhole of the same focal length: the dataset's effective focal lengths
+            focal = getattr(self.dataset, "focal_eff", None)
+            ops.grid_mark_untrained(self.density_grid, self.dataset.focal_lengths if focal is None else focal, self.dataset.transforms_gpu,
+                                    self.image_resolutions)
         self.density_grid_tmp.zero_()
         parts_p, parts_i = [], []
         for n, thresh in ((n_uniform, -0.01), (n_nonuniform, self.NERF_MIN_OPTICAL_THICKNESS)):

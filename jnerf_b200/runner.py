@@ -227,8 +227,10 @@ class Runner:
                 lo, hi = dp.shard_range(R, self.rank)
                 pix, bg = pix[lo:hi], bg[lo:hi]
             bg = bg.contiguous()
+            lens = getattr(ds, "distortion", None)                       # every rank the same lens
             img_ids, rays_o, rays_d, target = ops.prepare_batch(pix.contiguous(), ds.W, ds.H, ds.transforms_gpu, ds.focal_lengths,
-                                                                ds.principal, ds.image_data, bg)    # dataset.py:172-188 + runner.py:68
+                                                                ds.principal, ds.image_data, bg,
+                                                                **({} if lens is None else dict(distortion=lens)))  # dataset.py:172-188 + runner.py:68
             return img_ids, rays_o, rays_d, bg, target
         img_ids, rays_o, rays_d, rgba = batch
         R = rays_o.shape[0]
@@ -1045,13 +1047,16 @@ def lego_cfg(fp16=True, synthetic=True, **over):
     return c
 
 
-def fox_cfg(fp16=True, synthetic=True, **over):
+def fox_cfg(fp16=True, synthetic=True, undistort=False, **over):
     """projects/ngp/configs/ngp_fox.py key for key (BASELINE config #3: aabb_scale 4 from the capture's transforms, cone stepping
     `const_dt=False`, fp16, no validation split); `synthetic` swaps data/fox for the procedural stand-in with the capture's
-    resolution, intrinsics, camera arc and aabb_scale (plugin/dataset.py: SyntheticNerfDataset(style="fox"))."""
+    resolution, intrinsics, camera arc and aabb_scale (plugin/dataset.py: SyntheticNerfDataset(style="fox")).  `undistort` sets the
+    datasets' key of that name in every split: training and test rays through the capture's lens (DESIGN.md section 7)."""
     c = lego_cfg(fp16=fp16, synthetic=synthetic)
     ds_type = "SyntheticNerfDataset" if synthetic else "NerfDataset"
     extra = dict(style="fox") if synthetic else {}
+    if undistort:
+        extra.update(undistort=True)
     c.update(dataset=dict(train=dict(type=ds_type, root_dir="data/fox", batch_size=4096, mode="train", **extra),
                           test=dict(type=ds_type, root_dir="data/fox", batch_size=4096, mode="test", preload_shuffle=False, **extra)),
              exp_name="fox", const_dt=False)

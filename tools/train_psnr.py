@@ -3,6 +3,7 @@
 
     python tools/train_psnr.py [--steps 5000] [--images 100] [--res 400] [--evals 500,1000,2000,5000] [--out gpurun_out/psnr.json]
     python tools/train_psnr.py --workload llff [--data-dir CAPTURE] [--images 40]
+    python tools/train_psnr.py --workload fox [--data-dir CAPTURE] [--undistort] [--distortion K1 K2 P1 P2]
 
 This is the quality check that goes with bench.py's throughput number: same Runner.train_step path, same configuration
 (projects/ngp/configs/ngp_base.py + fp16), validation views drawn from cameras the model never trains on
@@ -32,7 +33,14 @@ def main():
                     help="fox = projects/ngp/configs/ngp_fox.py (aabb_scale from the capture, cone stepping); PSNR on training views (the capture has no val split). "
                          "llff = projects/ngp/configs/ngp_llff.py (aabb_scale 64: 7 occupancy cascades, every 8th view held out) on --data-dir, an LLFF "
                          "capture (poses_bounds.npy + images/), or on the forward-facing stand-in written to a temporary directory")
+    ap.add_argument("--undistort", action="store_true", help="fox: train and evaluate through the capture's lens (datasets' undistort=True)")
+    ap.add_argument("--distortion", type=float, nargs=4, default=None, metavar=("K1", "K2", "P1", "P2"),
+                    help="fox stand-in: take its images through this lens (k1 k2 p1 p2)")
     args = ap.parse_args()
+    if (args.undistort or args.distortion) and args.workload != "fox":
+        ap.error("--undistort and --distortion go with --workload fox")
+    if args.distortion and args.data_dir:
+        ap.error("--distortion is the stand-in's lens; a capture brings its own in its transforms json")
 
     import torch
     from jnerf_b200 import lib, plugin  # noqa: F401
@@ -53,8 +61,10 @@ def main():
         update_cfg(**llff_cfg(root, fp16=True, seed=1))
         cfg = get_cfg()
     elif args.workload == "fox":
-        update_cfg(**fox_cfg(fp16=True, synthetic=args.data_dir is None, seed=1))
+        update_cfg(**fox_cfg(fp16=True, synthetic=args.data_dir is None, undistort=args.undistort, seed=1))
         cfg = get_cfg()
+        if args.distortion:
+            cfg.dataset.train.distortion = cfg.dataset.test.distortion = list(args.distortion)
         if args.data_dir:
             cfg.dataset.train.root_dir = args.data_dir
             cfg.dataset.test.root_dir = args.data_dir
@@ -96,7 +106,8 @@ def main():
         res["config"] = f"ngp_base + fp16 on {args.data_dir}, {args.val_images} validation views"
     if args.workload == "fox":
         res["config"] = (f"ngp_fox.py (fp16, cone stepping) on {args.data_dir or 'the synthetic fox stand-in'}, PSNR on {args.val_images} training views "
-                         f"(the capture has no validation split)")
+                         f"(the capture has no validation split)" + (f", images through the lens {args.distortion}" if args.distortion else "")
+                         + (", rays undistorted" if args.undistort else ""))
     if args.workload == "llff":
         res["config"] = (f"ngp_llff.py (fp16, cone stepping, aabb_scale 64) on {args.data_dir or 'the forward-facing stand-in'}: "
                          f"{runner.dataset['train'].n_images} training views of {runner.W}x{runner.H}, PSNR on {args.val_images} held-out views")
