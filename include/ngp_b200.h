@@ -397,6 +397,11 @@ int ngp_render_composite_round_normals(void* stream, uint32_t n_rays, uint32_t c
 /* ---- R10 occupancy-grid maintenance (DGS/density_grid_sampler.py:204-264 + five headers) ------------- */
 int ngp_grid_mark_untrained(void* stream, uint32_t n_elements, float* grid, uint32_t n_images, const float* focal_lengths,
                             const float* xforms, int res_x, int res_y);
+/* ngp_grid_mark_untrained for captures whose frames carry their own cameras (extends mark_untrained_density_grid.h, which takes one
+ * symmetric frustum per image): extents is a 16-byte aligned (n_images, 4) f32 device array of every image's normalised frustum
+ * (x_lo, x_hi, y_lo, y_hi) in camera coordinates (x right, y down, z forward), signed, so an off-centre principal point or a lens is
+ * represented exactly. */
+int ngp_grid_mark_untrained_cams(void* stream, uint32_t n_elements, float* grid, uint32_t n_images, const float* extents, const float* xforms);
 int ngp_grid_generate_samples(void* stream, uint32_t n_elements, uint64_t rng_state, uint64_t rng_inc, const uint32_t* step_dev,
                               float aabb_lo, float aabb_hi, const float* grid_in, float* positions_out, uint32_t* indices_out,
                               uint32_t n_cascades, float thresh);
@@ -457,6 +462,19 @@ int ngp_raygen_lens(void* stream, uint32_t n, const uint32_t* pix_index, uint32_
 int ngp_prepare_batch_lens(void* stream, uint32_t n, const uint32_t* pix_index, uint32_t W, uint32_t H, const float* xforms,
                            const float* focal, const float* principal, const float* distortion, const void* images_rgba, int image_is_u8,
                            const float* bg, uint32_t* img_id_out, float* rays_o, float* rays_d, float* target);
+
+/* ngp_raygen / ngp_prepare_batch for captures whose frames carry their own cameras and image sizes (extends dataset/dataset.py:172-188,
+ * which takes one W, H for all images): image i is wh[i] = (w, h) pixels (an 8-byte aligned (n_images, 2) uint32 device array) and
+ * owns the global pixel ids [pixel_offsets[i], pixel_offsets[i+1]) of the ragged (total_pixels, 4) RGBA table, row-major; pixel_offsets
+ * holds the n_images + 1 prefix sums of w*h.  A NULL distortion builds pinhole rays, else every pixel goes through its image's lens as in
+ * ngp_raygen_lens.  On a capture whose images all share one size the rays and targets are those of ngp_raygen / ngp_prepare_batch (or
+ * their _lens forms) bit for bit. */
+int ngp_raygen_cams(void* stream, uint32_t n, const uint32_t* pix_index, uint32_t n_images, const uint32_t* pixel_offsets, const uint32_t* wh,
+                    const float* xforms, const float* focal, const float* principal, const float* distortion, uint32_t* img_id_out, float* rays_o,
+                    float* rays_d);
+int ngp_prepare_batch_cams(void* stream, uint32_t n, const uint32_t* pix_index, uint32_t n_images, const uint32_t* pixel_offsets, const uint32_t* wh,
+                           const float* xforms, const float* focal, const float* principal, const float* distortion, const void* images_rgba,
+                           int image_is_u8, const float* bg, uint32_t* img_id_out, float* rays_o, float* rays_d, float* target);
 
 /* target = rgb*a + bg*(1-a) (runner/runner.py:68) for a batch whose RGBA (n,4) f32 is already gathered (host-fed ray batches) */
 int ngp_blend_target(void* stream, uint32_t n, const float* rgba, const float* bg, float* target);

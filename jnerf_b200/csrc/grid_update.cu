@@ -35,6 +35,35 @@ __global__ void mark_untrained_kernel(uint32_t n_elements, float* __restrict__ g
     if ((grid[i] < 0) != (count <= 0)) grid[i] = (count > 0) ? 0.f : -1.f;
 }
 
+// mark_untrained_kernel for captures whose frames carry their own cameras: a cell is seen by image j when its bounding sphere reaches
+// into the image's frustum, x_lo < c_x / c_z < x_hi and y_lo < c_y / c_z < y_hi, with the image's normalised extents (x_lo, x_hi,
+// y_lo, y_hi) = extents[j] computed on the host (plugin/dataset.py: frame_extent) from its size, principal point, focal lengths and
+// lens.  The symmetric |c_x| < c_z (W/2) / f test above holds only for a centred principal point.
+__global__ void mark_untrained_cams_kernel(uint32_t n_elements, float* __restrict__ grid, uint32_t n_images, const float4* __restrict__ extents,
+                                           const float* __restrict__ xforms) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_elements) return;
+    const uint32_t level = i / NERF_GRID_N, pos_idx = i % NERF_GRID_N;
+    const uint32_t x = morton3D_invert(pos_idx >> 0), y = morton3D_invert(pos_idx >> 1), z = morton3D_invert(pos_idx >> 2);
+    const float sc = scalbnf(1.0f, (int)level);
+    const float p[3] = {(((float)x + 0.5f) / NERF_GRIDSIZE - 0.5f) * sc + 0.5f, (((float)y + 0.5f) / NERF_GRIDSIZE - 0.5f) * sc + 0.5f,
+                        (((float)z + 0.5f) / NERF_GRIDSIZE - 0.5f) * sc + 0.5f};
+    const float voxel_radius = 0.5f * 1.73205080757f * sc / NERF_GRIDSIZE;
+    bool seen = false;
+    for (uint32_t j = 0; j < n_images && !seen; ++j) {
+        const float* m = xforms + 12 * j;
+        const float pl[3] = {p[0] - __ldg(m + 9), p[1] - __ldg(m + 10), p[2] - __ldg(m + 11)};
+        const float cx = pl[0] * __ldg(m + 0) + (pl[1] * __ldg(m + 1) + pl[2] * __ldg(m + 2));
+        const float cy = pl[0] * __ldg(m + 3) + (pl[1] * __ldg(m + 4) + pl[2] * __ldg(m + 5));
+        const float cz = pl[0] * __ldg(m + 6) + (pl[1] * __ldg(m + 7) + pl[2] * __ldg(m + 8));
+        if (cz > 0.f) {
+            const float4 e = __ldg(extents + j);
+            seen = cx + voxel_radius > cz * e.x && cx - voxel_radius < cz * e.y && cy + voxel_radius > cz * e.z && cy - voxel_radius < cz * e.w;
+        }
+    }
+    if ((grid[i] < 0) != !seen) grid[i] = seen ? 0.f : -1.f;
+}
+
 __global__ void generate_samples_kernel(uint32_t n_elements, uint64_t rng_state, uint64_t rng_inc, const uint32_t* __restrict__ step_p,
                                         float lo, float hi, const float* __restrict__ grid_in, float* __restrict__ positions,
                                         uint32_t* __restrict__ indices, uint32_t n_cascades, float thresh) {
@@ -141,6 +170,16 @@ int ngp_grid_mark_untrained(void* stream, uint32_t n_elements, float* grid, uint
     if (n_elements == 0) return 0;
     mark_untrained_kernel<<<(n_elements + 127) / 128, 128, 0, (cudaStream_t)stream>>>(n_elements, grid, n_images, focal_lengths, xforms,
                                                                                      res_x * 0.5f, res_y * 0.5f);
+    NGP_LAUNCH_CHECK();
+    return 0;
+}
+
+int ngp_grid_mark_untrained_cams(void* stream, uint32_t n_elements, float* grid, uint32_t n_images, const float* extents, const float* xforms) {
+    if (n_elements == 0) return 0;
+    NGP_REQUIRE(extents != nullptr && (reinterpret_cast<uintptr_t>(extents) & 15) == 0,
+                "ngp_grid_mark_untrained_cams: extents must be a 16-byte aligned (n_images, 4) float array");
+    mark_untrained_cams_kernel<<<(n_elements + 127) / 128, 128, 0, (cudaStream_t)stream>>>(n_elements, grid, n_images,
+                                                                                          reinterpret_cast<const float4*>(extents), xforms);
     NGP_LAUNCH_CHECK();
     return 0;
 }

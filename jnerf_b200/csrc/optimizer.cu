@@ -210,6 +210,74 @@ __global__ void prepare_batch_kernel(uint32_t n, const uint32_t* __restrict__ pi
     target[3 * (size_t)i + 2] = c.z * c.w + bg[3 * (size_t)i + 2] * ia;
 }
 
+// Captures whose frames carry their own cameras (plugin/dataset.py, per_frame_cameras): image i owns the global pixel ids
+// [offsets[i], offsets[i+1]) of a ragged, row-major table, and is wh[i] = (w, h) pixels.  The image of pixel p is found by a binary
+// search over the n_images + 1 prefix sums; off = p - offsets[id] is then the pixel's row-major offset in its own image.
+__device__ __forceinline__ uint32_t frame_of_pixel(uint32_t p, uint32_t n_images, const uint32_t* __restrict__ offsets) {
+    uint32_t lo = 0, hi = n_images;                        // offsets[lo] <= p < offsets[hi]
+    while (hi - lo > 1) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (__ldg(offsets + mid) <= p) lo = mid;
+        else hi = mid;
+    }
+    return lo;
+}
+
+// The ray of raygen_kernel<LENS> for the pixel p of a ragged capture, with the image's own W and H: the same operations in the same
+// order, so a capture whose images all share one size gives raygen_kernel's rays bit for bit.
+template <bool LENS>
+__device__ __forceinline__ uint32_t frame_ray(uint32_t p, uint32_t n_images, const uint32_t* __restrict__ offsets, const uint2* __restrict__ wh,
+                                              const float* __restrict__ xforms, const float* __restrict__ focal,
+                                              const float* __restrict__ principal, const float4* __restrict__ lens, uint32_t i,
+                                              float* __restrict__ rays_o, float* __restrict__ rays_d) {
+    const uint32_t id = frame_of_pixel(p, n_images, offsets);
+    const uint2 s = __ldg(wh + id);
+    const uint32_t W = s.x, H = s.y, off = p - __ldg(offsets + id);
+    const float* m = xforms + 12 * (size_t)id;
+    const float x = ((off % W) + 0.5f) / W, y = ((off / W) + 0.5f) / H;
+    float dx = (x - principal[2 * id]) * W / focal[2 * id], dy = (y - principal[2 * id + 1]) * H / focal[2 * id + 1];
+    if constexpr (LENS) lens_undistort(dx, dy, lens[id]);
+    const float d0 = m[0] * dx + m[3] * dy + m[6], d1 = m[1] * dx + m[4] * dy + m[7], d2 = m[2] * dx + m[5] * dy + m[8];
+    const float nrm = fmaxf(sqrtf(d0 * d0 + d1 * d1 + d2 * d2), 1e-12f);
+    rays_o[3 * (size_t)i] = m[9]; rays_o[3 * (size_t)i + 1] = m[10]; rays_o[3 * (size_t)i + 2] = m[11];
+    rays_d[3 * (size_t)i] = d0 / nrm; rays_d[3 * (size_t)i + 1] = d1 / nrm; rays_d[3 * (size_t)i + 2] = d2 / nrm;
+    return id;
+}
+
+template <bool LENS>
+__global__ void raygen_cams_kernel(uint32_t n, const uint32_t* __restrict__ pix, uint32_t n_images, const uint32_t* __restrict__ offsets,
+                                   const uint2* __restrict__ wh, const float* __restrict__ xforms, const float* __restrict__ focal,
+                                   const float* __restrict__ principal, const float4* __restrict__ lens, uint32_t* __restrict__ img_id,
+                                   float* __restrict__ rays_o, float* __restrict__ rays_d) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    img_id[i] = frame_ray<LENS>(pix[i], n_images, offsets, wh, xforms, focal, principal, lens, i, rays_o, rays_d);
+}
+
+// raygen_cams_kernel + the pixel's RGBA from the ragged (total_pixels, 4) table, blended as prepare_batch_kernel blends it
+template <typename IMG, bool LENS>
+__global__ void prepare_batch_cams_kernel(uint32_t n, const uint32_t* __restrict__ pix, uint32_t n_images, const uint32_t* __restrict__ offsets,
+                                          const uint2* __restrict__ wh, const float* __restrict__ xforms, const float* __restrict__ focal,
+                                          const float* __restrict__ principal, const float4* __restrict__ lens, const IMG* __restrict__ images,
+                                          const float* __restrict__ bg, uint32_t* __restrict__ img_id, float* __restrict__ rays_o,
+                                          float* __restrict__ rays_d, float* __restrict__ target) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint32_t px = pix[i];
+    img_id[i] = frame_ray<LENS>(px, n_images, offsets, wh, xforms, focal, principal, lens, i, rays_o, rays_d);
+    float4 c;
+    if constexpr (sizeof(IMG) == 1) {
+        const uchar4 u = reinterpret_cast<const uchar4*>(images)[px];
+        c = make_float4(u.x / 255.0f, u.y / 255.0f, u.z / 255.0f, u.w / 255.0f);
+    } else {
+        c = reinterpret_cast<const float4*>(images)[px];
+    }
+    const float ia = 1.0f - c.w;
+    target[3 * (size_t)i] = c.x * c.w + bg[3 * (size_t)i] * ia;
+    target[3 * (size_t)i + 1] = c.y * c.w + bg[3 * (size_t)i + 1] * ia;
+    target[3 * (size_t)i + 2] = c.z * c.w + bg[3 * (size_t)i + 2] * ia;
+}
+
 // target = rgb*a + bg*(1-a) (runner.py:68) for a ray batch that arrives with its RGBA already gathered (host-fed batches)
 __global__ void blend_target_kernel(uint32_t n, const float4* __restrict__ rgba, const float* __restrict__ bg, float* __restrict__ target) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -362,6 +430,14 @@ void launch_prepare_batch(cudaStream_t s, uint32_t n, const uint32_t* pix_index,
                                  uint32_t* img_id_out, float* rays_o, float* rays_d, float* target, const float4* lens) {
     if (image_is_u8) prepare_batch_kernel<uint8_t, LENS><<<(n + 127) / 128, 128, 0, s>>>(n, pix_index, W, H, xforms, focal, principal, (const uint8_t*)images_rgba, bg, img_id_out, rays_o, rays_d, target, lens);
     else prepare_batch_kernel<float, LENS><<<(n + 127) / 128, 128, 0, s>>>(n, pix_index, W, H, xforms, focal, principal, (const float*)images_rgba, bg, img_id_out, rays_o, rays_d, target, lens);
+}
+
+template <bool LENS>
+void launch_prepare_batch_cams(cudaStream_t s, uint32_t n, const uint32_t* pix_index, uint32_t n_images, const uint32_t* offsets, const uint2* wh,
+                               const float* xforms, const float* focal, const float* principal, const float4* lens, const void* images_rgba,
+                               int image_is_u8, const float* bg, uint32_t* img_id_out, float* rays_o, float* rays_d, float* target) {
+    if (image_is_u8) prepare_batch_cams_kernel<uint8_t, LENS><<<(n + 127) / 128, 128, 0, s>>>(n, pix_index, n_images, offsets, wh, xforms, focal, principal, lens, (const uint8_t*)images_rgba, bg, img_id_out, rays_o, rays_d, target);
+    else prepare_batch_cams_kernel<float, LENS><<<(n + 127) / 128, 128, 0, s>>>(n, pix_index, n_images, offsets, wh, xforms, focal, principal, lens, (const float*)images_rgba, bg, img_id_out, rays_o, rays_d, target);
 }
 
 }  // namespace
@@ -519,6 +595,40 @@ int ngp_raygen_lens(void* stream, uint32_t n, const uint32_t* pix_index, uint32_
                 "ngp_raygen_lens: distortion must be a 16-byte aligned (n_images, 4) float array");
     raygen_kernel<true><<<(n + 127) / 128, 128, 0, (cudaStream_t)stream>>>(n, pix_index, W, H, xforms, focal, principal, img_id_out, rays_o, rays_d,
                                                                            reinterpret_cast<const float4*>(distortion));
+    NGP_LAUNCH_CHECK();
+    return 0;
+}
+
+static int require_cams(const char* fn, uint32_t n_images, const uint32_t* pixel_offsets, const uint32_t* wh, const float* distortion) {
+    NGP_REQUIRE(n_images >= 1 && pixel_offsets != nullptr, std::string(fn) + ": needs n_images >= 1 and the (n_images + 1) pixel offsets");
+    NGP_REQUIRE(wh != nullptr && (reinterpret_cast<uintptr_t>(wh) & 7) == 0, std::string(fn) + ": wh must be an 8-byte aligned (n_images, 2) uint32 array");
+    NGP_REQUIRE((reinterpret_cast<uintptr_t>(distortion) & 15) == 0, std::string(fn) + ": distortion must be NULL or a 16-byte aligned (n_images, 4) float array");
+    return 0;
+}
+
+int ngp_raygen_cams(void* stream, uint32_t n, const uint32_t* pix_index, uint32_t n_images, const uint32_t* pixel_offsets, const uint32_t* wh,
+                    const float* xforms, const float* focal, const float* principal, const float* distortion, uint32_t* img_id_out, float* rays_o,
+                    float* rays_d) {
+    if (n == 0) return 0;
+    if (const int e = require_cams("ngp_raygen_cams", n_images, pixel_offsets, wh, distortion)) return e;
+    const uint2* wh2 = reinterpret_cast<const uint2*>(wh);
+    const float4* lens = reinterpret_cast<const float4*>(distortion);
+    if (lens) raygen_cams_kernel<true><<<(n + 127) / 128, 128, 0, (cudaStream_t)stream>>>(n, pix_index, n_images, pixel_offsets, wh2, xforms, focal, principal, lens, img_id_out, rays_o, rays_d);
+    else raygen_cams_kernel<false><<<(n + 127) / 128, 128, 0, (cudaStream_t)stream>>>(n, pix_index, n_images, pixel_offsets, wh2, xforms, focal, principal, nullptr, img_id_out, rays_o, rays_d);
+    NGP_LAUNCH_CHECK();
+    return 0;
+}
+
+int ngp_prepare_batch_cams(void* stream, uint32_t n, const uint32_t* pix_index, uint32_t n_images, const uint32_t* pixel_offsets, const uint32_t* wh,
+                           const float* xforms, const float* focal, const float* principal, const float* distortion, const void* images_rgba,
+                           int image_is_u8, const float* bg, uint32_t* img_id_out, float* rays_o, float* rays_d, float* target) {
+    if (n == 0) return 0;
+    if (const int e = require_cams("ngp_prepare_batch_cams", n_images, pixel_offsets, wh, distortion)) return e;
+    const uint2* wh2 = reinterpret_cast<const uint2*>(wh);
+    const float4* lens = reinterpret_cast<const float4*>(distortion);
+    cudaStream_t s = (cudaStream_t)stream;
+    if (lens) launch_prepare_batch_cams<true>(s, n, pix_index, n_images, pixel_offsets, wh2, xforms, focal, principal, lens, images_rgba, image_is_u8, bg, img_id_out, rays_o, rays_d, target);
+    else launch_prepare_batch_cams<false>(s, n, pix_index, n_images, pixel_offsets, wh2, xforms, focal, principal, nullptr, images_rgba, image_is_u8, bg, img_id_out, rays_o, rays_d, target);
     NGP_LAUNCH_CHECK();
     return 0;
 }

@@ -58,6 +58,17 @@ SRC = {
                     "out2_p));"),
     "prepare_batch_lens": ("NGP_OK(ngp_prepare_batch_lens(0, in0_shape0, (uint32_t*)in0_p, {W}, {H}, in1_p, in2_p, in3_p, in4_p, in5_p, 1, in6_p, "
                            "(uint32_t*)out0_p, out1_p, out2_p, out3_p));"),
+    # the same for captures whose frames carry their own cameras (INTEGRATION.md section 18): inputs pix, pixel offsets, wh, xforms, focal,
+    # principal, distortion (pinhole rays: use the _pinhole bodies, which pass nullptr), images, bg; and the occupancy grid's frustum test
+    "raygen_cams": ("NGP_OK(ngp_raygen_cams(0, in0_shape0, (uint32_t*)in0_p, in2_shape0, (uint32_t*)in1_p, (uint32_t*)in2_p, in3_p, in4_p, in5_p, "
+                    "in6_p, (uint32_t*)out0_p, out1_p, out2_p));"),
+    "raygen_cams_pinhole": ("NGP_OK(ngp_raygen_cams(0, in0_shape0, (uint32_t*)in0_p, in2_shape0, (uint32_t*)in1_p, (uint32_t*)in2_p, in3_p, in4_p, "
+                            "in5_p, nullptr, (uint32_t*)out0_p, out1_p, out2_p));"),
+    "prepare_batch_cams": ("NGP_OK(ngp_prepare_batch_cams(0, in0_shape0, (uint32_t*)in0_p, in2_shape0, (uint32_t*)in1_p, (uint32_t*)in2_p, in3_p, "
+                           "in4_p, in5_p, in6_p, in7_p, 1, in8_p, (uint32_t*)out0_p, out1_p, out2_p, out3_p));"),
+    "prepare_batch_cams_pinhole": ("NGP_OK(ngp_prepare_batch_cams(0, in0_shape0, (uint32_t*)in0_p, in2_shape0, (uint32_t*)in1_p, (uint32_t*)in2_p, "
+                                   "in3_p, in4_p, in5_p, nullptr, in6_p, 1, in7_p, (uint32_t*)out0_p, out1_p, out2_p, out3_p));"),
+    "grid_mark_untrained_cams": "NGP_OK(ngp_grid_mark_untrained_cams(0, out0_shape0, out0_p, in0_shape0, in0_p, in1_p));",
     # optims/adam.py + optims/ema.py in one sweep per parameter tensor
     "adam_ema": "NGP_OK(ngp_adam_ema(0, in0_shape0, in0_p, NGP_F16, in1_p, NGP_F16, 1.0f, in2_p, in3_p, in4_p, (float){lr}, 0.9f, 0.99f, 1e-15f, {step}, 0.95f, 1));",
     # contrib/plenoxel: volume_render_cuvol.py (forward, and forward + MSE + backward fused), tv_grad_sparse.py, optims/svox2_optim.py,
@@ -273,3 +284,20 @@ def prepare_batch_lens(pix, W, H, xforms, focal, principal, distortion, images_u
     n = pix.shape[0]
     return _code([(n,), (n, 3), (n, 3), (n, 3)], ["uint32", "float32", "float32", "float32"],
                  [pix, xforms, focal, principal, distortion, images_u8, bg], SRC["prepare_batch_lens"].format(W=int(W), H=int(H)))
+
+
+def raygen_cams(pix, pixel_offsets, wh, xforms, focal, principal, distortion=None):
+    """The rays of the global pixel ids pix (uint32) of a ragged capture whose image i is wh[i] = (w, h) pixels and owns the ids
+    [pixel_offsets[i], pixel_offsets[i+1]), through every image's lens when `distortion` (n_img, 4) is given: (img_ids, rays_o, rays_d)."""
+    n = pix.shape[0]
+    ins = [pix, pixel_offsets, wh, xforms, focal, principal] + ([] if distortion is None else [distortion])
+    return _code([(n,), (n, 3), (n, 3)], ["uint32", "float32", "float32"], ins, SRC["raygen_cams" if distortion is not None else "raygen_cams_pinhole"])
+
+
+def prepare_batch_cams(pix, pixel_offsets, wh, xforms, focal, principal, images_u8, bg, distortion=None):
+    """raygen_cams + the pixels' uint8 RGBA from the ragged (total_pixels, 4) table blended over bg (n, 3): (img_ids, rays_o, rays_d,
+    target)."""
+    n = pix.shape[0]
+    ins = [pix, pixel_offsets, wh, xforms, focal, principal] + ([] if distortion is None else [distortion]) + [images_u8, bg]
+    return _code([(n,), (n, 3), (n, 3), (n, 3)], ["uint32", "float32", "float32", "float32"], ins,
+                 SRC["prepare_batch_cams" if distortion is not None else "prepare_batch_cams_pinhole"])

@@ -86,6 +86,7 @@ SIGNATURES = {
     "ngp_composite_infer": (_i32, [_vp, _u32, _vp, _i32, _vp, _vp, _u32, _vp, _vp]),
     "ngp_composite_loss_bwd": (_i32, [_vp, _u32, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _f32, _vp, _u32, _vp, _vp, _vp, _f32]),
     "ngp_grid_mark_untrained": (_i32, [_vp, _u32, _vp, _u32, _vp, _vp, _i32, _i32]),
+    "ngp_grid_mark_untrained_cams": (_i32, [_vp, _u32, _vp, _u32, _vp, _vp]),
     "ngp_grid_generate_samples": (_i32, [_vp, _u32, _u64, _u64, _vp, _f32, _f32, _vp, _vp, _vp, _u32, _f32]),
     "ngp_grid_splat": (_i32, [_vp, _u32, _vp, _vp, _i32, _vp]),
     "ngp_grid_ema": (_i32, [_vp, _u32, _f32, _vp, _vp]),
@@ -103,6 +104,8 @@ SIGNATURES = {
     "ngp_prepare_batch": (_i32, [_vp, _u32, _vp, _u32, _u32, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp]),
     "ngp_raygen_lens": (_i32, [_vp, _u32, _vp, _u32, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "ngp_prepare_batch_lens": (_i32, [_vp, _u32, _vp, _u32, _u32, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp]),
+    "ngp_raygen_cams": (_i32, [_vp, _u32, _vp, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "ngp_prepare_batch_cams": (_i32, [_vp, _u32, _vp, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp]),
     "ngp_blend_target": (_i32, [_vp, _u32, _vp, _vp, _vp]),
     "ngp_pcg32_seed": (None, [_u64, _u64, _vp]),
     "ngp_pcg32_advance": (None, [_vp, _i64]),
@@ -114,7 +117,8 @@ KERNELS_PER_CALL = {
     "ngp_network_fwd": 1, "ngp_network_bwd": 1, "ngp_network_bwd_fx": 1, "ngp_train_sweep": 1, "ngp_density_fwd": 1, "ngp_march": 3, "ngp_compact": 1, "ngp_composite_fwd": 1,
     "ngp_composite_bwd": 1, "ngp_composite_infer": 1, "ngp_composite_loss_bwd": 1, "ngp_grid_mark_untrained": 1,
     "ngp_grid_generate_samples": 1, "ngp_grid_splat": 1, "ngp_grid_ema": 1, "ngp_grid_update_bitfield": 7, "ngp_adam_ema": 1, "ngp_dp_exchange_step": 1, "ngp_dp_exchange_wait": 1, "ngp_raygen": 1, "ngp_prepare_batch": 1,
-    "ngp_raygen_lens": 1, "ngp_prepare_batch_lens": 1, "ngp_blend_target": 1,
+    "ngp_raygen_lens": 1, "ngp_prepare_batch_lens": 1, "ngp_raygen_cams": 1, "ngp_prepare_batch_cams": 1,
+    "ngp_grid_mark_untrained_cams": 1, "ngp_blend_target": 1,
     "ngp_density_lattice": 1, "ngp_nerf_density_lattice": 1, "ngp_marching_cubes": 3, "ngp_mesh_largest_component": 18, "ngp_mesh_vertex_normals": 7,
     "ngp_render_init": 3, "ngp_render_march_round": 3, "ngp_render_composite_round": 3, "ngp_render_composite_round_depth": 3,
     "ngp_render_composite_round_normals": 3, "ngp_density_grad": 1,

@@ -638,6 +638,11 @@ def grid_mark_untrained(grid, focal, xforms, res):
     lib.call("ngp_grid_mark_untrained", _stream(), grid.numel(), _p(grid), xforms.shape[0], _p(focal), _p(xforms), int(res[0]), int(res[1]))
 
 
+def grid_mark_untrained_cams(grid, extents, xforms):
+    """grid_mark_untrained with every image's own signed normalised frustum extents (n_images, 4) = (x_lo, x_hi, y_lo, y_hi)."""
+    lib.call("ngp_grid_mark_untrained_cams", _stream(), grid.numel(), _p(grid), xforms.shape[0], _p(extents), _p(xforms))
+
+
 def grid_generate_samples(n, rng, step_dev, aabb, grid, n_cascades, thresh):
     pos = torch.empty((n, 3), dtype=torch.float32, device=grid.device)
     idx = torch.empty(n, dtype=torch.int32, device=grid.device)
@@ -690,6 +695,36 @@ def raygen(pix, W, H, xforms, focal, principal, distortion=None):
     else:
         lib.call("ngp_raygen_lens", _stream(), n, _p(pix), W, H, _p(xforms), _p(focal), _p(principal), _p(lens), _p(img), _p(o), _p(d))
     return img, o, d
+
+
+def raygen_cams(pix, pixel_offsets, wh, xforms, focal, principal, distortion=None):
+    """raygen for a capture whose frames carry their own cameras: pix are global pixel ids into the ragged table in which image i is
+    wh[i] = (w, h) pixels and owns [pixel_offsets[i], pixel_offsets[i+1]) (int32 device tensors); with a non-zero `distortion` (see
+    lens_of) every pixel is undistorted through its image's lens first."""
+    n = pix.numel()
+    dev = pix.device
+    img = torch.empty(n, dtype=torch.int32, device=dev)
+    o = torch.empty((n, 3), dtype=torch.float32, device=dev)
+    d = torch.empty((n, 3), dtype=torch.float32, device=dev)
+    lens = lens_of(distortion)
+    lib.call("ngp_raygen_cams", _stream(), n, _p(pix), wh.shape[0], _p(pixel_offsets), _p(wh), _p(xforms), _p(focal), _p(principal),
+             _p(lens), _p(img), _p(o), _p(d))
+    return img, o, d
+
+
+def prepare_batch_cams(pix, pixel_offsets, wh, xforms, focal, principal, images, bg, distortion=None):
+    """raygen_cams + the pixels' RGBA from the ragged (total_pixels, 4) table blended over bg in one launch: (img_ids, rays_o, rays_d,
+    target)."""
+    n = pix.numel()
+    dev = pix.device
+    img = torch.empty(n, dtype=torch.int32, device=dev)
+    o = torch.empty((n, 3), dtype=torch.float32, device=dev)
+    d = torch.empty((n, 3), dtype=torch.float32, device=dev)
+    target = torch.empty((n, 3), dtype=torch.float32, device=dev)
+    lens = lens_of(distortion)
+    lib.call("ngp_prepare_batch_cams", _stream(), n, _p(pix), wh.shape[0], _p(pixel_offsets), _p(wh), _p(xforms), _p(focal), _p(principal),
+             _p(lens), _p(images), int(images.dtype == torch.uint8), _p(bg), _p(img), _p(o), _p(d), _p(target))
+    return img, o, d, target
 
 
 def prepare_batch(pix, W, H, xforms, focal, principal, images, bg, distortion=None):

@@ -108,19 +108,76 @@ def check_lens(k, W, H, focal, c, n_angles=512, n_radii=2048):
                          "farthest corner); the ray kernels cannot invert it reliably")
 
 
-def lens_extent(k, W, H, focal, c):
-    """(max |x_u|, max |y_u|): the undistorted extent, in fp64, of the pixel centres and corners of a W x H image.  check_lens makes the
-    map one to one, so the extremes lie on the image's border: its corners and the centres of its outer pixels are solved."""
+def frame_extent(k, W, H, focal, c):
+    """(x_lo, x_hi, y_lo, y_hi): the signed extent, in fp64, of the undistorted normalised coordinates of the pixel centres and corners of
+    a W x H image with focal lengths `focal`, principal point `c` (pixels) and lens k (None or zeros: a pinhole camera, whose extent is
+    that of the image's corners).  check_lens makes the map one to one, so the extremes lie on the image's border: its corners and the
+    centres of its outer pixels are solved."""
+    if k is None or not any(k):
+        return (-c[0] / focal[0], (W - c[0]) / focal[0], -c[1] / focal[1], (H - c[1]) / focal[1])
     cu, cv = np.arange(W + 1.0), np.arange(H + 1.0)                                  # corners
     pu, pv = np.arange(W) + 0.5, np.arange(H) + 0.5                                  # centres
     bu = np.concatenate([cu, cu, np.zeros(H + 1), np.full(H + 1, float(W)), pu, pu, np.full(H, 0.5), np.full(H, W - 0.5)])
     bv = np.concatenate([np.zeros(W + 1), np.full(W + 1, float(H)), cv, cv, np.full(W, 0.5), np.full(W, H - 0.5), pv, pv])
     x, y = lens_undistort((bu - c[0]) / focal[0], (bv - c[1]) / focal[1], k)
-    return float(np.abs(x).max()), float(np.abs(y).max())
+    return float(x.min()), float(x.max()), float(y.min()), float(y.max())
+
+
+def lens_extent(k, W, H, focal, c):
+    """(max |x_u|, max |y_u|): the undistorted extent, in fp64, of the pixel centres and corners of a W x H image (frame_extent)."""
+    x_lo, x_hi, y_lo, y_hi = frame_extent(k, W, H, focal, c)
+    return max(-x_lo, x_hi), max(-y_lo, y_hi)
+
+
+CAMERA_KEYS = ("w", "h", "fl_x", "fl_y", "camera_angle_x", "camera_angle_y", "cx", "cy", "k1", "k2", "k3", "k4", "p1", "p2", "camera_model",
+               "is_fisheye")
+MAX_PIXELS = 2 ** 31 - 1               # the shuffle holds int32 pixel ids and the kernels uint32 offsets: a split may have at most this many
+
+
+def read_focal_lengths(cam, W, H):
+    """(fx, fy) of a camera dict by the rules of dataset.py:125-142 (fl_<axis>, else camera_angle_<axis> at that axis's resolution; one
+    axis stands in for the other), or None when it names neither."""
+    def axis(a, res):                                                                               # dataset.py:125-131
+        if "fl_" + a in cam:
+            return float(cam["fl_" + a])
+        if "camera_angle_" + a in cam:
+            return fov_to_focal_length(res, cam["camera_angle_" + a] * 180 / math.pi)
+        return 0.0
+    x_fl, y_fl = axis("x", W), axis("y", H)
+    if x_fl != 0:
+        return (x_fl, y_fl if y_fl != 0 else x_fl)
+    if y_fl != 0:
+        return (y_fl, y_fl)
+    return None
+
+
+def frame_camera(top, frame):
+    """The camera keys of one entry of `frames` over those of the json's top level: a key in the frame wins over the same key at the top
+    level.  A frame that names a focal length or field of view of an axis (fl_<axis> or camera_angle_<axis>) takes both keys of that axis
+    from itself, so that its own camera_angle_x is not overruled by a top-level fl_x."""
+    cam = {k: top[k] for k in CAMERA_KEYS if k in top}
+    for a in ("x", "y"):
+        if ("fl_" + a) in frame or ("camera_angle_" + a) in frame:
+            cam.pop("fl_" + a, None)
+            cam.pop("camera_angle_" + a, None)
+    cam.update({k: frame[k] for k in CAMERA_KEYS if k in frame})
+    return cam
 
 
 class _RayBatcher:
     """Pixel shuffling + device ray generation shared by both datasets (dataset.py:57-66,172-188)."""
+
+    def _set_cameras(self, cams):
+        """cams: every image's camera (W, H, fx, fy, cx, cy, lens), lens None or (k1, k2, p1, p2) for the rays.  When they are all one
+        camera the dataset is set up exactly as from a top-level camera; otherwise the frames keep their own (frame_cameras)."""
+        if all(c == cams[0] for c in cams):
+            self.W, self.H, fx, fy, self._cx, self._cy, lens = cams[0]
+            self._focal = (fx, fy)
+            if lens is not None:
+                self._lens = lens
+        else:
+            self._frames = list(cams)
+            self.W, self.H = cams[0][0], cams[0][1]
 
     def _finish_init(self):
         dev = DEVICE
@@ -128,32 +185,68 @@ class _RayBatcher:
         self.n_images = len(self._xforms)
         xf = np.stack(self._xforms).astype(np.float32)                       # (n,3,4)
         self.transforms_gpu = torch.from_numpy(np.ascontiguousarray(xf.transpose(0, 2, 1)).reshape(self.n_images, 12)).to(dev)
-        self.focal_lengths = torch.tensor([self._focal] * self.n_images, dtype=torch.float32, device=dev)
+        frames = getattr(self, "_frames", None)                              # per-frame cameras that differ, else None
+        self.frame_cameras = frames is not None
+        self._wh = np.array([c[:2] for c in frames] if frames else [(self.W, self.H)] * self.n_images, np.int64)
+        self._offsets = np.concatenate([[0], np.cumsum(self._wh[:, 0] * self._wh[:, 1])])
+        self.total_pixels = int(self._offsets[-1])
+        if frames and self.total_pixels > MAX_PIXELS:
+            raise ValueError(f"per_frame_cameras: the split has {self.total_pixels} pixels; its pixel ids are int32, so at most {MAX_PIXELS}")
+        self.resolutions = torch.from_numpy(self._wh.astype(np.int32)).to(dev)
+        self.pixel_offsets = torch.from_numpy(self._offsets.astype(np.int32) if self.total_pixels <= MAX_PIXELS else self._offsets).to(dev)
         md = np.zeros((self.n_images, 11), np.float32)
-        md[:, 4], md[:, 5] = self._cx / self.W, self._cy / self.H
-        md[:, 6], md[:, 7] = self._focal
-        lens = getattr(self, "_lens", None)                                  # (k1, k2, p1, p2) with undistort=True, else None
         self.distortion = None
-        if lens is not None:
-            md[:, 0:4] = lens                                                # the reference's slots (dataset.py:123-126)
-            self.distortion = torch.tensor([lens] * self.n_images, dtype=torch.float32, device=dev)
-            if any(lens):
-                # the occupancy grid's visibility frustum (grid_mark_untrained) is symmetric, |x| < (W/2) / f: with these focal lengths
-                # it holds every direction a pixel of the capture sees through the lens
-                ex, ey = lens_extent(lens, self.W, self.H, self._focal, (self._cx, self._cy))
-                self.focal_eff = torch.tensor([[self.W / 2 / ex, self.H / 2 / ey]] * self.n_images, dtype=torch.float32, device=dev)
+        if frames:
+            md[:, 4] = [c[4] / c[0] for c in frames]                         # the principal point of every frame by its own size
+            md[:, 5] = [c[5] / c[1] for c in frames]
+            md[:, 6], md[:, 7] = [c[2] for c in frames], [c[3] for c in frames]
+            self.focal_lengths = torch.from_numpy(md[:, 6:8].copy()).to(dev)
+            lenses = [c[6] for c in frames]
+            if lenses[0] is not None:
+                md[:, 0:4] = lenses
+                self.distortion = torch.from_numpy(md[:, 0:4].copy()).to(dev)
+            # the occupancy grid's visibility test (grid_mark_untrained_cams): every frame's signed frustum, rounded outwards to f32
+            ext = np.array([frame_extent(c[6], c[0], c[1], c[2:4], c[4:6]) for c in frames], np.float64)
+            e32 = ext.astype(np.float32)
+            lo = np.array([True, False, True, False])
+            e32 = np.where(lo & (e32 > ext), np.nextafter(e32, np.float32(-np.inf)), e32)
+            e32 = np.where(~lo & (e32 < ext), np.nextafter(e32, np.float32(np.inf)), e32)
+            self.frame_extents = torch.from_numpy(np.ascontiguousarray(e32, np.float32)).to(dev)
+        else:
+            self.focal_lengths = torch.tensor([self._focal] * self.n_images, dtype=torch.float32, device=dev)
+            md[:, 4], md[:, 5] = self._cx / self.W, self._cy / self.H
+            md[:, 6], md[:, 7] = self._focal
+            lens = getattr(self, "_lens", None)                              # (k1, k2, p1, p2) with undistort=True, else None
+            if lens is not None:
+                md[:, 0:4] = lens                                            # the reference's slots (dataset.py:123-126)
+                self.distortion = torch.tensor([lens] * self.n_images, dtype=torch.float32, device=dev)
+                if any(lens):
+                    # the occupancy grid's visibility frustum (grid_mark_untrained) is symmetric, |x| < (W/2) / f: with these focal lengths
+                    # it holds every direction a pixel of the capture sees through the lens
+                    ex, ey = lens_extent(lens, self.W, self.H, self._focal, (self._cx, self._cy))
+                    self.focal_eff = torch.tensor([[self.W / 2 / ex, self.H / 2 / ey]] * self.n_images, dtype=torch.float32, device=dev)
         self.metadata = torch.from_numpy(md).to(dev)
         self.principal = self.metadata[:, 4:6].contiguous()
         self.aabb_range = (0.5 - self.aabb_scale / 2, 0.5 + self.aabb_scale / 2)    # dataset.py:155-156
         self.idx_now = 0
         self._gen = torch.Generator(device=dev).manual_seed(int(self.seed))
-        self.shuffle_index = torch.randperm(self.n_images * self.H * self.W, device=dev, generator=self._gen).int()
+        self.shuffle_index = torch.randperm(self.total_pixels, device=dev, generator=self._gen).int()
+
+    def image_resolution(self, img_id):
+        """(W, H) of image img_id."""
+        w, h = self._wh[int(img_id)]
+        return int(w), int(h)
+
+    def image_pixels(self, img_id):
+        """The global pixel ids of image img_id, row-major (int32): its rows of image_data.reshape(-1, 4)."""
+        w, h = self.image_resolution(img_id)
+        return torch.arange(w * h, device=DEVICE, dtype=torch.int32) + int(self._offsets[int(img_id)])
 
     def next_pixels(self, n=None):
         """The next n entries of the shuffled pixel list; the list is reshuffled in place when it runs out."""
         n = self.batch_size if n is None else n
         if self.idx_now + n >= self.shuffle_index.shape[0]:
-            self.shuffle_index.copy_(torch.randperm(self.n_images * self.H * self.W, device=DEVICE, generator=self._gen).int())
+            self.shuffle_index.copy_(torch.randperm(self.total_pixels, device=DEVICE, generator=self._gen).int())
             self.idx_now = 0
         start = self.idx_now
         self.idx_now += n
@@ -163,6 +256,9 @@ class _RayBatcher:
         """(img_ids, rays_o, rays_d) of the flat pixel indices pix, through the dataset's lens (or `distortion`) when it has one."""
         distortion = self.distortion if distortion is None else distortion
         lens = {} if distortion is None else dict(distortion=distortion)
+        if self.frame_cameras:
+            return ops.raygen_cams(pix.contiguous(), self.pixel_offsets, self.resolutions, self.transforms_gpu, self.focal_lengths, self.principal,
+                                   **lens)
         return ops.raygen(pix.contiguous(), self.W, self.H, self.transforms_gpu, self.focal_lengths, self.principal, **lens)
 
     def rgba_for(self, pix):
@@ -176,17 +272,20 @@ class _RayBatcher:
 
     def generate_rays_total_test(self, img_id):
         """All rays of one image in row-major pixel order (dataset.py:214-238)."""
-        pix = torch.arange(self.H * self.W, device=DEVICE, dtype=torch.int32) + int(img_id) * self.H * self.W
-        _, o, d = self.rays_for(pix)
+        _, o, d = self.rays_for(self.image_pixels(img_id))
         return o, d
 
 
 @DATASETS.register_module()
 class NerfDataset(_RayBatcher):
     def __init__(self, root_dir, batch_size, mode="train", H=0, W=0, correct_pose=(1, -1, -1), aabb_scale=None, scale=None, offset=None,
-                 img_alpha=True, to_jt=True, have_img=True, preload_shuffle=True, seed=0, undistort=False):
+                 img_alpha=True, to_jt=True, have_img=True, preload_shuffle=True, seed=0, undistort=False, per_frame_cameras=False):
         """undistort: read k1, k2, p1, p2 from the split's json and make every ray of its images through that lens (check_lens); off,
-        as in the reference, every ray is a pinhole ray."""
+        as in the reference, every ray is a pinhole ray.
+        per_frame_cameras: every entry of `frames` may carry its own w, h, fl_x, fl_y, camera_angle_x / _y, cx, cy (and, with undistort,
+        lens), over the json's top level (frame_camera); images of different sizes are kept in one ragged (total_pixels, 4) table.  When
+        the frames resolve to one camera the dataset is the one the top-level keys give.  Off, as in the reference, frame keys are
+        ignored."""
         from PIL import Image
         assert mode in ("train", "val", "test")
         self.root_dir, self.batch_size, self.mode, self.seed = root_dir, batch_size, mode, seed
@@ -208,6 +307,7 @@ class NerfDataset(_RayBatcher):
         frames = json_data["frames"][::10] if mode == "val" else json_data["frames"]
         imgs, self._xforms, self.poses = [], [], []
         self.correct_pose = tuple(correct_pose)
+        cams = []
         for fr in frames:
             p = os.path.join(root_dir, fr["file_path"])
             if not os.path.exists(p):
@@ -221,30 +321,54 @@ class NerfDataset(_RayBatcher):
                 im = np.concatenate([im, np.full(im.shape[:2] + (1,), 255, np.uint8)], -1)
             if self.H == 0 or self.W == 0:
                 self.H, self.W = im.shape[0], im.shape[1]
+            if per_frame_cameras:
+                cams.append(self._frame_camera(json_data, fr, im, W, H, undistort))
             imgs.append(im)
             self.poses.append(np.array(fr["transform_matrix"], np.float32))                           # NeRF camera-to-world, as in the file
             self._xforms.append(matrix_nerf2ngp(fr["transform_matrix"], self.scale, self.offset, correct_pose))
+        self.aabb_scale = json_data.get("aabb_scale", 1) if aabb_scale is None else aabb_scale
+        self.have_img = have_img
+        if per_frame_cameras:
+            self._set_cameras(cams)
+            if hasattr(self, "_frames"):
+                self.image_data = torch.from_numpy(np.concatenate([im.reshape(-1, 4) for im in imgs])).to(DEVICE)
+            else:
+                self.image_data = torch.from_numpy(np.stack(imgs)).to(DEVICE).reshape(len(imgs), -1, 4)
+            self._finish_init()
+            return
         self.image_data = torch.from_numpy(np.stack(imgs)).to(DEVICE).reshape(len(imgs), -1, 4)
-        def read_focal_length(resolution, axis):                                                   # dataset.py:125-131
-            if "fl_" + axis in json_data:
-                return float(json_data["fl_" + axis])
-            if "camera_angle_" + axis in json_data:
-                return fov_to_focal_length(resolution, json_data["camera_angle_" + axis] * 180 / math.pi)
-            return 0.0
-        x_fl, y_fl = read_focal_length(self.W, "x"), read_focal_length(self.H, "y")
-        if x_fl != 0:                                                                               # :134-142
-            self._focal = (x_fl, y_fl if y_fl != 0 else x_fl)
-        elif y_fl != 0:
-            self._focal = (y_fl, y_fl)
-        else:
+        self._focal = read_focal_lengths(json_data, self.W, self.H)
+        if self._focal is None:
             raise RuntimeError("Couldn't read fov.")
         self._cx, self._cy = json_data.get("cx", self.W / 2), json_data.get("cy", self.H / 2)
         if undistort:
             self._lens = read_lens(json_data)
             check_lens(self._lens, self.W, self.H, self._focal, (self._cx, self._cy))
-        self.aabb_scale = json_data.get("aabb_scale", 1) if aabb_scale is None else aabb_scale
-        self.have_img = have_img
         self._finish_init()
+
+    @staticmethod
+    def _frame_camera(json_data, fr, im, W, H, undistort):
+        """(W, H, fx, fy, cx, cy, lens) of one frame (frame_camera); lens is None unless undistort.  The refusals of the lens apply to
+        every frame at its own size, and a frame without a resolvable focal length raises."""
+        name = fr.get("file_path")
+        cam = frame_camera(json_data, fr)
+        w = int(cam["w"]) if "w" in cam else (int(W) or im.shape[1])
+        h = int(cam["h"]) if "h" in cam else (int(H) or im.shape[0])
+        if im.shape[:2] != (h, w):
+            raise ValueError(f"per_frame_cameras: frame {name!r} is {im.shape[1]}x{im.shape[0]} pixels but its camera is {w}x{h}")
+        f = read_focal_lengths(cam, w, h)
+        if f is None:
+            raise RuntimeError(f"Couldn't read fov of frame {name!r}: neither it nor the json's top level has fl_x, fl_y, camera_angle_x "
+                               "or camera_angle_y")
+        c = (cam.get("cx", w / 2), cam.get("cy", h / 2))
+        lens = None
+        if undistort:
+            try:
+                lens = read_lens(cam)
+                check_lens(lens, w, h, f, c)
+            except (NotImplementedError, ValueError) as e:
+                raise type(e)(f"frame {name!r}: {e}") from e
+        return (w, h, f[0], f[1], c[0], c[1], lens)
 
 
 def _normalize(x):
@@ -395,6 +519,35 @@ def write_synthetic_llff(dst, n_images=20, H=378, W=504, factor=None, seed=0, ra
     return np.stack(mats)
 
 
+def write_synthetic_frames(dst, cameras, n_images=20, seed=0, style="lego", lens_keys=True):
+    """A capture whose frames carry their own cameras, on disk in the Instant-NGP layout NerfDataset(per_frame_cameras=True) reads:
+    dst/{train,test}/r_{i}.png (RGBA, each at its own size) and dst/transforms_{train,test}.json whose top level holds only aabb_scale
+    and whose every frame holds its transform_matrix, w, h, fl_x, fl_y, cx, cy (and k1, k2, p1, p2 for a camera with a lens, unless
+    lens_keys is False).  The images are SyntheticNerfDataset(cameras=cameras, ...)'s, so the two datasets describe one scene; the test
+    split has n_images // 10 views.  Returns {split: that SyntheticNerfDataset}."""
+    from PIL import Image
+    out = {}
+    for split in ("train", "test"):
+        ds = SyntheticNerfDataset(batch_size=1, mode=split, n_images=n_images, seed=seed, style=style, cameras=cameras)
+        os.makedirs(os.path.join(dst, split), exist_ok=True)
+        table = ds.image_data.reshape(-1, 4).cpu().numpy()
+        frames = []
+        for i in range(ds.n_images):
+            c = tuple(cameras[i % len(cameras)])
+            w, h = ds.image_resolution(i)
+            lo, hi = int(ds._offsets[i]), int(ds._offsets[i + 1])
+            Image.fromarray(table[lo:hi].reshape(h, w, 4), "RGBA").save(os.path.join(dst, split, f"r_{i}.png"))
+            fr = dict(file_path=f"./{split}/r_{i}", transform_matrix=np.asarray(ds.poses[i], np.float64).tolist(), w=w, h=h,
+                      fl_x=float(c[2]), fl_y=float(c[3]), cx=float(c[4]), cy=float(c[5]))
+            if lens_keys and len(c) > 6 and c[6] is not None:
+                fr.update(zip(LENS_KEYS, (float(v) for v in c[6])))
+            frames.append(fr)
+        with open(os.path.join(dst, f"transforms_{split}.json"), "w") as fh:
+            json.dump(dict(aabb_scale=ds.aabb_scale, frames=frames), fh)
+        out[split] = ds
+    return out
+
+
 def synthetic_cameras(n_images, radius=4.0, seed=0, azimuth=(0.0, 360.0), elevation=(5.0, 85.0)):
     """Camera-to-world matrices (NeRF/blender convention, looking at the origin) on a sphere of `radius`,
     upper hemisphere like NeRF-synthetic (cf. dataset/camera_path.py:27-28 which also uses radius 4); `azimuth` / `elevation`
@@ -437,9 +590,12 @@ class SyntheticNerfDataset(_RayBatcher):
                elevation=(-8.0, 30.0), obj_scale=2.2, backdrop_radius=1.9)
 
     def __init__(self, batch_size=4096, mode="train", n_images=100, H=800, W=800, camera_angle_x=0.6911112070083618, aabb_scale=1, seed=0,
-                 root_dir=None, preload_shuffle=True, style="lego", distortion=None, undistort=False):
+                 root_dir=None, preload_shuffle=True, style="lego", distortion=None, undistort=False, cameras=None):
         """distortion: (k1, k2, p1, p2) of the lens the images are taken through (None: a pinhole camera); undistort: make the rays
-        through that lens, as NerfDataset(undistort=True) does with a capture's json."""
+        through that lens, as NerfDataset(undistort=True) does with a capture's json.
+        cameras: per-frame cameras (W, H, fx, fy, cx, cy[, lens]), image i taken with cameras[i % len(cameras)] (its lens, if given, in
+        place of `distortion`), as NerfDataset(per_frame_cameras=True) reads a capture whose frames carry their own cameras; H, W and
+        camera_angle_x are then unused."""
         assert style in ("lego", "fox")
         self.batch_size, self.mode, self.seed, self.style = batch_size, mode, seed, style
         self.scale, self.offset = NERF_SCALE, [0.5, 0.5, 0.5]
@@ -469,6 +625,20 @@ class SyntheticNerfDataset(_RayBatcher):
         self._xforms = [matrix_nerf2ngp(m, self.scale, self.offset) for m in mats]
         self.have_img = True
         capture = None if distortion is None else tuple(float(v) for v in distortion)
+        if cameras is not None:
+            cams, capture = [], []
+            for i in range(n):
+                c = tuple(cameras[i % len(cameras)])
+                w, h, fx, fy, cx, cy = int(c[0]), int(c[1]), float(c[2]), float(c[3]), float(c[4]), float(c[5])
+                k = tuple(float(v) for v in c[6]) if len(c) > 6 and c[6] is not None else None
+                if k is not None:
+                    check_lens(k, w, h, (fx, fy), (cx, cy))
+                capture.append(k or (0.0, 0.0, 0.0, 0.0))
+                cams.append((w, h, fx, fy, cx, cy, (k or (0.0, 0.0, 0.0, 0.0)) if undistort else None))
+            self._set_cameras(cams)
+            self._finish_init()
+            self.image_data = self._render_all(capture if any(any(k) for k in capture) else None)
+            return
         if capture is not None:
             check_lens(capture, self.W, self.H, self._focal, (self._cx, self._cy))
         if undistort:
@@ -482,16 +652,21 @@ class SyntheticNerfDataset(_RayBatcher):
         return p[[1, 2, 0]]
 
     def _render_all(self, lens=None):
-        """The images, every pixel's ray through `lens` (k1, k2, p1, p2) when one is given, whatever rays the dataset trains on."""
-        out = torch.empty((self.n_images, self.H * self.W, 4), dtype=torch.uint8, device=DEVICE)
-        lens = None if lens is None or not any(lens) else torch.tensor([lens] * self.n_images, dtype=torch.float32, device=DEVICE)
+        """The images, every pixel's ray through `lens` (k1, k2, p1, p2, or one such lens per image) when one is given, whatever rays the
+        dataset trains on: (n, H*W, 4), or the ragged (total_pixels, 4) table when the frames' cameras differ."""
+        out = torch.empty((self.total_pixels, 4), dtype=torch.uint8, device=DEVICE)
+        if lens is not None and any(np.ravel(lens)):
+            lens = torch.from_numpy(np.array(np.broadcast_to(np.asarray(lens, np.float32), (self.n_images, 4)), order="C")).to(DEVICE)
+        else:
+            lens = None
         for i in range(self.n_images):
+            pix = self.image_pixels(i)
             if lens is None:
                 o, d = self.generate_rays_total_test(i)
             else:
-                _, o, d = self.rays_for(torch.arange(self.H * self.W, device=DEVICE, dtype=torch.int32) + i * self.H * self.W, lens)
-            out[i] = (self.shade(o, d) * 255.0 + 0.5).clamp(0, 255).to(torch.uint8)
-        return out
+                _, o, d = self.rays_for(pix, lens)
+            out[pix.long()] = (self.shade(o, d) * 255.0 + 0.5).clamp(0, 255).to(torch.uint8)
+        return out if self.frame_cameras else out.reshape(self.n_images, self.H * self.W, 4)
 
     def shade(self, o, d, return_t=False, return_normal=False):
         """RGBA in [0,1] of the analytic scene along rays (o,d) given in NGP coordinates; with `return_t` also the distance to the

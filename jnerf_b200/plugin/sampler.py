@@ -165,10 +165,14 @@ class DensityGridSampler(Module):
     def update_density_grid_nerf(self, decay, n_uniform, n_nonuniform):
         if self.cfg.m_training_step == 0:
             self.density_grid.zero_()
-            # through a lens the images see further out than a pinhole of the same focal length: the dataset's effective focal lengths
-            focal = getattr(self.dataset, "focal_eff", None)
-            ops.grid_mark_untrained(self.density_grid, self.dataset.focal_lengths if focal is None else focal, self.dataset.transforms_gpu,
-                                    self.image_resolutions)
+            if getattr(self.dataset, "frame_cameras", False):
+                # frames with their own cameras: every image's own signed frustum, whatever its size, principal point and lens
+                ops.grid_mark_untrained_cams(self.density_grid, self.dataset.frame_extents, self.dataset.transforms_gpu)
+            else:
+                # through a lens the images see further out than a pinhole of the same focal length: the dataset's effective focal lengths
+                focal = getattr(self.dataset, "focal_eff", None)
+                ops.grid_mark_untrained(self.density_grid, self.dataset.focal_lengths if focal is None else focal, self.dataset.transforms_gpu,
+                                        self.image_resolutions)
         self.density_grid_tmp.zero_()
         parts_p, parts_i = [], []
         for n, thresh in ((n_uniform, -0.01), (n_nonuniform, self.NERF_MIN_OPTICAL_THICKNESS)):

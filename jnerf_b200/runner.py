@@ -228,6 +228,11 @@ class Runner:
                 pix, bg = pix[lo:hi], bg[lo:hi]
             bg = bg.contiguous()
             lens = getattr(ds, "distortion", None)                       # every rank the same lens
+            if getattr(ds, "frame_cameras", False):                      # frames with their own cameras: the ragged global pixel ids
+                img_ids, rays_o, rays_d, target = ops.prepare_batch_cams(pix.contiguous(), ds.pixel_offsets, ds.resolutions, ds.transforms_gpu,
+                                                                         ds.focal_lengths, ds.principal, ds.image_data, bg,
+                                                                         **({} if lens is None else dict(distortion=lens)))
+                return img_ids, rays_o, rays_d, bg, target
             img_ids, rays_o, rays_d, target = ops.prepare_batch(pix.contiguous(), ds.W, ds.H, ds.transforms_gpu, ds.focal_lengths,
                                                                 ds.principal, ds.image_data, bg,
                                                                 **({} if lens is None else dict(distortion=lens)))  # dataset.py:172-188 + runner.py:68
@@ -504,7 +509,7 @@ class Runner:
         self._table_ready()
         self._sync_front()
         ds = self.dataset[dataset_mode]
-        W, H = ds.resolution
+        W, H = image_resolution(ds, img_id)
         rays_o, rays_d = ds.generate_rays_total_test(img_id)
         tile = self.cfg.n_rays_per_batch
         img = torch.empty((H * W, 3), device="cuda")
@@ -532,9 +537,10 @@ class Runner:
 
     def _target_img(self, ds, img_id):
         """Image img_id of split ds as (H, W, 3), with the background colour blended in (runner.py:68)."""
-        W, H = ds.resolution
+        W, H = image_resolution(ds, img_id)
         bgc = torch.tensor(self.background_color, dtype=torch.float32, device="cuda")
-        tar = ds.rgba_for(torch.arange(H * W, device="cuda", dtype=torch.int32) + int(img_id) * H * W)
+        pix = ds.image_pixels(img_id) if hasattr(ds, "image_pixels") else torch.arange(H * W, device="cuda", dtype=torch.int32) + int(img_id) * H * W
+        tar = ds.rgba_for(pix)
         return (tar[:, :3] * tar[:, 3:] + bgc * (1 - tar[:, 3:])).reshape(H, W, 3)
 
     def _infer_tiles(self, rays_o, rays_d):
@@ -576,7 +582,7 @@ class Runner:
         self._table_ready()
         self._sync_front()
         ds = self.dataset[dataset_mode]
-        W, H = ds.resolution
+        W, H = image_resolution(ds, img_id)
         rays_o, rays_d = ds.generate_rays_total_test(img_id)
         tile = self.cfg.n_rays_per_batch
         n_pix = H * W
@@ -642,7 +648,8 @@ class Runner:
 
     def pose_rays(self, pose):
         """generate_rays_with_pose (dataset.py:236-253): the rays of every pixel, row-major, of a camera at `pose` (3x4 or 4x4 NeRF
-        camera-to-world) with the train split's image-0 intrinsics and its true [W, H] (DESIGN.md section 7)."""
+        camera-to-world) with the train split's image-0 intrinsics and its true [W, H] (DESIGN.md section 7).  The rays are pinhole rays
+        and, for a capture whose frames carry their own cameras, take train image 0's camera."""
         from .plugin.dataset import matrix_nerf2ngp
         ds = self.dataset["train"]
         W, H = ds.resolution
@@ -656,7 +663,7 @@ class Runner:
     @torch.no_grad()
     def render_img_with_pose(self, pose, min_transmittance=1e-4):
         """runner.py:238-264 on the whole-frame renderer: the (H, W, 3) image of a camera at `pose`, background blended in unless
-        alpha_image is set."""
+        alpha_image is set; train image 0's camera, pinhole (pose_rays)."""
         W, H = self.dataset["train"].resolution
         o, d = self.pose_rays(pose)
         return self._render_frame(o, d, W, H, min_transmittance)[0]
@@ -717,7 +724,8 @@ class Runner:
         clip((far - depth) / (far - near), 0, 1) with one (near, far) for the whole video, depth_range(poses): nearer is brighter and a
         shade is the same distance in every frame; empty pixels are black.
         normals: also write the normal video of the same frames ({stem}_normal.mp4), RGB = alpha * (n + 1) / 2 of the NeRF-axes normal
-        (normal_to_rgb).  Fused NGP model only."""
+        (normal_to_rgb).  Fused NGP model only.
+        Every frame takes train image 0's camera, pinhole (pose_rays), also for captures whose frames carry their own cameras."""
         if normals and not self.fast:
             raise NotImplementedError("normal maps need the gradient of the fused NGP density network; this model has none")
         try:
@@ -772,17 +780,18 @@ class Runner:
         depth: with save_img also {exp_name}_depth_{i}.npy (float32 (H,W), NeRF world units, depth_from_sum) and {exp_name}_depth_{i}.png
         (8-bit grey, nearer is brighter, one depth_range over the test views, as in render's depth video), from the same render.
         normals: with save_img also {exp_name}_normal_{i}.npy (float32 (H,W,3), unit NeRF-axes normals, normal_from_sum) and
-        {exp_name}_normal_{i}.png (RGB = alpha * (n + 1) / 2, normal_to_rgb), from the same render.  Fused NGP model only."""
+        {exp_name}_normal_{i}.png (RGB = alpha * (n + 1) / 2, normal_to_rgb), from the same render.  Fused NGP model only.
+        Every view is rendered and compared at its own size, through its own camera (image_resolution)."""
         ds = self.dataset["test"]
         save_path = self._save_path() if save_path is None else save_path
         if save_img:
             os.makedirs(save_path, exist_ok=True)
         exp = self.cfg.exp_name
-        W, H = ds.resolution
         have_img = getattr(ds, "have_img", True)
         near, far = self.depth_range(ds.poses, ds) if depth else (0.0, 0.0)
         mse = []
         for i in range(ds.n_images):
+            W, H = image_resolution(ds, i)                            # every view at its own size
             o, d = ds.generate_rays_total_test(i)
             frame = self._render_frame(o, d, W, H, min_transmittance, depth_scale=float(ds.scale) if depth else None, normals=normals)
             img, alpha = frame[0], frame[1]
@@ -899,7 +908,7 @@ class Runner:
 
     @torch.no_grad()
     def psnr(self, dataset_mode="val", max_images=None):
-        """mean over images of -10 log10(mse) (runner.py:86-99, mse_loss.py:6-7)."""
+        """mean over images of -10 log10(mse) (runner.py:86-99, mse_loss.py:6-7), every image at its own size."""
         ds = self.dataset[dataset_mode]
         n = ds.n_images if max_images is None else min(max_images, ds.n_images)
         tot = 0.0
@@ -983,6 +992,11 @@ class Runner:
             self._slice_param.copy_(self._table[self._lo:self._hi])
         self.optimizer._nested_optimizer.load_state_dict(nested)
         self.ema_optimizer.load_state_dict(ck["ema_optimizer"])
+
+
+def image_resolution(ds, img_id):
+    """(W, H) of image img_id of dataset ds: its own size for a capture whose frames carry their own cameras, else ds.resolution."""
+    return ds.image_resolution(img_id) if hasattr(ds, "image_resolution") else tuple(ds.resolution)
 
 
 def depth_from_sum(S, alpha, scale):

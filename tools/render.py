@@ -91,7 +91,7 @@ def main():
     import torch
     from jnerf_b200 import lib, plugin  # noqa: F401
     from jnerf_b200.plugin import losses as L
-    from jnerf_b200.runner import Runner, fox_cfg, lego_cfg, llff_cfg
+    from jnerf_b200.runner import Runner, fox_cfg, image_resolution, lego_cfg, llff_cfg
     from jnerf_b200.utils.config import get_cfg, init_cfg, update_cfg
     from jnerf_b200.utils.registry import DATASETS, build_from_cfg
 
@@ -178,8 +178,10 @@ def main():
                 return img, tar, None
             if mode == "train":
                 o, d = runner.pose_rays(ds.poses[i])
+                W, H = ds.resolution
             else:
                 o, d = ds.generate_rays_total_test(i)
+                W, H = image_resolution(ds, i)                       # every test view at its own size
             if kind == "depth":
                 img, alpha, n, rounds, dep = runner._render_frame(o, d, W, H, m, depth_scale=float(ds.scale))
             elif kind == "normal":
@@ -187,7 +189,8 @@ def main():
             else:
                 img, alpha, n, rounds = runner._render_frame(o, d, W, H, m)
                 dep = None
-            tar = ds.rgba_for(torch.arange(H * W, device="cuda", dtype=torch.int32) + i * H * W)
+            pix = ds.image_pixels(i) if hasattr(ds, "image_pixels") else torch.arange(H * W, device="cuda", dtype=torch.int32) + i * H * W
+            tar = ds.rgba_for(pix)
             tar = (tar[:, :3] * tar[:, 3:] + bgc * (1 - tar[:, 3:])).reshape(H, W, 3)
             return img, tar, (n, rounds, dep, alpha)
 

@@ -4,6 +4,7 @@
     python tools/train_psnr.py [--steps 5000] [--images 100] [--res 400] [--evals 500,1000,2000,5000] [--out gpurun_out/psnr.json]
     python tools/train_psnr.py --workload llff [--data-dir CAPTURE] [--images 40]
     python tools/train_psnr.py --workload fox [--data-dir CAPTURE] [--undistort] [--distortion K1 K2 P1 P2]
+    python tools/train_psnr.py --workload frames [--data-dir CAPTURE] [--res 400] [--images 100]
 
 This is the quality check that goes with bench.py's throughput number: same Runner.train_step path, same configuration
 (projects/ngp/configs/ngp_base.py + fp16), validation views drawn from cameras the model never trains on
@@ -29,10 +30,13 @@ def main():
                     help="BASELINE metric 'PSNR@5min': keep training after --steps until this much device time has been spent on training "
                          "steps or the configuration's tot_train_steps (40 000, ngp_base.py) is reached, then evaluate once more")
     ap.add_argument("--data-dir", default=None, help="a real capture in the reference's dataset layout (train/val splits) instead of the stand-in")
-    ap.add_argument("--workload", default="lego", choices=["lego", "fox", "llff"],
+    ap.add_argument("--workload", default="lego", choices=["lego", "fox", "llff", "frames"],
                     help="fox = projects/ngp/configs/ngp_fox.py (aabb_scale from the capture, cone stepping); PSNR on training views (the capture has no val split). "
                          "llff = projects/ngp/configs/ngp_llff.py (aabb_scale 64: 7 occupancy cascades, every 8th view held out) on --data-dir, an LLFF "
-                         "capture (poses_bounds.npy + images/), or on the forward-facing stand-in written to a temporary directory")
+                         "capture (poses_bounds.npy + images/), or on the forward-facing stand-in written to a temporary directory. "
+                         "frames = ngp_base.py on a capture whose frames carry their own cameras (NerfDataset(per_frame_cameras=True)): --data-dir, or "
+                         "the lego stand-in written to a temporary directory with frames cycling through a res x res camera, a 1.2 res x 0.8 res one "
+                         "and a zoomed 0.8 res x 1.2 res one with an off-centre principal point; PSNR on the test split")
     ap.add_argument("--undistort", action="store_true", help="fox: train and evaluate through the capture's lens (datasets' undistort=True)")
     ap.add_argument("--distortion", type=float, nargs=4, default=None, metavar=("K1", "K2", "P1", "P2"),
                     help="fox stand-in: take its images through this lens (k1 k2 p1 p2)")
@@ -60,6 +64,23 @@ def main():
             write_synthetic_llff(root, n_images=args.images, H=8 * 192, W=8 * 256)    # read at 192 x 256 (factor 8); the fern capture is read at 378 x 504
         update_cfg(**llff_cfg(root, fp16=True, seed=1))
         cfg = get_cfg()
+    elif args.workload == "frames":
+        root = args.data_dir
+        if root is None:
+            import tempfile
+            from jnerf_b200.plugin.dataset import write_synthetic_frames
+            tmp = tempfile.TemporaryDirectory()
+            root = tmp.name
+            r = args.res
+            f = 0.5 * r / 0.36                                          # the stand-in's field of view (camera_angle_x 0.6911)
+            cams = [(r, r, f, f, r / 2, r / 2), (int(1.2 * r), int(0.8 * r), f, f, 0.6 * r, 0.4 * r),
+                    (int(0.8 * r), int(1.2 * r), 1.5 * f, 1.5 * f, 0.28 * r, 0.75 * r)]
+            write_synthetic_frames(root, cams, n_images=args.images)
+        update_cfg(**lego_cfg(fp16=True, synthetic=False, seed=1))
+        cfg = get_cfg()
+        for split in ("train", "val", "test"):
+            cfg.dataset[split].update(root_dir=root, per_frame_cameras=True, mode="test" if split == "val" else split)
+        cfg.dataset.test = None
     elif args.workload == "fox":
         update_cfg(**fox_cfg(fp16=True, synthetic=args.data_dir is None, undistort=args.undistort, seed=1))
         cfg = get_cfg()
@@ -108,6 +129,10 @@ def main():
         res["config"] = (f"ngp_fox.py (fp16, cone stepping) on {args.data_dir or 'the synthetic fox stand-in'}, PSNR on {args.val_images} training views "
                          f"(the capture has no validation split)" + (f", images through the lens {args.distortion}" if args.distortion else "")
                          + (", rays undistorted" if args.undistort else ""))
+    if args.workload == "frames":
+        res["config"] = (f"ngp_base + fp16 on {args.data_dir or 'the per-frame-camera lego stand-in'}, per_frame_cameras=True: "
+                         f"{runner.dataset['train'].n_images} training views of {sorted({runner.dataset['train'].image_resolution(i) for i in range(runner.dataset['train'].n_images)})}, "
+                         f"PSNR on {args.val_images} held-out views")
     if args.workload == "llff":
         res["config"] = (f"ngp_llff.py (fp16, cone stepping, aabb_scale 64) on {args.data_dir or 'the forward-facing stand-in'}: "
                          f"{runner.dataset['train'].n_images} training views of {runner.W}x{runner.H}, PSNR on {args.val_images} held-out views")
